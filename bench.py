@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""bench.py — measurement of the two BPE hot paths on B200 (contract: task statement ④; BASELINE.json metric
-"GB/s BPE-train scan + Msent/s encode at 1/2/4/8 B200 vs ref CPU n_threads").
+"""bench.py — measurement of the two BPE hot paths on H100 (BASELINE.json metric: GB/s BPE-train scan + Msent/s encode
+at 1/2/4/8 GPUs vs the reference's CPU n_threads).
 
 The JSON line's `value` / `e2e` are hot path (b), BASELINE configs[1]: batch encode_as_ids of 1 M synthetic 128-byte
 sentences, vocab 32 000 (one "step" = one pass over the batch; the model is trained by this framework's own GPU
@@ -21,6 +21,8 @@ Hot path (a), training, travels in keys the driver keeps (`config.train`, `roofl
   cpu_baseline           the unmodified reference (oracle/_ref prod build) on the host: encode_as_ids with 1 / 8 / all
                          threads, train_bpe with 8 threads (its cap) on the 1 GB corpus and 1 thread on a 125 MB chunk
 `--impl reference` times the reference's own CPU encode_as_ids (all host threads) on the same workload.
+`--dump-outputs DIR` writes what the last timed step computed (rank 0): the ids of a fixed, seeded sample of sentences
+and every sentence's id count, as .npy files (see dump_outputs).
 N > 1 (torchrun): sentences shard by rank (no collective); training runs through distributed.train_distributed (words
 hash-partitioned across ranks, per-merge count exchange by peer stores inside the merge-loop kernel).
 """
@@ -57,20 +59,7 @@ def peaks():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except (OSError, KeyError, ValueError, TypeError):  # absent or of another shape: the recipe's stated fallback
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def measured_traffic(kernel, n_sent):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed ncu --set full capture of
-    this very workload (profiles/r02_traffic.json, written from the .ncu-rep by tools/ncu_summary.py); None if absent."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as f:
-            t = json.load(f)
-        if t.get("n_sent") == n_sent and kernel in t.get("kernels", {}):
-            return int(t["kernels"][kernel]["dram_bytes"]), t.get("source")
-    except (OSError, ValueError, KeyError, TypeError):
-        pass
-    return None, None
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def workload(rank, n_sent, train_bytes):
@@ -103,7 +92,7 @@ def workload(rank, n_sent, train_bytes):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.rows, self.proc = [], None
@@ -251,6 +240,37 @@ def emit(out):
         os.write(_REAL_STDOUT, line)
 
 
+class _DeviceArray:
+    """A library-owned device buffer, viewed by torch through the CUDA array interface (no copy)."""
+
+    def __init__(self, ptr, n, typestr):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 3}
+
+
+DUMP_SAMPLE = 100_000   # sentences whose ids are written (~3 M ids, 12 MB as float32)
+
+
+def dump_outputs(out_dir, last, n_sent):
+    """What a caller of yttm_enc_run_device received from the last timed step, written as .npy files:
+      ids.npy               float32  ids of DUMP_SAMPLE sentences drawn with a fixed seed (exact: ids < 2^24)
+      ids_offsets.npy       float64  start of each sampled sentence in ids.npy, plus the end
+      sample_index.npy      float64  indices of the sampled sentences in the batch
+      sentence_n_ids.npy    float32  number of ids of every sentence of the batch
+    The inputs are seeded, so two builds run with the same arguments can be compared file by file."""
+    import torch
+    offs = torch.as_tensor(_DeviceArray(last["offsets"], n_sent + 1, "<i8"), device="cuda").cpu().numpy().astype(np.int64)
+    ids = torch.as_tensor(_DeviceArray(last["ids"], last["n"], "<i4"), device="cuda").cpu().numpy()
+    assert offs[-1] == last["n"]
+    pick = np.sort(np.random.default_rng(20240611).choice(n_sent, min(DUMP_SAMPLE, n_sent), replace=False))
+    lens = offs[pick + 1] - offs[pick]
+    starts = np.repeat(offs[pick] - np.concatenate([[0], np.cumsum(lens)[:-1]]), lens)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "ids.npy"), ids[np.arange(lens.sum()) + starts].astype(np.float32))
+    np.save(os.path.join(out_dir, "ids_offsets.npy"), np.concatenate([[0], np.cumsum(lens)]).astype(np.float64))
+    np.save(os.path.join(out_dir, "sample_index.npy"), pick.astype(np.float64))
+    np.save(os.path.join(out_dir, "sentence_n_ids.npy"), np.diff(offs).astype(np.float32))
+
+
 def r3(x):
     return None if x is None else float("%.4g" % x)
 
@@ -314,6 +334,7 @@ def main():
     ap.add_argument("--no-train-legs", action="store_true", help="encode only (profiling runs)")
     ap.add_argument("--scan-tokens", type=int, default=256 * 1024 * 1024)
     ap.add_argument("--budget-s", type=float, default=420.0, help="optional legs are skipped once the run is this old")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -362,12 +383,15 @@ def main():
     page_ids = np.empty(out_cap, dtype=np.int32)
     page_oo = np.empty(n_sent + 1, dtype=np.uint64)
 
+    last = {}
+
     def step_device():
         out_n = C.c_uint64(0)
         p1, p2 = C.c_void_p(), C.c_void_p()
         rc = L.yttm_enc_run_device(enc, d_bytes.data_ptr(), d_offs.data_ptr(), n_bytes, n_sent, 0, 0, 0, 0.0, 0, 0,
                                    C.byref(p1), C.byref(p2), C.byref(out_n))
         assert rc == 0, L.yttm_last_error(ctx)
+        last.update(ids=p1.value, offsets=p2.value, n=out_n.value)
         return out_n.value
 
     def step_host():
@@ -417,6 +441,8 @@ def main():
     sampler = ClockSampler(local) if rank == 0 else None
     time.sleep(0.3 if rank == 0 else 0.0)
     sec_d, n_ids, kern, launches = timed(step_device, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:     # the results stay valid until the next call on this encoder
+        dump_outputs(args.dump_outputs, last, n_sent)
     sec_h, n_ids_h, _, _ = timed(step_host, args.steps, args.warmup)
     sec_p, n_ids_p, _, _ = timed(step_pageable, max(3, args.steps // 2), 2)
     for _ in range(20):                       # keep the GPU busy long enough for a few more samples
@@ -436,7 +462,7 @@ def main():
              "enc_scan": "scan", "enc_dedup": "dedup_words_kernel", "enc_rep": "encode_rep_words_kernel",
              "enc_copy": "copy_word_ids_kernel"}
     ach = algo / (single[dom] * 1e-3) / 1e9
-    traffic, traffic_src = measured_traffic(names[dom], n_sent)
+    traffic, traffic_src = None, None     # no DRAM counter capture on H100 yet
     roofline = {"bound": "hbm", "kernel": names[dom], "achieved": r3(ach), "peak": hbm_peak, "unit": "GB/s",
                 "frac": r3(ach / hbm_peak), "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": algo, "kernel_ms": {k: r3(v) for k, v in kern.items() if v > 0},
@@ -462,8 +488,7 @@ def main():
                                        "char_hist_GBps": None if piped else r3(nb / fm["char_hist"] / 1e6),
                                        "word_count_GBps": None if piped else r3(nb / fm["word_count"] / 1e6),
                                        "note": ("char_hist + word split run per 32 MB piece on a second stream while the next piece is "
-                                                "copied: their time is inside h2d (kernel rates: profiles/r02_prof_front.raw.csv, "
-                                                "57 / 25 GB/s)") if piped else None,
+                                                "copied: their time is inside h2d") if piped else None,
                                        "algorithmic_bytes": "B per pass (SURVEY 8d)"}
         del shard3
         # ---- BASELINE configs[4] shape: multilingual, vocab 64k, coverage 0.9999, 1.25 GB per GPU (weak)
@@ -621,7 +646,7 @@ def main():
     if rank == 0:
         config = {"workload": WORKLOAD, "sharding": "per GPU: the workload above on every rank (weak scaling), no collective",
                   "sentences_per_gpu": n_sent, "bytes_per_gpu": n_bytes, "ids_per_gpu": n_ids,
-                  "l2": "inputs + slot buffers (%.0f MB) exceed the 126 MB L2" % ((5 * n_bytes) / 1e6),
+                  "l2": "inputs + slot buffers (%.0f MB) exceed the 50 MB L2" % ((5 * n_bytes) / 1e6),
                   "train": cfg_train}
         if enc4:
             config["encode_config4"] = enc4

@@ -1,4 +1,4 @@
-// bpe_b200.h — host C++ surface of the B200 BPE trainer / encoder.
+// bpe_b200.h — host C++ surface of the H100 BPE trainer / encoder.
 //
 // Mirrors the reference's C++ API (youtokentome/cpp/bpe.h:19 train_bpe, :22-82 BaseEncoder;
 // value types of utils.h:11-86) — same names, argument meaning and error behaviour — so code and

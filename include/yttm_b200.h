@@ -1,4 +1,4 @@
-/* yttm_b200.h — the drop-in boundary: a C ABI over the two BPE hot paths on one B200.
+/* yttm_b200.h — the drop-in boundary: a C ABI over the two BPE hot paths on one H100.
  *
  * The reference (VKCOM/YouTokenToMe) has no FFI of its own; its boundary is the C++ header
  * youtokentome/cpp/bpe.h (train_bpe :19, class BaseEncoder :22-82) bound by Cython

@@ -1,7 +1,11 @@
 """ctypes bindings for the CHECKERS (test infrastructure): oracle/liboracle.so (our CPU
 restatement) and oracle/_ref/libyttm_ref_{det,prod}.so (the unmodified reference compiled by
 oracle/Makefile).  Only tests/, __graft_entry__.smoke() and bench.py's CPU legs import this."""
+import atexit
 import ctypes as C
+import hashlib
+import json
+import lzma
 import os
 import subprocess
 import tempfile
@@ -14,7 +18,7 @@ ERRLEN = 1024
 
 
 def build_checkers():
-    """Compile oracle/liboracle.so and, when /root/reference exists, oracle/_ref/*.so."""
+    """Compile oracle/liboracle.so and, when the reference sources exist (oracle/Makefile: REF), oracle/_ref/*.so."""
     subprocess.run(["make", "-s", "-C", ORACLE_DIR, "all"], check=True, stdout=subprocess.DEVNULL)
 
 
@@ -226,6 +230,164 @@ class OracleEncoder(_Enc):
 
 def have_reference(kind="det"):
     return os.path.exists(os.path.join(ORACLE_DIR, "_ref", "libyttm_ref_%s.so" % kind))
+
+
+# ---- stored answers of the reference ---------------------------------------------------------------------------
+# The parity tests compare with the unmodified reference (DETERMINISTIC_QUEUE build).  Its answers to every call those
+# tests make are stored in tests/golden/reference_answers.json.xz, keyed by a digest of the call's inputs, so that the
+# comparison runs without the reference.  YTTM_REFERENCE_RECORD=<file> with oracle/_ref built runs the live reference
+# and writes the stored answers plus its own to <file>.  Large id lists are stored as a digest and compare equal only to the same ids.
+ANSWERS = os.path.join(ROOT, "tests", "golden", "reference_answers.json.xz")
+_FULL_LIST_LIMIT = 4000   # characters of JSON; a longer list answer is stored as its digest
+
+
+def _digest(*parts):
+    h = hashlib.sha256()
+    for p in parts:
+        p = p if isinstance(p, bytes) else repr(p).encode()
+        h.update(len(p).to_bytes(8, "little") + p)
+    return h.hexdigest()[:32]
+
+
+class ListDigest:
+    """A stored list answer too long to keep: compares equal to the list it was taken from, and to nothing else."""
+
+    def __init__(self, digest):
+        self.digest = digest
+
+    @staticmethod
+    def of(value):
+        return hashlib.sha256(json.dumps(value).encode()).hexdigest()[:32]
+
+    def __eq__(self, other):
+        return isinstance(other, list) and ListDigest.of(other) == self.digest
+
+    def __repr__(self):
+        return "ListDigest(%s)" % self.digest
+
+
+class _Answers:
+    def __init__(self):
+        self.record = os.environ.get("YTTM_REFERENCE_RECORD")
+        self.table, self.models = {}, {}
+        if os.path.exists(ANSWERS):
+            with lzma.open(ANSWERS, "rt") as f:
+                d = json.load(f)
+            self.table, self.models = d["calls"], d["models"]
+        if self.record:
+            atexit.register(self.save)
+
+    def save(self):
+        with lzma.open(self.record, "wb", preset=9 | lzma.PRESET_EXTREME) as f:
+            f.write(json.dumps({"calls": self.table, "models": self.models}, sort_keys=True, separators=(",", ":")).encode())
+
+    def get(self, key):
+        if key not in self.table:
+            raise LookupError("no stored reference answer for this call (record it with YTTM_REFERENCE_RECORD): " + key)
+        return self.table[key]
+
+
+_answers = None
+
+
+def _store():
+    global _answers
+    if _answers is None:
+        _answers = _Answers()
+    return _answers
+
+
+def _call(key, live, full=False):
+    """The stored answer of `key`, or (recording) the live reference's, stored on the way: ("ok", value) / ("err", text).
+    A long list is stored as {"digest": ...} and returned as a ListDigest, unless `full`."""
+    st = _store()
+    if st.record and have_reference("det"):
+        try:
+            value = live()
+            if not full and isinstance(value, list) and len(json.dumps(value)) > _FULL_LIST_LIMIT:
+                value = {"digest": ListDigest.of(value)}
+            st.table[key] = ["ok", value]
+        except ValueError as e:
+            st.table[key] = ["err", str(e)]
+    kind, value = st.get(key)
+    if kind == "err":
+        raise ValueError(value)
+    return ListDigest(value["digest"]) if isinstance(value, dict) and "digest" in value else value
+
+
+def _file_bytes(path):
+    with open(path, "rb") as f:
+        return f.read()
+
+
+class StoredReference:
+    """The reference's answers, from the live library while recording, else from tests/golden/reference_answers.json.xz."""
+
+    def train(self, text, model_path, vocab_size, coverage=1.0, n_threads=1, pad=0, unk=1, bos=2, eos=3):
+        args = (vocab_size, coverage, n_threads, pad, unk, bos, eos)
+        return self._train("train", text, lambda: Reference("det").train(text, model_path, *args), model_path, args)
+
+    def train_file(self, input_path, model_path, vocab_size, coverage=1.0, n_threads=1, pad=0, unk=1, bos=2, eos=3):
+        args = (vocab_size, coverage, n_threads, pad, unk, bos, eos)
+        return self._train("train_file", _file_bytes(input_path),
+                           lambda: Reference("det").train_file(input_path, model_path, *args), model_path, args)
+
+    @staticmethod
+    def _train(kind, text, live_train, model_path, args):
+        def live():
+            live_train()
+            model = _file_bytes(model_path)
+            _store().models[_digest(model)] = model.decode("latin-1")   # a model file is ASCII text
+            return {"model": _digest(model)}
+        model = _store().models[_call(_digest(kind, text, *args), live)["model"]]
+        with open(model_path, "wb") as f:
+            f.write(model.encode("latin-1"))
+        return 0.0
+
+    def encoder(self, model_path, n_threads=1):
+        return StoredRefEncoder(model_path, n_threads)
+
+    def char2id_order(self, keys):
+        """Slot order of the reference's char2id container after inserting `keys` in this order."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint32)
+
+        def live():
+            lib = Reference("det").lib
+            lib.ref_char2id_order.restype = C.c_int
+            lib.ref_char2id_order.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
+            out = np.zeros(len(keys), dtype=np.uint32)
+            assert lib.ref_char2id_order(keys.ctypes.data, len(keys), out.ctypes.data) == 0
+            return out.tolist()
+        return _call(_digest("char2id_order", keys.tobytes()), live)
+
+
+class StoredRefEncoder:
+    def __init__(self, model_path, n_threads):
+        self.path, self.n_threads, self.model = model_path, n_threads, _file_bytes(model_path)
+        _call(_digest("open", self.model), lambda: Reference("det").encoder(model_path, n_threads) and 0)
+
+    def _live(self):
+        return Reference("det").encoder(self.path, self.n_threads)
+
+    def vocab_size(self):
+        return _call(_digest("vocab_size", self.model), lambda: self._live().vocab_size())
+
+    def encode(self, sentences, **kw):
+        return _call(_digest("encode", self.model, *sentences, len(sentences), sorted(kw.items())),
+                     lambda: self._live().encode(sentences, **kw))
+
+    def encode_lengths(self, sentences, **kw):
+        """Number of ids of every sentence (where a test needs no more of a long answer)."""
+        return _call(_digest("encode_lengths", self.model, *sentences, len(sentences), sorted(kw.items())),
+                     lambda: [len(s) for s in self._live().encode(sentences, **kw)], full=True)
+
+    def encode_subwords(self, sentences, **kw):
+        return _call(_digest("subwords", self.model, *sentences, len(sentences), sorted(kw.items())),
+                     lambda: self._live().encode_subwords(sentences, **kw))
+
+    def decode(self, ids):
+        return _call(_digest("decode", self.model, np.asarray(ids, dtype=np.int64).tobytes()),
+                     lambda: self._live().decode(ids))
 
 
 def tmp_model_path(tag="m"):

@@ -1,7 +1,7 @@
 // tests/emul/emul.cpp — TEST HARNESS ONLY (never shipped, never a fallback).
 //
 // Runs the kernels' building blocks of youtokentome_b200/csrc/bpe_core.cuh — the SAME source the
-// sm_100a kernels compile — sequentially on the CPU, following the kernels' control flow
+// sm_90a kernels compile — sequentially on the CPU, following the kernels' control flow
 // (per-byte unit/word detection, byte-keyed word dedup, run-rule pair counting, arg-max by
 // pair_prio, has_pair / rewrite_word / whole-word recount, encode_word).  tests/test_emul_cpu.py
 // compares the result with the oracle, so logic errors in the device functions are caught in

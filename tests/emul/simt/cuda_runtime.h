@@ -190,7 +190,7 @@ inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaDeviceGetAttribute(int *v, cudaDeviceAttr a, int) {
-  *v = a == cudaDevAttrMultiProcessorCount ? (int)emu::n_sm() : 232448;  // 227 KB, as on sm_100a
+  *v = a == cudaDevAttrMultiProcessorCount ? (int)emu::n_sm() : 232448;  // 227 KB, as on sm_90a
   return cudaSuccess;
 }
 inline cudaError_t cudaMalloc(void **p, size_t n) {

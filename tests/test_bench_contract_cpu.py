@@ -6,7 +6,9 @@ import os
 import subprocess
 import sys
 
-from _bind import ROOT
+import pytest
+
+from _bind import ROOT, have_reference
 
 
 def test_bench_line_contract_on_the_emulator(tmp_path):
@@ -36,21 +38,26 @@ def test_bench_line_contract_on_the_emulator(tmp_path):
     # hot path (a) travels in keys the driver keeps: config.train.* and roofline.train_*
     tr = d["config"]["train"]
     assert set(tr) >= {"config1", "config3", "config5"}
+    with_reference = have_reference("det") and have_reference("prod")   # bench.py's parity legs run the reference itself
     for key in ("config3", "config5"):
         leg = tr[key]
         assert leg["gpus"] == 1 and leg["merges"] > 0 and leg["GBps"] > 0 and leg["us_per_merge"] > 0 and len(leg["model_sha1"]) == 12
-        assert leg["parity_chunk0"]["equals_reference"] is True
-    assert tr["config1"]["equals_reference"] is True
+        if with_reference:
+            assert leg["parity_chunk0"]["equals_reference"] is True
+    if with_reference:
+        assert tr["config1"]["equals_reference"] is True
     assert set(rf["train_scan"]) >= {"heavy", "light", "algorithmic_bytes_per_merge"} and rf["train_scan"]["heavy"]["frac"] > 0
     assert set(rf["train_front"]) >= {"char_hist_GBps", "word_count_GBps"}
     e4 = d["config"]["encode_config4"]
     assert e4["dropout"] == 0.1 and e4["ids_equal_oracle_on_sample"] is True and e4["Msent_s_device"] > 0
-    assert d["e2e"]["pageable_value"] > 0 and set(cb) >= {"n_threads_1", "train_1GB_8thr"}
+    assert d["e2e"]["pageable_value"] > 0 and set(cb) >= {"n_threads_1"} | ({"train_1GB_8thr"} if with_reference else set())
     assert len(lines[0]) < 8000, "the line must stay small enough for the driver's retained tail"
 
 
-def test_reference_arm_line_contract(tmp_path, reference):
+def test_reference_arm_line_contract(tmp_path, checkers):
     """`bench.py --impl reference` (the unmodified reference's CPU encode_as_ids from oracle/_ref, no GPU involved)."""
+    if not checkers.have_reference("prod"):
+        pytest.skip("oracle/_ref not built: the reference arm times the reference library itself")
     env = dict(os.environ, YTTM_BENCH_CACHE=str(tmp_path / "cache"))
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "1"],
                        cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, timeout=900)

@@ -118,12 +118,10 @@ def test_model_writer_is_byte_identical_to_the_reference(special):
     """write_model (rank 0 of train_distributed) writes the very bytes the reference's BPEState::dump does,
     char2id lines in flat_hash_map order included: feed it the reference's own result un-renamed."""
     import _bind
-    if not _bind.have_reference("det"):
-        pytest.skip("oracle/_ref not built")
     pad, unk, bos, eos = special
     text = _cases.zipf().text(60_000)
     m = tmp_model_path("refw")
-    _bind.Reference("det").train(text, m, 900, 1.0, n_threads=1, pad=pad, unk=unk, bos=bos, eos=eos)
+    _bind.StoredReference().train(text, m, 900, 1.0, n_threads=1, pad=pad, unk=unk, bos=bos, eos=eos)
     c2i, rules, _ = read_model(m)
     # undo rename_tokens: final ids -> internal ids (specials first, then the rest ascending)
     taken = {s for s in special if s != -1}

@@ -1,7 +1,7 @@
 """Byte-identical model dump (SURVEY.md §8f-4): the char2id lines of a model written by the reference
 come in ska::flat_hash_map slot order (utils.cpp:57-59).  `yttm_api_dump_order` replays that order
 from the insertion sequence alone; checked here against model files the UNMODIFIED reference writes
-(oracle/_ref, DETERMINISTIC_QUEUE build) — CPU only, no GPU needed."""
+(DETERMINISTIC_QUEUE build; its stored answers) — CPU only, no GPU needed."""
 import ctypes as C
 import os
 
@@ -11,9 +11,6 @@ import pytest
 import _bind
 from _cases import dirty_zipf_text, stress_case, zipf
 from youtokentome_b200 import _lib, synth
-
-pytestmark = pytest.mark.skipif(not _bind.have_reference("det"), reason="oracle/_ref not built")
-
 
 def file_order(path):
     with open(path) as f:
@@ -35,7 +32,7 @@ def replay(char2id):
 def check(text, vocab, coverage=1.0, **special):
     path = _bind.tmp_model_path("dumporder")
     try:
-        _bind.Reference("det").train(text, path, vocab, coverage, n_threads=1, **special)
+        _bind.StoredReference().train(text, path, vocab, coverage, n_threads=1, **special)
         order, c2i = file_order(path)
         assert replay(c2i) == order
         return len(order)
@@ -78,13 +75,7 @@ def test_wide_code_point_range():
 
 # ---- the replay against the reference's own container on arbitrary key sets ---------------------
 def ref_order(keys):
-    lib = _bind.Reference("det").lib
-    lib.ref_char2id_order.restype = C.c_int
-    lib.ref_char2id_order.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
-    keys = np.ascontiguousarray(keys, dtype=np.uint32)
-    out = np.zeros(len(keys), dtype=np.uint32)
-    assert lib.ref_char2id_order(keys.ctypes.data, len(keys), out.ctypes.data) == 0
-    return out.tolist()
+    return _bind.StoredReference().char2id_order(keys)
 
 
 def our_order(keys):
@@ -153,7 +144,7 @@ def test_product_dump_is_byte_identical_to_the_reference_file(case):
     }[case]
     path = _bind.tmp_model_path("refdump")
     try:
-        _bind.Reference("det").train(text, path, vocab, cov, n_threads=1, **special)
+        _bind.StoredReference().train(text, path, vocab, cov, n_threads=1, **special)
         _redump_equals(path)
     finally:
         if os.path.exists(path):

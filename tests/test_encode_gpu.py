@@ -83,12 +83,10 @@ def test_dropout_matches_oracle_stream(product, oracle, p):
 
 def test_dropout_distribution_vs_reference(product, checkers, oracle):
     """mean tokens / sentence at p = 0.1 within 2 % of the reference's own DropoutQueue."""
-    if not checkers.have_reference("det"):
-        pytest.skip("oracle/_ref absent")
     m = _model(oracle, _cases.dirty_zipf_text(), 1500)
     sents = _cases.zipf_sentences(3000)
-    ref = checkers.Reference("det").encoder(m, n_threads=1)
-    r = sum(map(len, ref.encode(sents, dropout=0.1)))
+    ref = checkers.StoredReference().encoder(m, n_threads=1)
+    r = sum(ref.encode_lengths(sents, dropout=0.1))
     g = sum(map(len, GpuEncoder(m).encode(sents, dropout=0.1, seed=99)))
     assert abs(g - r) / r < 0.02
 
@@ -166,10 +164,8 @@ def test_python_api_roundtrip(product, tmp_path):
 def test_config2_shape_vs_reference(product, checkers):
     """BASELINE config 2 shape at 1/20 scale: 50k x 128-byte Zipf sentences, vocab 8000 model
     trained by the reference; ids identical to the reference (8 threads)."""
-    if not checkers.have_reference("det"):
-        pytest.skip("oracle/_ref absent")
     zc = synth.ZipfCorpus(n_words=50_000, seed=11)
-    ref = checkers.Reference("det")
+    ref = checkers.StoredReference()
     m = tmp_model_path("ref")
     ref.train(zc.text(6_000_000), m, 8000, 1.0, n_threads=8)
     sents = zc.sentences(50_000, 128, seed=77)

@@ -2,7 +2,7 @@
 manual case, batch == single) compiled UNMODIFIED — fed to g++ on stdin from /root/reference, never copied — against
 this repo's drop-in headers (include/compat) and run against the product's kernels under the SIMT emulator
 (tests/emul/simt; test harness only).  The same source linked with the real libyttm_b200.so is built by oracle/Makefile
-into oracle/_ref/ref_stress_b200 and run on the B200 by tests/test_zz_reference_stress_gpu.py."""
+into oracle/_ref/ref_stress_b200 and run on the GPU by tests/test_zz_reference_stress_gpu.py."""
 import os
 import subprocess
 

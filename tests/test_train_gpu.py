@@ -76,23 +76,20 @@ def test_special_ids(product, oracle):
 
 
 def test_readme_config(product, oracle, checkers):
-    """BASELINE config 1 at full size; also against the unmodified reference when present."""
+    """BASELINE config 1 at full size; also against the unmodified reference."""
     text = synth.readme_corpus()
     m = _same(oracle, text, 5000)
-    if checkers.have_reference("det"):
-        ref = checkers.Reference("det")
-        m_r = tmp_model_path("ref")
-        ref.train(text, m_r, 5000, 1.0, n_threads=4)
-        assert read_model(m_r) == read_model(m)
+    ref = checkers.StoredReference()
+    m_r = tmp_model_path("ref")
+    ref.train(text, m_r, 5000, 1.0, n_threads=4)
+    assert read_model(m_r) == read_model(m)
 
 
 def test_zipf_medium_vs_reference(product, checkers):
     """8 MB multi-script Zipf corpus, vocab 8000: too slow for nothing, checked against _ref."""
-    if not checkers.have_reference("det"):
-        pytest.skip("oracle/_ref absent")
     zc = synth.ZipfCorpus(n_words=50_000, seed=11)
     text = zc.text(8_000_000)
-    ref = checkers.Reference("det")
+    ref = checkers.StoredReference()
     m_r = tmp_model_path("ref")
     ref.train(text, m_r, 8000, 0.9995, n_threads=8)
     m_g = gpu_train(text, 8000, 0.9995)
@@ -184,9 +181,7 @@ def test_zz_model_file_bytes_equal_the_reference(product, checkers):
     """SURVEY.md §8f-4: the model FILE (not only its parsed content) equals the one the unmodified reference
     (DETERMINISTIC_QUEUE build) writes — char2id lines in flat_hash_map slot order (tests/test_dump_order.py
     pins that order on the CPU).  Kept last: everything above compares parsed models."""
-    if not checkers.have_reference("det"):
-        pytest.skip("oracle/_ref absent")
-    ref = checkers.Reference("det")
+    ref = checkers.StoredReference()
     for text, vocab, cov in [(synth.readme_corpus(n_lines=800), 600, 1.0), (_cases.zipf().text(300_000), 3000, 1.0),
                              (_cases.dirty_zipf_text(), 2500, 0.995)]:
         m_r = tmp_model_path("refbytes")

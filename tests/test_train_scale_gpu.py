@@ -66,7 +66,7 @@ def test_streaming_merges_equal_a_numpy_recount(product, log2_first, alpha):
     assert L.yttm_ctx_create(0, C.byref(ctx)) == 0
     try:
         wl, iters = 8, 6
-        n_w = 1_500_000                     # 12 M tokens = 48 MB: beyond the 148 x ~200 KB of shared memory
+        n_w = 1_500_000                     # 12 M tokens = 48 MB: beyond the 132 x 227 KB of shared memory of an H100
         assert L.yttm_train_synth_words(ctx, n_w, wl, alpha | (log2_first << 24), 7) == 0, L.yttm_last_error(ctx)
         nw, nt = C.c_uint64(0), C.c_uint64(0)
         assert L.yttm_train_export_words(ctx, None, 0, None, None, 0, C.byref(nw), C.byref(nt)) == 0

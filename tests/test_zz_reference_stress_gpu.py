@@ -1,5 +1,5 @@
 """The reference's OWN stress test (tests/unit_tests/stress_test.cpp, compiled unmodified against include/compat by
-oracle/Makefile -> oracle/_ref/ref_stress_b200, linked with libyttm_b200.so) on the B200: its asserts compare
+oracle/Makefile -> oracle/_ref/ref_stress_b200, linked with libyttm_b200.so) on the GPU: its asserts compare
 learn_bpe_from_string with its learn_bpe_slow spec, encode_as_ids / encode_as_subwords with its decode_slow spec, batch
 with single-sentence encoding, and the decode round trip (stress_test.cpp:313-493).  Runs last (zz)."""
 import os

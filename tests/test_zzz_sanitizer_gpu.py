@@ -3,7 +3,8 @@ sanitizer job: tests/unit_tests/test_stress.py:19-30).  memcheck and synccheck m
 report no ERROR-severity hazard (its WARNING-severity reports are the two documented benign ones of process_tile —
 merge_loop.cuh: a warp re-reads a word that another warp may be rewriting and then competes for the word's claim bit;
 a stale read only costs a no-op rewrite).  Every result of the workload is also compared with the oracle inside the
-script.  A report, a crash or a timeout FAILS.  Logs go to gpurun_out/.  Runs last (zzz)."""
+script.  A report, a crash or a timeout FAILS; a sanitizer that refuses the device (where the driver does not let it
+attach) skips.  Runs last (zzz)."""
 import os
 import re
 import shutil
@@ -27,12 +28,8 @@ def test_sanitizer(product, tool):
     r = subprocess.run([exe, "--tool", tool, sys.executable, os.path.join(ROOT, "tools", "sanitize_small.py")], cwd=ROOT,
                        env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=600)
     text = r.stdout.decode(errors="replace")
-    try:
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(ROOT, "gpurun_out", "sanitizer_%s.log" % tool), "w") as fh:
-            fh.write(text)
-    except OSError:
-        pass
+    if "Error: Device not supported" in text:
+        pytest.skip("compute-sanitizer does not support this device here")
     assert "checks identical to the oracle" in text, text[-1500:]
     if tool == "racecheck":
         m = re.search(r"RACECHECK SUMMARY: (\d+) hazards? displayed \((\d+) errors?, (\d+) warnings?\)", text)

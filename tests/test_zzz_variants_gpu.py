@@ -37,9 +37,3 @@ def test_encode_variants_return_the_default_ids_on_the_bench_shape(product, tmp_
     assert res["default"]["n_ids"] > 0 and set(res) >= {"default", "slots", "plain", "plain+find_vec", "plain+dedup", "bucketed"}
     bad = [k for k, v in res.items() if not v.get("ids_equal_default", True)]
     assert not bad, "variants differ from the default ids on hardware: %s" % bad
-    try:  # evidence (scratch directory; ignored if not writable)
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        with open(os.path.join(ROOT, "gpurun_out", "ab_encode_200k.json"), "w") as fh:
-            json.dump(res, fh, indent=1)
-    except OSError:
-        pass

@@ -1,4 +1,4 @@
-"""A/B of the encode kernels' variants on the bench workload (run on a B200):
+"""A/B of the encode kernels' variants on the bench workload (run on one GPU):
     python tools/ab_encode.py [n_sentences] [reps] [result.json] [model file]
 For each of {default, YTTM_ENC_PLAIN (the round-1 kernels), plain + one variant, ...}: median CUDA-event ms of find / words / gather
 over `reps` runs of yttm_enc_run_device on inputs resident in HBM, and a check that the ids are identical."""

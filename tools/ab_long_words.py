@@ -1,4 +1,4 @@
-"""A/B of the long-word encode path on a B200 (see DESIGN.md "Known weaknesses"):
+"""A/B of the long-word encode path on one GPU (see DESIGN.md "Known weaknesses"):
     python tools/ab_long_words.py [word_bytes=16384] [n_words=8]
 Encodes `n_words` sentences that are each ONE word of `word_bytes` random 'abcd' bytes with the default kernel
 (one thread per word, O(n^2)) and with YTTM_ENC_LONG=1 (a block per word, a pass per rule); wall-clock ms of

@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B of merge-loop launch geometry on a B200: µs per merge and phase split (tools/probe_train.py) for each setting.
+# A/B of merge-loop launch geometry on one GPU: µs per merge and phase split (tools/probe_train.py) for each setting.
 #   usage: tools/ab_train.sh [corpus: zipf|readme] [vocab] [bytes]
 cd "$(dirname "$0")/.."
 C=${1:-zipf}; V=${2:-32000}; B=${3:-100e6}

@@ -19,7 +19,7 @@ it = max(g("loop_iters"), 1.0)
 t_scan = (g("loop_apply") + g("loop_partition") + g("loop_drain")) / it
 ab = 4 * T + 4 * (T // wl)
 print(json.dumps({"log2_first": log2_first, "T": T, "wl": wl, "iters": int(nd.value), "resident": g("loop_resident"), "ms_scan": t_scan,
-                  "GBps": ab / (t_scan * 1e-3) / 1e9, "frac_of_6571.6": ab / (t_scan * 1e-3) / 1e9 / 6571.6,
+                  "GBps": ab / (t_scan * 1e-3) / 1e9, "frac_of_3350": ab / (t_scan * 1e-3) / 1e9 / 3350.0,
                   "phase_ms": {k: g(k) / it for k in ["loop_elect", "loop_apply", "loop_partition", "loop_drain"]},
                   "rules_head": rules[:6].tolist(), "freq_head": fr[:2].tolist()}))
 L.yttm_ctx_destroy(c2)

@@ -1,4 +1,4 @@
-"""Small train + encode workload for compute-sanitizer (SURVEY §8f-4, second half; run on a B200):
+"""Small train + encode workload for compute-sanitizer (SURVEY §8f-4, second half; run on one GPU):
     compute-sanitizer --tool memcheck  --error-exitcode 9 python tools/sanitize_small.py
     compute-sanitizer --tool racecheck --error-exitcode 9 python tools/sanitize_small.py
     compute-sanitizer --tool synccheck --error-exitcode 9 python tools/sanitize_small.py

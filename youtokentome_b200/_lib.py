@@ -10,7 +10,7 @@ LIB_PATH = os.path.join(_HERE, "libyttm_b200.so")
 
 
 def build(force=False):
-    """Compile the CUDA library in-tree (nvcc cross-compiles sm_100a without a GPU)."""
+    """Compile the CUDA library in-tree (nvcc cross-compiles sm_90a without a GPU)."""
     args = ["make", "-s", "-C", os.path.join(_HERE, "csrc")]
     if force:
         subprocess.run(args + ["clean"], check=True)

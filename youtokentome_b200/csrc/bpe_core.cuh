@@ -1,7 +1,7 @@
 // bpe_core.cuh — host/device building blocks of the BPE hot paths.
 //
 // Everything here is __host__ __device__ so the very same source is exercised sequentially on the
-// CPU by tests/emul (a test harness, not a product path) and in parallel by the sm_100a kernels.
+// CPU by tests/emul (a test harness, not a product path) and in parallel by the sm_90a kernels.
 // Reference behaviour restated (never copied); file:line of the reference cited per function.
 #pragma once
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// encode.cu — hot path (b): batch encode_as_ids on one B200.
+// encode.cu — hot path (b): batch encode_as_ids on one H100.
 //
 // Replaces BaseEncoder::encode_parallel / encode_sentence (youtokentome/cpp/bpe.cpp:1697-1738,
 // 1455-1632) behind yttm_enc_run* of include/yttm_b200.h.  The reference gives each CPU thread a
@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(256) find_words_kernel(EncArgs a) {
   }
 }
 
-// EXPERIMENTAL variant (env YTTM_ENC_FIND_CACHED=1, off by default until measured on a B200): the same two
+// EXPERIMENTAL variant (env YTTM_ENC_FIND_CACHED=1, off by default until measured): the same two
 // passes, but the word-start ballots of the first FIND_CACHE chunks (256 bytes) of a sentence stay in registers, so
 // pass 2 re-runs word_start_at only for the tail of longer sentences (128-byte sentences: never).
 constexpr int FIND_CACHE = 8;
@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(256) find_words_cached_kernel(EncArgs a) {
   }
 }
 
-// EXPERIMENTAL variant (env YTTM_ENC_FIND_VEC=1, off by default until measured on a B200): the same two passes and the
+// EXPERIMENTAL variant (env YTTM_ENC_FIND_VEC=1, off by default until measured): the same two passes and the
 // same work-list order, but a lane owns FOUR consecutive bytes - one aligned 32-bit load - instead of one, and decides
 // the word starts on a 12-byte register window (previous / own / next word, the neighbours' by shuffle) instead of
 // 3 - 6 byte loads per position; the 4-bit flags of the first FIND_VEC_CACHE x 128 bytes of a sentence stay in one
@@ -401,7 +401,7 @@ struct LongList {
   uint32_t cap;                // 0 = feature off
 };
 
-// EXPERIMENTAL variant (env YTTM_ENC_BUCKETED=1, off by default until measured on a B200): the same
+// EXPERIMENTAL variant (env YTTM_ENC_BUCKETED=1, off by default until measured): the same
 // per-word work, but a block first takes a window of BUCKET_WINDOW consecutive work items, measures
 // every word (end position, number of UTF-8 lead bytes = tokens before merging) and hands the items
 // out in order of that token count (counting sort in shared memory).  A warp then holds 32 words of
@@ -668,7 +668,7 @@ __global__ void __launch_bounds__(LONG_T) encode_long_words_kernel(EncArgs a, Lo
   }
 }
 
-// EXPERIMENTAL variant (env YTTM_ENC_DEDUP=1, dropout = 0 only, off by default until measured on a B200): every
+// EXPERIMENTAL variant (env YTTM_ENC_DEDUP=1, dropout = 0 only, off by default until measured): every
 // distinct word of the batch is encoded ONCE.  Without dropout the ids of a word are a pure function of its bytes
 // [p0, q): a lead byte whose announced length reaches past q sees either the end of the sentence or the first byte of
 // a space unit (never a continuation byte), INVALID_CP with length 1 in both cases (decode_unit), so nothing outside
@@ -803,7 +803,7 @@ __global__ void __launch_bounds__(256) copy_word_ids_kernel(EncArgs a, uint64_t 
 // The words of sentence s are the work items [sent_wbase[s], + sent_wcnt[s]) in byte order (find_words_vec_kernel); the
 // ids of work item w are the n_tok[r] values at slot(word_pos[r] + 3 word_sent[r] + 1) of its representative r = rep[w]
 // (r = w without dedup).  Two warp-per-sentence kernels replace the 4 (B + 3 S)-byte slot buffer round trip of round 1
-// (memset + per-occurrence copy + ordered compaction: 1.5 GB of DRAM traffic per 128 MB batch, profiles/):
+// (memset + per-occurrence copy + ordered compaction: 1.5 GB of DRAM traffic per 128 MB batch):
 //   sentence_ids_kernel   n_ids[s] = bos + eos + sum of n_tok over the sentence's words
 //   emit_ids_kernel       every lane takes one word, a warp scan gives its place, ids are copied from the
 //                         representative (reverse = mirrored index)
@@ -953,10 +953,10 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   auto *d_total = e->counter.as<unsigned long long>() + 1;
   if (n_sent == 0) return 0;
   ytc::timer_begin(c, "encode");
-  // Kernel selection.  Defaults since round 2 (measured on B200, profiles/r02_ab_encode_*.json, ids identical):
+  // Kernel selection.  Defaults since round 2 (chosen by tools/ab_encode.py, ids identical):
   //   * the 4-bytes-per-lane word finder (SWAR space detection, 4 sentences per warp and round);
-  //   * dropout = 0: the word-dedup path — every distinct word of the batch is encoded once (3.45 -> 1.24 ms), words of
-  //     more than LONG_W slots get a whole block each (a 16 KB word: 30 s on one thread, 9 ms on a block);
+  //   * dropout = 0: the word-dedup path — every distinct word of the batch is encoded once, words of
+  //     more than LONG_W slots get a whole block each (a 16 KB word takes seconds on one thread);
   //   * the DIRECT output path: ids go from the encoded words straight to the packed output (sentence_ids_kernel +
   //     emit_ids_kernel) instead of through the 4 (B + 3 S)-byte slot buffer (memset + copy + ordered compaction).
   // YTTM_ENC_PLAIN=1 selects the round-1 kernels and slot flow (A/B, tests); YTTM_ENC_SLOTS=1 keeps the new kernels

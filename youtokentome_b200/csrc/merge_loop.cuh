@@ -24,10 +24,9 @@
 // There is NO grid barrier in the loop and ONE store -> load hop per merge: a block ends its apply phase by storing
 // "round | flags | entries" for its segment; a block starts its drain by polling those words of all blocks (of all
 // GPUs) until they carry the round — barrier and count fetch are one round trip; the entries carry their own stamps
-// (no fence).  History, measured on B200 with a 100 MB Zipf corpus (profiles/r02_merge_loop_phases.md): two cg
-// grid.sync() + separate fetches 18.7 us per merge; stamped words with every block polling every block's best 17.3 us
-// (the 23.7 k sector requests of a poll round queue at a few L2 slices); last-arriver / block-0 reducer 16.4 - 16.9 us
-// (two more hops and the skew of the owner's partition sweep); replicated front: see DESIGN.md section 7.
+// (no fence).  Tried before and slower: two cg grid.sync() + separate fetches; stamped words with every block polling
+// every block's best (the sector requests of a poll round queue at a few L2 slices); a last-arriver / block-0 reducer
+// (two more hops and the skew of the owner's partition sweep).
 // The launch is still cooperative: all blocks must be co-resident for the polling to terminate.
 // Words live in TILES: RESIDENT mode keeps tile b in the shared memory of block b for the whole
 // launch; STREAMING mode (token buffer larger than the chip's shared memory) stages tiles through
@@ -56,9 +55,9 @@ constexpr uint32_t XQ_CNT_COMPACT = 0x20000000u;  // count word: > 25 % of the b
 constexpr uint32_t XQ_CNT_PLIMIT = 0x10000000u;   // count word: the block's partition is over the load limit
 constexpr uint32_t XQ_CNT_PFULL = 0x08000000u;    // count word: the block's partition ran full (an update was lost)
 constexpr uint32_t XQ_CNT_MASK = 0x07ffffffu;
-// What bounds the exchange on B200 is the SM's load/store unit, not L2: a warp-wide load or store costs ~2 cycles per
+// What bounds the exchange is the SM's load/store unit, not L2: a warp-wide load or store costs ~2 cycles per
 // 128-byte line it touches, so 32 lanes on 32 lines are 64 cycles, and a POLL LOOP that does this from 16 warps keeps
-// the unit busy for a microsecond per sweep (ncu, profiles/r02_merge_loop_stalls.md).  Hence the layout:
+// the unit busy for a microsecond per sweep.  Hence the layout:
 //   * count words: one ROW per reader block (XqHdr::counts[reader][sender]) — the words a block polls are consecutive
 //     (a warp's poll touches 2 lines) and are read by nobody else (no hot L2 lines);
 //   * the first XQ_BOX entries of every segment sit in a place-major MATRIX (XqHdr::places[place][sender]): lanes that
@@ -68,8 +67,8 @@ constexpr int XQ_BOX = 7;
 struct XqHdr {
   // ROWS: the count word (round << 32) | flags | entries of the sender's segment b exists once per local READER block r, at
   // counts[r * XQ_MAX_BLOCKS + b]: the sender stores it nblocks times (posted stores to distinct lines), reader r polls
-  // its own row — nblocks consecutive words that nobody else reads.  (Round 2, measured on B200: with one word per
-  // segment, polled by all 148 blocks, a poll round was 21.9 k sector requests on 148 lines shared by every SM.)
+  // its own row — nblocks consecutive words that nobody else reads.  (With one word per segment, polled by every
+  // block, a poll round was tens of thousands of sector requests on lines shared by every SM.)
   unsigned long long counts[XQ_MAX_BLOCKS * XQ_MAX_BLOCKS];
   uint4 places[XQ_BOX * XQ_MAX_BLOCKS];   // entry e (< XQ_BOX) of the sender's block b: places[e * XQ_MAX_BLOCKS + b]
   // count words of the merge loop for the readers of ANOTHER rank: one per sender block, polled by all blocks of that
@@ -176,7 +175,7 @@ constexpr uint32_t BB_ID_LIMIT = 1u << 22;
 // the low bits of its round, so neither the producer needs a fence between its entries and its count word nor the
 // consumer an acquire — an entry whose stamps are not the round's has simply not arrived yet (NVLink and L2 deliver an
 // aligned 8-byte word whole; nothing orders different addresses without a fence, and a system-scope fence after peer
-// stores cost 9 us per merge on 2 x B200).  w0 = stamp20 | x22 | y22, w1 = stamp20 | value44 (signed).
+// stores cost microseconds per merge).  w0 = stamp20 | x22 | y22, w1 = stamp20 | value44 (signed).
 // stamp = round % 0xfffff, never 0xfffff: the buffer starts as all-ones.  (A slot left untouched for exactly k * 0xfffff
 // rounds of its parity would carry a matching stamp again; with at most 2^22 merges per job that needs one slot to be
 // idle for half a million merges and then be read in the few hundred nanoseconds before its new content lands.)
@@ -701,7 +700,7 @@ __device__ __forceinline__ void xq_drain(const LoopArgs &a, uint32_t round, uint
 //     and the largest member of the front is the global arg-max as long as it is not below the bound;
 //   * otherwise (front exhausted, front too full, too many new pairs in one round) all blocks — they see the same
 //     front — refresh in the same iteration.  A refresh costs FRONT_TOP partition sweeps and one gather, and pays for
-//     a few hundred merges (148 partitions x 8 pairs; the bound sits where the first partition runs out).
+//     a few hundred merges (one partition per SM x 8 pairs; the bound sits where the first partition runs out).
 // The pair table in HBM/L2 stays the ground truth (rebuilds, refreshes, the multi-GPU table build): a block parks the
 // entries it owns in shared memory during the drain and adds them to its partition while it waits for the other blocks'
 // next count words — off the critical path of the merge.
@@ -736,7 +735,7 @@ __device__ __forceinline__ uint32_t smem_tab_find(const unsigned long long *keys
 // 64-bit shared word compiles to a compare-and-swap loop (ATOMS.CAST.SPIN), and the count changes of a merge pile up
 // on few keys (the new token next to its most frequent neighbours), where a loop retries.  (Introduced when the drain
 // was thought to be atomics bound; the session that added it measured no gain by itself — the real limit was the
-// load/store unit, profiles/r02_merge_loop_stalls.md — it stayed because it bounds the work per add.)  The sum is exact
+// load/store unit — it stayed because it bounds the work per add.)  The sum is exact
 // once all adds have landed (nobody reads a count inside the drain).
 __device__ __forceinline__ void smem_add64(unsigned long long *p, unsigned long long delta) {
   uint32_t *w = reinterpret_cast<uint32_t *>(p);   // little endian: w[0] low, w[1] high
@@ -882,7 +881,7 @@ struct FrontCtx {
   PairTab tab;
 };
 // One drained entry.  (Tried out of line, to shrink the loop: the calls and the context struct in local memory made the
-// drain 2 us per merge SLOWER on B200.)
+// drain slower.)
 __device__ __forceinline__ void front_take(const FrontCtx &f, unsigned long long key, long long delta) {
   const uint64_t hh = mix64(key);
   const uint32_t fs = smem_tab_find(f.fk, FRONT_SLOTS - 1, hh, key);
@@ -1249,7 +1248,7 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
             // eight tokens per lane from two 16-byte shared loads; the token after them comes from the
             // next lane.  p = position in the aligned window; occurrence p is inside the tile iff
             // head <= p and p + 1 < total (a word-initial token is never y, so none straddles tiles).
-            // Measured on B200, 2 stages: scalar 45 %, 4 per lane 74-87 %, 8 per lane 75-92 % of HBM peak.
+            // 8 tokens per lane: a scalar scan left most of the HBM bandwidth unused.
             const uint32_t total = head + span;
             for (uint32_t base = cw * 256; base < total; base += ncw * 256) {
               const uint32_t p = base + lane * 8;

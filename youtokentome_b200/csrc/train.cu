@@ -1,4 +1,4 @@
-// train.cu — hot path (a): BPE training on one B200.
+// train.cu — hot path (a): BPE training on one H100.
 //
 // Replaces, behind the C ABI of include/yttm_b200.h, the data-parallel phases of the
 // reference's learn_bpe_from_string (youtokentome/cpp/bpe.cpp:859-1293):
@@ -8,7 +8,7 @@
 //   pair_hist_kernel     <- build_linked_list pair2cnt     (bpe.cpp:436-478)
 //   merge_loop_kernel    <- main loop + worker_doing_merge + PriorityQueue
 //                           (bpe.cpp:1121-1282, 601-811, 149-314; order :110-126)
-// Design (B200-first, not a port): words are deduplicated on the device, their tokens live in
+// Design (GPU-first, not a port): words are deduplicated on the device, their tokens live in
 // one packed uint32 buffer (offsets + uint64 frequencies beside it) that stays resident in
 // HBM/L2; the whole merge loop runs inside ONE persistent cooperative kernel (grid-wide
 // barriers instead of the reference's mutex/condvar ping-pong): each iteration is an exact
@@ -241,10 +241,10 @@ __device__ __forceinline__ bool word_table_insert(const uint8_t *__restrict__ s,
 }
 
 // Word split + dedup of running text: thread per byte position; a position that starts a word hashes it and inserts
-// it into the global word table (exact byte compare on a tag match).  ncu (profiles/r02_prof_front.*): instruction
+// it into the global word table (exact byte compare on a tag match).  Instruction
 // bound — the per-word hash / compare loops run with ~5 of 32 lanes active.  A variant that first aggregated the words
 // of a 64 KB chunk in a shared-memory table (to take the hot words' same-address atomics off L2) was measured SLOWER
-// on B200 (5.5 - 6.4 ms vs 4.4 ms per 100 MB: 4.1 G warp instructions) and was dropped.
+// (more warp instructions than the atomics it saved) and was dropped.
 __global__ void __launch_bounds__(256) word_insert_kernel(const uint8_t *__restrict__ s, uint64_t n, uint64_t lo, uint64_t hi,
                                                           WordTab wt, unsigned long long *counters, uint64_t max_unique) {
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;   // word starts in [lo, hi) of the text [0, n)
@@ -576,7 +576,7 @@ int ensure_loop_geometry(yttm_ctx *c) {
   // STREAMING: n_stage stages; a stage holds a window of q slots plus the overhang of its last
   // word (words of up to q/4 slots stay on the shared-memory path) and at most q/2 + 1 offsets
   {
-    int n_stage = 2;  // measured best on B200 (2: 46 %, 3: 44 %, 4: 41 %, 6: 34 %, 8: 30 % of HBM peak)
+    int n_stage = 2;  // H100: 2, 3 and 4 stages scan within 1.5 % of each other (tools/probe_scan.py, YTTM_STAGES)
     if (const char *e = std::getenv("YTTM_STAGES")) n_stage = std::max(2, std::min(MAX_STAGES, std::atoi(e)));
     const uint32_t per_stage = (uint32_t)(tile_bytes / n_stage / 4) & ~3u;  // uint32 per stage
     // tokens: q + q/4 + 8, offsets: q/2 + 16  ->  q * 1.75 + 24 <= per_stage
@@ -589,7 +589,7 @@ int ensure_loop_geometry(yttm_ctx *c) {
   }
   YT_CUDA(c, cudaFuncSetAttribute(merge_loop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
   YT_CUDA(c, cudaFuncSetAttribute(merge_loop_kernel_512, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
-  int threads = 512, per_sm = 0;   // measured on B200: 8.8 us per merge with 512 threads (128 registers), 10.7 us with 1024
+  int threads = 512, per_sm = 0;   // H100, 100 MB Zipf: 8.1 us per merge with 512 threads (128 registers), 11.3 with 1024 (64, spills)
   if (const char *e = std::getenv("YTTM_LOOP_THREADS")) threads = std::max(64, std::min(1024, std::atoi(e) / 32 * 32));
   YT_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, threads <= 512 ? merge_loop_kernel_512 : merge_loop_kernel, threads, dyn));
   if (per_sm < 1) YT_FAIL(c, "merge_loop_kernel does not fit on an SM");
@@ -918,7 +918,7 @@ double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
 }
 uint64_t yttm_launch_count(const yttm_ctx *c) { return c->launches; }
 
-// EXPERIMENTAL (env YTTM_TRAIN_PINNED_H2D=<host threads>, off by default until measured on a B200; SURVEY 8f-1): the
+// EXPERIMENTAL (env YTTM_TRAIN_PINNED_H2D=<host threads>, off by default until measured; SURVEY 8f-1): the
 // corpus comes from PAGEABLE host memory, which cudaMemcpyAsync stages through the driver's own bounce buffer at
 // ~10 GB/s (9.4 ms for 100 MB measured, ~1 s for 10 GB).  Here `threads` host threads copy 32 MB slices into one of two
 // pinned staging buffers while the DMA engine drains the other one; an event per buffer guards its reuse.
@@ -1525,7 +1525,7 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
       if (c->loop_relaunches == 0) YT_CUDA(c, cudaMemsetAsync(c->scratch_cnt.p, 0, (size_t)c->loop_blocks * 128, c->stream));
       a.dbg_blk = c->scratch_cnt.as<unsigned long long>();
     }
-    a.front_top = 4;   // measured on B200 (100 MB Zipf): 8 -> 9.6, 4 -> 8.8, 2 -> 9.3 us per merge (smaller front: shorter probes and scans, more refreshes)
+    a.front_top = 4;   // smaller front: shorter probes and scans, but more refreshes (A/B: YTTM_FRONT_TOP)
     if (const char *e = std::getenv("YTTM_FRONT_TOP")) a.front_top = (uint32_t)std::max(1, std::min((int)FRONT_TOP, std::atoi(e)));
     {  // as many places per segment as ONE trip of the drain's items holds (1 GPU: all 7; 8 GPUs: 1)
       const uint32_t nseg = c->xq_world * c->xq_nblocks;

@@ -1,5 +1,5 @@
 """The reference's Python surface (youtokentome/youtokentome.py:1-99 + the Cython class
-youtokentome/cpp/yttm.pyx:52-181) over the B200 library: same class, method names, argument
+youtokentome/cpp/yttm.pyx:52-181) over the CUDA library: same class, method names, argument
 meaning, return types and exceptions (ValueError(status.message), TypeError for bad argument
 types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path) and
 `dropout_seed`."""

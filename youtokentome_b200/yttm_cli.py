@@ -1,5 +1,5 @@
 """`yttm bpe | encode | decode | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
-same sub-commands, option names, defaults and stdin/stdout framing) over the B200 library.
+same sub-commands, option names, defaults and stdin/stdout framing) over the CUDA library.
 Run as `python -m youtokentome_b200.yttm_cli ...`.  `--n_threads` is accepted and ignored."""
 import click
 
