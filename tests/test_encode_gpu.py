@@ -92,7 +92,6 @@ def test_dropout_distribution_vs_reference(product, checkers, oracle):
 
 
 def check_space_id_zero(oracle, special):
-    import os
     text = _cases.zipf().text(60_000) + b" zab zab ab z zz z q"
     n_chars = len(set(text.decode().replace("\n", " ").replace(" ", "")))
     m = tmp_model_path("orc")
@@ -103,14 +102,8 @@ def check_space_id_zero(oracle, special):
     kws = [dict(), dict(reverse=True), dict(dropout=0.3, seed=5)]
     if special["bos"] != -1:
         kws.append(dict(bos=True, eos=True))
-    for plain in (False, True):
-        if plain:
-            os.environ["YTTM_ENC_PLAIN"] = "1"
-        try:
-            for kw in kws:
-                assert g.encode(sents, **kw) == o.encode(sents, **kw), (plain, kw)
-        finally:
-            os.environ.pop("YTTM_ENC_PLAIN", None)
+    for kw in kws:
+        assert g.encode(sents, **kw) == o.encode(sents, **kw), kw
 
 
 @pytest.mark.parametrize("special", [dict(pad=-1, unk=1, bos=2, eos=3), dict(pad=-1, unk=5, bos=-1, eos=-1)])

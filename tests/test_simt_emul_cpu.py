@@ -155,52 +155,25 @@ def test_encode_manual_corpora(emu, oracle, name):
 
 
 def test_encode_unicode_long_words_dropout(emu, oracle):
+    """Multi-script words, invalid bytes, words longer than the thread-local arrays (LOCAL_W) and than 512 slots, and
+    more than 3 x 512 words in one batch; with and without dropout."""
     m = EG._model(oracle, _cases.dirty_zipf_text(), 1500, 0.95)
     zc = _cases.zipf()
     long_word = b"".join(zc.sentences(20, 60, seed=6)).replace(b" ", b"")  # > LOCAL_W: works in its global slots
-    sents = _cases.zipf_sentences(300) + _cases.EDGE_SENTENCES + [long_word, b"a" * 700, long_word + b" x " + long_word]
+    sents = (_cases.zipf_sentences(400) + _cases.EDGE_SENTENCES +
+             [long_word, b"a" * 700, long_word + b" x " + long_word, b"\x80\x80\x80 \xbf\xbf"])
+    assert sum(len(s.split()) for s in sents) > 3 * 512
     g, o = EG.GpuEncoder(m), oracle.encoder(m)
     for kw in EG.KW:
         assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    for p, seed in ((0.1, 3), (0.6, 4), (1.0, 5)):
+    for p, seed in ((0.1, 3), (0.3, 9), (0.6, 4), (1.0, 5)):
         assert g.encode(sents, dropout=p, seed=seed) == o.encode(sents, dropout=p, seed=seed)
 
 
-def test_encode_bucketed_variant(emu, oracle, monkeypatch):
-    """The experimental length-bucketed word kernel (YTTM_ENC_BUCKETED, off by default, not yet run on hardware):
-    same ids as the oracle, with and without dropout, across window boundaries (BUCKET_WINDOW = 512 words)."""
-    monkeypatch.setenv("YTTM_ENC_BUCKETED", "1")
-    m = EG._model(oracle, _cases.dirty_zipf_text(), 1500)
-    zc = _cases.zipf()
-    long_word = b"".join(zc.sentences(20, 60, seed=6)).replace(b" ", b"")
-    sents = _cases.zipf_sentences(400) + _cases.EDGE_SENTENCES + [long_word, b"\x80\x80\x80 \xbf\xbf"]
-    g, o = EG.GpuEncoder(m), oracle.encoder(m)
-    assert sum(len(s.split()) for s in sents) > 3 * 512
-    for kw in EG.KW[:2]:
-        assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    assert g.encode(sents, dropout=0.3, seed=9) == o.encode(sents, dropout=0.3, seed=9)
-
-
-def test_encode_find_cached_variant(emu, oracle, monkeypatch):
-    """The experimental find_words kernel that keeps the ballots of the first 256 bytes in registers
-    (YTTM_ENC_FIND_CACHED, off by default): sentences shorter, equal and longer than the cached window."""
-    monkeypatch.setenv("YTTM_ENC_FIND_CACHED", "1")
-    m = EG._model(oracle, _cases.dirty_zipf_text(), 1500)
-    zc = _cases.zipf()
-    sents = (_cases.zipf_sentences(200) + _cases.EDGE_SENTENCES + zc.sentences(40, 255, seed=2) + zc.sentences(40, 257, seed=3) +
-             [b" ".join(zc.sentences(30, 100, seed=5)), b"x" * 256, b"x " * 128, b" " * 300 + b"y", b"z" * 31 + b" " + b"w" * 300])
-    g, o = EG.GpuEncoder(m), oracle.encoder(m)
-    for kw in EG.KW:
-        assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    monkeypatch.setenv("YTTM_ENC_BUCKETED", "1")   # both experimental kernels together
-    assert g.encode(sents, bos=True) == o.encode(sents, bos=True)
-
-
 @pytest.mark.parametrize("special", [dict(), dict(pad=-1, bos=-1, eos=7, unk=0), dict(pad=3, unk=40, bos=41, eos=1000)])
-def test_encode_linear_product_id_variant(emu, oracle, monkeypatch, special):
-    """YTTM_ENC_ZLIN (experimental, off by default): the id a rule produces is computed from its rank (special ids
-    skipped) instead of probing the table again; enabled by the host only if it reproduces every rule of the model."""
-    monkeypatch.setenv("YTTM_ENC_ZLIN", "1")
+def test_encode_special_id_layouts(emu, oracle, special):
+    """Special ids below, between and above the ids of the characters and rules (the product of rule k is the k-th
+    free id): with and without dropout."""
     m = tmp_model_path("orc")
     oracle.train(_cases.dirty_zipf_text(), m, 1200, 1.0, **special)
     sents = _cases.zipf_sentences(300) + _cases.EDGE_SENTENCES
@@ -209,14 +182,12 @@ def test_encode_linear_product_id_variant(emu, oracle, monkeypatch, special):
     for kw in kws:
         assert g.encode(sents, **kw) == o.encode(sents, **kw)
     assert g.encode(sents, dropout=0.4, seed=11) == o.encode(sents, dropout=0.4, seed=11)
-    assert emu.yttm_stage_ms(emu.yttm_api_device_context(g.h), b"enc_variant") == 3.0  # the shortcut really ran
 
 
-def test_encode_linear_product_id_is_refused_for_a_foreign_model(emu, oracle, monkeypatch, tmp_path):
-    """A model whose rule products are NOT the k-th free id (two product ids swapped by hand): the shortcut must be
-    switched off by the check at load time, the result stays exact."""
+def test_encode_rule_products_are_read_from_the_model(emu, oracle, tmp_path):
+    """A model whose rule products are NOT the k-th free id (two product ids swapped by hand): the encoder takes the
+    id a rule produces from the model, never from the rule's rank."""
     from _bind import read_model
-    monkeypatch.setenv("YTTM_ENC_ZLIN", "1")
     m = tmp_model_path("orc")
     oracle.train(synth.readme_corpus(n_lines=200), m, 60, 1.0)
     c2i, rules, special = read_model(m)
@@ -234,7 +205,6 @@ def test_encode_linear_product_id_is_refused_for_a_foreign_model(emu, oracle, mo
     sents = [synth.readme_corpus(n_lines=3, seed=4), b"abab cdcd abcd", b"dddd aaaa"]
     g = EG.GpuEncoder(m2)
     assert g.encode(sents) == oracle.encoder(m2).encode(sents)
-    assert emu.yttm_stage_ms(emu.yttm_api_device_context(g.h), b"enc_variant") == 24.0  # refused: the default path (dedup 8 + direct output 16)
 
 
 def test_encode_chunked_pipeline(emu, oracle, monkeypatch):
@@ -248,10 +218,6 @@ def test_encode_chunked_pipeline(emu, oracle, monkeypatch):
     # (the previous version used 1.2 MB: the "no tiny tail chunk" rule folded it into ONE chunk)
     assert emu.yttm_stage_ms(emu.yttm_api_device_context(g.h), b"enc_chunks") >= 3
     assert g.encode(sents, dropout=0.2, seed=77) == oracle.encoder(m).encode(sents, dropout=0.2, seed=77)
-    monkeypatch.setenv("YTTM_ENC_CHUNK_MB", "2")
-    monkeypatch.setenv("YTTM_ENC_FIRST_CHUNK_MB", "1")   # A/B knob: a smaller first chunk (1 + 2 + rest)
-    assert g.encode(sents, bos=True, eos=True) == want
-    assert emu.yttm_stage_ms(emu.yttm_api_device_context(g.h), b"enc_chunks") == 2
 
 
 def test_python_api_on_the_emulated_library(emu, tmp_path):
@@ -331,13 +297,10 @@ def test_train_deferred_list_overflow_falls_back_to_the_direct_pass(emu, oracle,
     TG._same(oracle, synth.readme_corpus(n_lines=120), 150)
 
 
-def test_encode_long_words_block_kernel(emu, oracle, monkeypatch):
+def test_encode_long_words_merged_by_a_block(emu, oracle):
     """Words of more than 512 slots get a whole block and are merged pass by pass (all occurrences of the minimum rule
-    per pass) instead of one merge at a time by one thread (default since round 2, dropout = 0).  Here through the
-    bucketed kernel (YTTM_ENC_BUCKETED); the default dedup path hands its long representatives to the same kernel
-    (test_encode_dedup_variant, test_encode_space_token_with_id_zero)."""
-    monkeypatch.setenv("YTTM_ENC_LONG", "1")
-    monkeypatch.setenv("YTTM_ENC_BUCKETED", "1")
+    per pass) instead of one merge at a time by one thread (dropout = 0: the dedup path hands its long representatives
+    to encode_long_words_kernel)."""
     rng = np.random.default_rng(3)
     train = synth.readme_corpus(n_lines=400) + b" " + _cases.dirty_zipf_text(60_000)
     m = EG._model(oracle, train, 700)
@@ -351,7 +314,6 @@ def test_encode_long_words_block_kernel(emu, oracle, monkeypatch):
     g, o = EG.GpuEncoder(m), oracle.encoder(m)
     for kw in EG.KW:
         assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    assert emu.yttm_stage_ms(emu.yttm_api_device_context(g.h), b"enc_variant") == 5.0   # long-word path + bucketed
     # with dropout the words stay on the sequential path (the per-event draws are order dependent)
     assert g.encode(sents[:4], dropout=0.3, seed=5) == o.encode(sents[:4], dropout=0.3, seed=5)
     # a model made of x x rules ((a,a), (aa,aa), ...): runs take every second occurrence from the run's start
@@ -366,13 +328,12 @@ def test_encode_long_words_block_kernel(emu, oracle, monkeypatch):
 
 @pytest.mark.parametrize("knobs", [dict(), dict(YTTM_ENC_DEDUP_SLOTS="4"), dict(YTTM_ENC_DEDUP_WEAKTAG="1"),
                                    dict(YTTM_ENC_DEDUP_SLOTS="64", YTTM_ENC_DEDUP_WEAKTAG="1")])
-def test_encode_dedup_variant(emu, oracle, monkeypatch, knobs):
-    """The word-dedup path (default since round 2 for dropout = 0): every distinct word of the batch is encoded once, the other
-    occurrences copy the ids of their representative.  Same ids as the oracle, including words that differ only in
+def test_encode_word_dedup(emu, oracle, monkeypatch, knobs):
+    """The word-dedup path (dropout = 0): every distinct word of the batch is encoded once, the other occurrences
+    copy the ids of their representative.  Same ids as the oracle, including words that differ only in
     what follows them (end of sentence / space / U+2581), prefixes of each other, truncated UTF-8, repeated long words
     (> LOCAL_W, merged in global slots); a 4-slot table (nearly every word represents itself), equal tags (every
     probe ends in the byte compare) and both."""
-    monkeypatch.setenv("YTTM_ENC_DEDUP", "1")
     for k, v in knobs.items():
         monkeypatch.setenv(k, v)
     m = EG._model(oracle, _cases.dirty_zipf_text(), 1500, 0.95)
@@ -391,21 +352,8 @@ def test_encode_dedup_variant(emu, oracle, monkeypatch, knobs):
     g, o = EG.GpuEncoder(m), oracle.encoder(m)
     for kw in EG.KW:
         assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    ctx = emu.yttm_api_device_context(g.h)
-    assert emu.yttm_stage_ms(ctx, b"enc_variant") == 24.0   # dedup (8) + direct output (16)
-    # with dropout every occurrence draws for itself: the per-word kernel runs (direct output stays)
+    # with dropout every occurrence draws for itself: the per-word kernel runs
     assert g.encode(sents[:200], dropout=0.3, seed=5) == o.encode(sents[:200], dropout=0.3, seed=5)
-    assert emu.yttm_stage_ms(ctx, b"enc_variant") == 16.0
-    monkeypatch.setenv("YTTM_ENC_SLOTS", "1")      # the same kernels through the round-1 slot flow (copy + ordered compaction)
-    for kw in EG.KW:
-        assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    assert emu.yttm_stage_ms(ctx, b"enc_variant") == 8.0
-    monkeypatch.delenv("YTTM_ENC_SLOTS")
-    monkeypatch.setenv("YTTM_ENC_PLAIN", "1")      # the round-1 kernels remain selectable
-    monkeypatch.delenv("YTTM_ENC_DEDUP")
-    assert g.encode(sents, eos=True) == o.encode(sents, eos=True)
-    assert emu.yttm_stage_ms(ctx, b"enc_variant") == 0.0
-    monkeypatch.delenv("YTTM_ENC_PLAIN")
     monkeypatch.setenv("YTTM_ENC_CHUNK_MB", "1")  # representatives never cross a chunk of the host-buffer pipeline
     if n1 == 400:   # (2 MB through a 4-slot table would take the emulator minutes; the chunking does not depend on the table)
         big = sents * 40
@@ -413,13 +361,12 @@ def test_encode_dedup_variant(emu, oracle, monkeypatch, knobs):
         assert g.encode(big, eos=True) == o.encode(big, eos=True)
 
 
-def test_encode_find_vec_variant(emu, oracle, monkeypatch):
-    """YTTM_ENC_FIND_VEC (experimental, off by default): the word-start kernel that gives a lane four bytes (one aligned
-    32-bit load) and decides on a register window.  Sentence starts at every alignment, sentences shorter / equal /
-    longer than the 1024-byte flag cache, U+2581 and stray bytes at the sentence bounds, a batch whose base address is
-    not 4-byte aligned (yttm_enc_run_device on an offset pointer), and the variant combined with the dedup kernels."""
+def test_encode_word_finder_edges_and_misaligned_base(emu, oracle):
+    """The word-start kernel gives a lane four bytes (one aligned 32-bit load) and decides on a register window.
+    Sentence starts at every alignment, sentences shorter / equal / longer than the flag cache and than 255 / 256 / 257
+    bytes, U+2581 and stray bytes at the sentence bounds, and a batch whose base address is not 4-byte aligned
+    (yttm_enc_run_device on an offset pointer)."""
     import ctypes as C
-    monkeypatch.setenv("YTTM_ENC_FIND_VEC", "1")
     m = EG._model(oracle, _cases.dirty_zipf_text(), 1500)
     zc = _cases.zipf()
     sp = b"\xe2\x96\x81"
@@ -429,14 +376,13 @@ def test_encode_find_vec_variant(emu, oracle, monkeypatch):
             # U+2581 split over a sentence boundary must not be seen as one: neither side's neighbour bytes count
             b"a\xe2\x96", b"\x81b c", b"a\xe2", b"\x96\x81b c", b"ab\xe2\x96", b"\x81", b"q", b"\x96\x81", b"zz " + sp[:2], sp[2:] + sp + b"k"]
     sents = (_cases.zipf_sentences(200) + _cases.EDGE_SENTENCES + edge + zc.sentences(12, 1023, seed=2) + zc.sentences(12, 1025, seed=3) +
-             [b" ".join(zc.sentences(40, 100, seed=5)), b"x" * 1024, b"x " * 700, b" " * 1100 + b"y", b"z" * 31 + b" " + b"w" * 1300] + edge[::-1])
+             [b" ".join(zc.sentences(40, 100, seed=5)), b"x" * 1024, b"x " * 700, b" " * 1100 + b"y", b"z" * 31 + b" " + b"w" * 1300] + edge[::-1] +
+             zc.sentences(40, 255, seed=2) + zc.sentences(40, 257, seed=3) +
+             [b" ".join(zc.sentences(30, 100, seed=5)), b"x" * 256, b"x " * 128, b" " * 300 + b"y", b"z" * 31 + b" " + b"w" * 300])
     g, o = EG.GpuEncoder(m), oracle.encoder(m)
     for kw in EG.KW:
         assert g.encode(sents, **kw) == o.encode(sents, **kw)
     assert g.encode(sents, dropout=0.4, seed=11) == o.encode(sents, dropout=0.4, seed=11)
-    monkeypatch.setenv("YTTM_ENC_DEDUP", "1")
-    assert g.encode(sents, eos=True) == o.encode(sents, eos=True)
-    monkeypatch.delenv("YTTM_ENC_DEDUP")
     # misaligned batch base: the same bytes at offsets 1, 2, 3 of an aligned buffer
     import _bind
     buf, offs = _bind._pack(sents)

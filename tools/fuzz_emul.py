@@ -17,8 +17,7 @@ from _emu import emu_lib  # noqa: E402
 from youtokentome_b200 import synth  # noqa: E402
 
 KNOBS = ["YT_EMU_SMS", "YT_EMU_SCHED_SEED", "YTTM_FORCE_STREAM", "YTTM_STREAM_Q", "YTTM_STAGES", "YTTM_PAIR_CAP_FLOOR", "YTTM_DEFER_CAP",
-         "YTTM_ENC_BUCKETED", "YTTM_ENC_FIND_CACHED", "YTTM_ENC_ZLIN", "YTTM_ENC_LONG", "YTTM_ENC_CHUNK_MB",
-         "YTTM_ENC_DEDUP", "YTTM_ENC_DEDUP_SLOTS", "YTTM_ENC_DEDUP_WEAKTAG", "YTTM_ENC_FIND_VEC", "YTTM_XQ_SEG_CAP", "YTTM_ENC_PLAIN", "YTTM_ENC_SLOTS",
+         "YTTM_ENC_CHUNK_MB", "YTTM_ENC_DEDUP_SLOTS", "YTTM_ENC_DEDUP_WEAKTAG", "YTTM_XQ_SEG_CAP",
          "YTTM_PAIR_MAX_LOAD_PCT", "YTTM_TRAIN_PINNED_H2D", "YTTM_TRAIN_PINNED_CHUNK_KB", "YTTM_LOOP_BLOCKS",
          "YTTM_FRONT_TOP", "YTTM_NEWP_LIMIT", "YTTM_DRAIN_PLACES", "YTTM_TRAIN_PIPELINE", "YTTM_TRAIN_PIPELINE_PIECE_KB", "YTTM_LOOP_THREADS"]
 
@@ -55,11 +54,9 @@ def encode_case(rng, L, orc, model, text):
             kw = dict(bos=bool(rng.integers(0, 2)), eos=bool(rng.integers(0, 2)), reverse=bool(rng.integers(0, 2)))
             p = float(rng.choice([0.0, 0.0, 0.1, 0.5, 1.0]))
             seed = int(rng.integers(0, 2 ** 31))
-            for k in ("YTTM_ENC_BUCKETED", "YTTM_ENC_FIND_CACHED", "YTTM_ENC_ZLIN", "YTTM_ENC_LONG", "YTTM_ENC_DEDUP",
-                      "YTTM_ENC_DEDUP_WEAKTAG", "YTTM_ENC_FIND_VEC", "YTTM_ENC_PLAIN", "YTTM_ENC_SLOTS"):
-                os.environ.pop(k, None)
-                if rng.integers(0, 2):
-                    os.environ[k] = "1"
+            os.environ.pop("YTTM_ENC_DEDUP_WEAKTAG", None)
+            if rng.integers(0, 2):
+                os.environ["YTTM_ENC_DEDUP_WEAKTAG"] = "1"   # equal tags: every probe ends in the byte compare
             os.environ.pop("YTTM_ENC_DEDUP_SLOTS", None)
             if rng.integers(0, 2):
                 os.environ["YTTM_ENC_DEDUP_SLOTS"] = str(int(rng.choice([1, 8, 64, 1024])))  # tiny tables: probe overflow

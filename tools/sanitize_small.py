@@ -3,8 +3,8 @@
     compute-sanitizer --tool racecheck --error-exitcode 9 python tools/sanitize_small.py
     compute-sanitizer --tool synccheck --error-exitcode 9 python tools/sanitize_small.py
 Sizes are tiny on purpose (the tools slow kernels down 10 - 100x): stress-shaped and dirty multi-script corpora of a few
-KB, RESIDENT and forced-STREAMING merge loops (roomy and tiny exchange segments / table partitions), the default encode kernels with and without dropout, then every
-experimental encode variant.  Every result is also compared with the oracle (test infrastructure), so a run that is
+KB, RESIDENT and forced-STREAMING merge loops (roomy and tiny exchange segments / table partitions), the encode kernels
+with and without dropout.  Every result is also compared with the oracle (test infrastructure), so a run that is
 clean but wrong still fails.  `--emulate` runs the same script on the CPU SIMT emulator (a dry run of the script)."""
 import os
 import sys
@@ -17,9 +17,6 @@ import _cases  # noqa: E402
 from _bind import read_model, tmp_model_path  # noqa: E402
 from youtokentome_b200 import _lib, synth  # noqa: E402
 
-ENC_KNOBS = ["YTTM_ENC_PLAIN", "YTTM_ENC_SLOTS", "YTTM_ENC_FIND_CACHED", "YTTM_ENC_FIND_VEC", "YTTM_ENC_BUCKETED", "YTTM_ENC_ZLIN", "YTTM_ENC_LONG", "YTTM_ENC_DEDUP"]
-
-
 def main():
     if "--emulate" in sys.argv:
         from _emu import emu_lib
@@ -31,7 +28,7 @@ def main():
     n_ok = 0
     corpora = [(synth.stress_text(3), 60, 1.0), (synth.stress_text(11), 90, 0.97), (_cases.dirty_zipf_text(30_000), 400, 0.98),
                (synth.readme_corpus(n_lines=60), 120, 1.0)]
-    quick = bool(os.environ.get("YTTM_SANITIZE_QUICK"))   # under a sanitizer: fewer corpora, fewer encode variants
+    quick = bool(os.environ.get("YTTM_SANITIZE_QUICK"))   # under a sanitizer: fewer corpora
     if quick:
         corpora = corpora[1:3]
     for stream, tiny in ((False, False), (True, False), (False, True), (True, True)):
@@ -56,18 +53,11 @@ def main():
     long_word = b"".join(zc.sentences(12, 60, seed=6)).replace(b" ", b"")
     sents = _cases.zipf_sentences(150) + list(_cases.EDGE_SENTENCES) + [long_word, b"a" * 700 + b" " + b"a" * 700, long_word + b" x " + long_word]
     g, o = GpuEncoder(model), orc.encoder(model)
-    variants = [[]] + [[k] for k in ENC_KNOBS] + [["YTTM_ENC_FIND_VEC", "YTTM_ENC_DEDUP"], ["YTTM_ENC_FIND_CACHED", "YTTM_ENC_BUCKETED", "YTTM_ENC_ZLIN"]]
-    if quick:
-        variants = [[], ["YTTM_ENC_PLAIN"], ["YTTM_ENC_SLOTS"], ["YTTM_ENC_BUCKETED", "YTTM_ENC_LONG"]]
-    for env in variants:
-        for k in ENC_KNOBS:
-            os.environ.pop(k, None)
-        for k in env:
-            os.environ[k] = "1"
-        assert g.encode(sents, bos=True, eos=True) == o.encode(sents, bos=True, eos=True), env
-        assert g.encode(sents, reverse=True) == o.encode(sents, reverse=True), env
-        assert g.encode(sents, dropout=0.3, seed=7) == o.encode(sents, dropout=0.3, seed=7), env
-        n_ok += 3
+    # long_word and the 700-byte words are longer than 512 slots: they reach the block-per-word kernel
+    assert g.encode(sents, bos=True, eos=True) == o.encode(sents, bos=True, eos=True)
+    assert g.encode(sents, reverse=True) == o.encode(sents, reverse=True)
+    assert g.encode(sents, dropout=0.3, seed=7) == o.encode(sents, dropout=0.3, seed=7)
+    n_ok += 3
     del g
     os.remove(model)
     print("sanitize_small: %d checks identical to the oracle" % n_ok)
