@@ -164,6 +164,18 @@ class BaseEncoder {
                               const int32_t **d_ids, const uint64_t **d_id_offsets, uint64_t *total_ids, bool bos = false,
                               bool eos = false, bool reverse = false, double dropout_prob = 0) const;
 
+  // decode() of a packed batch on the GPU: sentence i = ids[offsets[i], offsets[i+1]), text i =
+  // text[text_offsets[i], text_offsets[i+1]).  Status code 2 (nothing written, *total_bytes = size needed) when
+  // text_cap is too small.
+  Status decode_packed_into(const int32_t *ids, const uint64_t *offsets, uint64_t n_sentences, const int32_t *ignore_ids,
+                            uint64_t n_ignore, uint8_t *text, uint64_t text_cap, uint64_t *text_offsets,
+                            uint64_t *total_bytes) const;
+  // DEVICE-resident ids[n_ids] / offsets, results left on the device: *d_text / *d_text_offsets point into
+  // library-owned memory that stays valid until the next decode_packed_device call on this object.
+  Status decode_packed_device(const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sentences,
+                              const int32_t *ignore_ids, uint64_t n_ignore, const uint8_t **d_text,
+                              const uint64_t **d_text_offsets, uint64_t *total_bytes) const;
+
   Status id_to_subword(int id, std::string *subword, bool replace_space = false) const;
   int subword_to_id(const std::string &token) const;
 

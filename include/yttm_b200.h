@@ -29,7 +29,8 @@ const char *yttm_last_error(const yttm_ctx *ctx); /* ctx may be NULL: error of t
 int yttm_device_count(void);
 
 /* cudaEvent milliseconds of the last call of the named stage ("char_hist", "word_count",
- * "tokenise", "pair_hist", "merge_loop", "encode", "h2d", "d2h"); < 0 if unknown. */
+ * "tokenise", "pair_hist", "merge_loop", "encode", "h2d", "d2h", "decode", "dec_count", "dec_scan",
+ * "dec_emit", "dec_e2e"); < 0 if unknown. */
 double yttm_stage_ms(const yttm_ctx *ctx, const char *stage);
 /* number of kernel launches issued by this context so far (bench.py: gpu_launches) */
 uint64_t yttm_launch_count(const yttm_ctx *ctx);
@@ -161,6 +162,27 @@ int yttm_enc_run(yttm_enc *enc, const char *bytes, const uint64_t *offsets, uint
 int yttm_enc_run_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
                         uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                         uint64_t first_sentence_index, const int32_t **d_out_ids, const uint64_t **d_out_offsets,
+                        uint64_t *out_n);
+
+/* ---- decoding: BaseEncoder::decode (bpe.cpp:1843-1861 + id_to_subword :1774-1807) of a batch ---- */
+
+/* Sentence i = ids[offsets[i], offsets[i+1]) (absolute indices; offsets[0] need not be 0, offsets must not decrease).
+ * Ids listed in ignore[n_ignore] (a HOST array) are skipped; any other id outside [0, vocab_size) fails with the
+ * host decode's text ("id must be in the range ...") for the first such id in batch order, and nothing is written.
+ * Every other id gives its piece (special tokens as "<UNK>" / "<PAD>" / "<BOS>" / "<EOS>", a leading U+2581 as one
+ * space); a sentence's text is its pieces back to back without the leading space of its first piece.  Text i =
+ * out[out_offsets[i], out_offsets[i+1]), out_offsets has n_sent+1 entries, *out_n = total bytes.  The first call on an
+ * encoder builds its piece table (host work + one upload).  At most 2^32 - 16 ids and sentences per call.
+ * HOST buffers; returns 2 with *out_n = the size needed when out_cap is too small (nothing written). */
+int yttm_dec_run(yttm_enc *enc, const int32_t *ids, const uint64_t *offsets, uint64_t n_sent, const int32_t *ignore,
+                 uint64_t n_ignore, uint8_t *out, uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_n);
+
+/* Same with DEVICE-resident ids[n_ids] and offsets; offsets past n_ids are an error.  *d_out / *d_out_offsets point into
+ * library-owned memory, complete when the call returns and valid until the next yttm_dec_run_device call on the
+ * encoder (yttm_dec_run and the encode calls use other memory, so the ids yttm_enc_run_device returned can be decoded
+ * in place). */
+int yttm_dec_run_device(yttm_enc *enc, const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
+                        const int32_t *ignore, uint64_t n_ignore, const uint8_t **d_out, const uint64_t **d_out_offsets,
                         uint64_t *out_n);
 
 #ifdef __cplusplus

@@ -61,6 +61,16 @@ void yttm_api_result_offsets(void *handle, uint64_t *piece_off, uint64_t *sent_o
 /* yttm.pyx:136-158 decode: one piece per sentence; id_to_subword: one piece; vocab: vocab_size pieces */
 int64_t yttm_api_decode(void *handle, const int32_t *ids, const uint64_t *offsets, uint64_t n_sent,
                         const int32_t *ignore, uint64_t n_ignore);
+/* decode on the GPU (yttm_dec_run of yttm_b200.h): text i = text[text_offsets[i], text_offsets[i+1]); 0 ok, 1 error,
+ * 2 text_cap too small (*total_bytes = size needed, nothing written) */
+int yttm_api_decode_into(void *handle, const int32_t *ids, const uint64_t *offsets, uint64_t n_sent,
+                         const int32_t *ignore, uint64_t n_ignore, uint8_t *text, uint64_t text_cap,
+                         uint64_t *text_offsets, uint64_t *total_bytes);
+/* device-resident ids / offsets and results (pointers into library-owned device memory, valid until the next
+ * decode_device call; not the memory of yttm_api_encode_device's results) */
+int yttm_api_decode_device(void *handle, const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets,
+                           uint64_t n_sent, const int32_t *ignore, uint64_t n_ignore, const uint8_t **d_text,
+                           const uint64_t **d_text_offsets, uint64_t *total_bytes);
 int64_t yttm_api_id_to_subword(void *handle, int id);
 int yttm_api_subword_to_id(void *handle, const char *subword);
 int64_t yttm_api_vocab(void *handle);

@@ -568,6 +568,27 @@ Status BaseEncoder::encode_packed_device(const char *d_bytes, const uint64_t *d_
   return Status();
 }
 
+Status BaseEncoder::decode_packed_into(const int32_t *ids, const uint64_t *offsets, uint64_t n_sent, const int32_t *ignore_ids,
+                                       uint64_t n_ignore, uint8_t *text, uint64_t text_cap, uint64_t *text_offsets,
+                                       uint64_t *total_bytes) const {
+  if (!device_status_.ok()) return device_status_;
+  *total_bytes = 0;
+  int rc = yttm_dec_run(enc_, ids, offsets, n_sent, ignore_ids, n_ignore, text, text_cap, text_offsets, total_bytes);
+  if (rc == 2) return Status(2, "decode_packed_into: output buffer too small");
+  if (rc) return Status(1, ctx_err(ctx_));
+  return Status();
+}
+
+Status BaseEncoder::decode_packed_device(const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
+                                         const int32_t *ignore_ids, uint64_t n_ignore, const uint8_t **d_text,
+                                         const uint64_t **d_text_offsets, uint64_t *total_bytes) const {
+  if (!device_status_.ok()) return device_status_;
+  int rc = yttm_dec_run_device(enc_, d_ids, n_ids, d_offsets, n_sent, ignore_ids, n_ignore, d_text, d_text_offsets,
+                               total_bytes);
+  if (rc) return Status(1, ctx_err(ctx_));
+  return Status();
+}
+
 Status BaseEncoder::encode_as_ids(const std::vector<std::string> &sentences, std::vector<std::vector<int>> *ids,
                                   bool bos, bool eos, bool reverse, double dropout_prob) const {
   std::vector<uint64_t> offs(sentences.size() + 1, 0);

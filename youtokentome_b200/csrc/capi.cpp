@@ -191,6 +191,31 @@ int64_t yttm_api_decode(void *hv, const int32_t *ids, const uint64_t *offsets, u
   return (int64_t)g_res.text.size();
 }
 
+// decode on the GPU into caller-supplied buffers: 0, 1 (error) or 2 (text_cap too small: *total_bytes holds the size
+// needed, nothing written)
+int yttm_api_decode_into(void *hv, const int32_t *ids, const uint64_t *offsets, uint64_t n_sent, const int32_t *ignore,
+                         uint64_t n_ignore, uint8_t *text, uint64_t text_cap, uint64_t *text_offsets, uint64_t *total_bytes) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->decode_packed_into(ids, offsets, n_sent, ignore, n_ignore, text, text_cap, text_offsets, total_bytes);
+  if (st.code == 2) return 2;
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
+// decode of device-resident ids: pointers into library-owned device memory, valid until the next decode_device call on
+// this handle (callers that share a handle between threads copy the result out under their own lock)
+int yttm_api_decode_device(void *hv, const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
+                           const int32_t *ignore, uint64_t n_ignore, const uint8_t **d_text, const uint64_t **d_text_offsets,
+                           uint64_t *total_bytes) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->decode_packed_device(d_ids, n_ids, d_offsets, n_sent, ignore, n_ignore, d_text, d_text_offsets,
+                                           total_bytes);
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
 int64_t yttm_api_id_to_subword(void *hv, int id) {
   auto *h = static_cast<Handle *>(hv);
   std::string piece;

@@ -1,0 +1,33 @@
+// enc_state.cuh — the opened model on the device (struct yttm_enc), shared by encode.cu and decode.cu.
+#pragma once
+#include <vector>
+
+#include "common.cuh"
+
+struct yttm_dec;  // decode state (decode.cu): piece table + per-call buffers, made by the first decode call
+void yttm_dec_free(yttm_dec *d);
+
+struct yttm_enc {
+  yttm_ctx *ctx = nullptr;
+  ytc::DevBuf cp2id, rules;
+  uint32_t rule_mask = 0, space_id = 0;
+  int unk = -1, pad = -1, bos = -1, eos = -1;
+  // host copies of the model tables as yttm_enc_create received them: decode builds its piece table from them
+  std::vector<uint32_t> h_char_cp, h_char_id, h_rules_xyz;
+  uint64_t vocab = 0;  // n_chars + n_rules + special tokens, BaseEncoder::vocab_size
+  yttm_dec *dec = nullptr;
+  // per-call device buffers: two sets, so that the host-buffer entry point can pipeline chunks
+  // (H2D of chunk i+1 and D2H of chunk i-1 overlap the kernels of chunk i)
+  struct Slot {
+    ytc::DevBuf d_bytes, d_offs, slots, ranks, aux, wpos, wsent, nids, out_off, out_ids, counter, longw;
+    ytc::DevBuf dd_tab, dd_rep, dd_list;  // word dedup
+    ytc::DevBuf swb, swc, ntok;            // per-sentence word ranges, per-word id counts
+    void release() {
+      ytc::DevBuf *b[] = {&d_bytes, &d_offs, &slots, &ranks, &aux, &wpos, &wsent, &nids, &out_off, &out_ids, &counter, &longw,
+                          &dd_tab, &dd_rep, &dd_list, &swb, &swc, &ntok};
+      for (auto *x : b) x->release();
+    }
+  } slot[2];
+  cudaStream_t s_in = nullptr, s_out = nullptr;
+  cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
+};

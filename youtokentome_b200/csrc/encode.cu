@@ -24,6 +24,7 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "enc_state.cuh"
 
 using namespace yt;
 
@@ -619,27 +620,6 @@ __global__ void __launch_bounds__(256) add_base_kernel(unsigned long long *__res
 
 }  // namespace
 
-struct yttm_enc {
-  yttm_ctx *ctx = nullptr;
-  ytc::DevBuf cp2id, rules;
-  uint32_t rule_mask = 0, space_id = 0;
-  int unk = -1, pad = -1, bos = -1, eos = -1;
-  // per-call device buffers: two sets, so that the host-buffer entry point can pipeline chunks
-  // (H2D of chunk i+1 and D2H of chunk i-1 overlap the kernels of chunk i)
-  struct Slot {
-    ytc::DevBuf d_bytes, d_offs, slots, ranks, aux, wpos, wsent, nids, out_off, out_ids, counter, longw;
-    ytc::DevBuf dd_tab, dd_rep, dd_list;  // word dedup
-    ytc::DevBuf swb, swc, ntok;            // per-sentence word ranges, per-word id counts
-    void release() {
-      ytc::DevBuf *b[] = {&d_bytes, &d_offs, &slots, &ranks, &aux, &wpos, &wsent, &nids, &out_off, &out_ids, &counter, &longw,
-                          &dd_tab, &dd_rep, &dd_list, &swb, &swc, &ntok};
-      for (auto *x : b) x->release();
-    }
-  } slot[2];
-  cudaStream_t s_in = nullptr, s_out = nullptr;
-  cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-};
-
 namespace {
 
 int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const uint64_t *d_offs, uint64_t n_bytes,
@@ -789,6 +769,10 @@ int yttm_enc_create(yttm_ctx *c, const uint32_t *char_cp, const uint32_t *char_i
     if (char_cp[i] == SPACE_CP) { e->space_id = char_id[i]; have_space = true; }
   }
   if (!have_space) { delete e; YT_FAIL(c, "model: U+2581 missing from char2id"); }
+  e->h_char_cp.assign(char_cp, char_cp + n_chars);
+  e->h_char_id.assign(char_id, char_id + n_chars);
+  e->h_rules_xyz.assign(rules_xyz, rules_xyz + 3 * n_rules);
+  e->vocab = n_chars + n_rules + (unk_id != -1) + (pad_id != -1) + (bos_id != -1) + (eos_id != -1);
   // 2 slots per rule of the open-addressed rule table (load <= 1/2, the measured configuration); most adjacent token
   // pairs have NO rule, and an unsuccessful linear-probe search costs ~2.5 probes at load 1/2, each probe a dependent
   // 16-byte load.
@@ -823,6 +807,7 @@ void yttm_enc_destroy(yttm_enc *e) {
   cudaSetDevice(e->ctx->device);
   e->cp2id.release();
   e->rules.release();
+  yttm_dec_free(e->dec);
   for (int i = 0; i < 2; i++) {
     e->slot[i].release();
     if (e->ev_in[i]) cudaEventDestroy(e->ev_in[i]);

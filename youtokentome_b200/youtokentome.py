@@ -1,8 +1,8 @@
 """The reference's Python surface (youtokentome/youtokentome.py:1-99 + the Cython class
 youtokentome/cpp/yttm.pyx:52-181) over the CUDA library: same class, method names, argument
 meaning, return types and exceptions (ValueError(status.message), TypeError for bad argument
-types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path) and
-`dropout_seed`."""
+types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path), `decode_packed` (its inverse,
+on the GPU) and `dropout_seed`."""
 import ctypes as C
 import threading
 from collections.abc import Collection
@@ -25,6 +25,10 @@ def _pack(sentences):
     if enc:
         np.cumsum([len(b) for b in enc], out=offs[1:])
     return b"".join(enc), offs
+
+
+def _offsets_error(n_ids):  # the library's text for the same error
+    return "decode: offsets must be non-decreasing and lie within the ids (n_ids = %d)" % n_ids
 
 
 class BPE:
@@ -214,6 +218,128 @@ class BPE:
         if need < 0:
             raise self._err()
         return [s[0] for s in self._pieces(need)]
+
+    def decode_packed(self, ids, offsets, ignore_ids: Optional[Collection] = None, out="numpy"):
+        """Additive GPU path of `decode` for a packed batch: sentence i = ids[offsets[i]:offsets[i+1]] (absolute
+        indices, offsets[0] need not be 0).  `ids`: int32 / int64 numpy array or torch tensor (CPU or CUDA);
+        `offsets`: uint64 / int64 array or tensor.  Returns (text_bytes uint8, text_offsets), text i =
+        text_bytes[text_offsets[i]:text_offsets[i+1]] as UTF-8, the same text as decode(); as
+          out="numpy"  numpy uint8 + uint64 arrays,
+          out="torch"  CPU torch tensors (uint8 + int64),
+          out="cuda"   CUDA torch tensors: ids uploaded if needed, results stay on the device."""
+        if out not in ("numpy", "torch", "cuda"):
+            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+        if not isinstance(ignore_ids, Collection) and ignore_ids is not None:
+            raise TypeError("{} is not a Collection instance".format(type(ignore_ids)))
+        ignore = sorted({int(i) for i in ignore_ids}) if ignore_ids else []
+        is_torch = type(ids).__module__.startswith("torch")
+        if out == "cuda" or (is_torch and ids.is_cuda):
+            return self._decode_device(ids, offsets, ignore, out)
+        ids = ids.numpy() if is_torch else np.asarray(ids)
+        if type(offsets).__module__.startswith("torch"):
+            offsets = offsets.cpu().numpy()
+        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
+        n = len(offsets) - 1
+        if n < 0:
+            raise ValueError("offsets must hold at least one value")
+        if int(offsets[-1]) > len(ids):
+            raise ValueError(_offsets_error(len(ids)))
+        ids, extra = self._ids_int32(ids, lambda: offsets, ignore, np)
+        ign = np.asarray([i for i in ignore if -2**31 <= i < 2**31] + extra, dtype=np.int32)
+        L = _lib.lib()
+        total = C.c_uint64(0)
+        cap = 8 * (int(offsets[-1]) - int(offsets[0])) + 64   # a first guess; the exact size on return code 2
+        for _ in range(2):
+            text = np.empty(max(cap, 1), dtype=np.uint8)
+            oo = np.empty(n + 1, dtype=np.uint64)
+            rc = L.yttm_api_decode_into(self._h, ids.ctypes.data, offsets.ctypes.data, n, ign.ctypes.data, len(ign),
+                                        text.ctypes.data, cap, oo.ctypes.data, C.byref(total))
+            if rc != 2:
+                break
+            cap = total.value
+        if rc != 0:
+            raise self._err()
+        text = text[:total.value]
+        if out == "torch":
+            import torch
+            return torch.from_numpy(text), torch.from_numpy(oo.astype(np.int64))
+        return text, oo
+
+    def _ids_int32(self, ids, offsets, ignore, xp):
+        """ids as contiguous int32 (numpy, or torch on the ids' device) + values to add to the ignore list.  A value
+        that does not fit in int32 is never truncated: if one is decoded (not ignored), the first invalid id of the
+        batch raises decode's ValueError here; ignored ones become -1, which is then ignored as well.  `offsets()`
+        gives the offsets as numpy uint64 (only needed on that rare path)."""
+        if xp is np:
+            if ids.dtype.kind not in "iu":
+                raise TypeError("ids must be an integer array, not %s" % ids.dtype)
+            if ids.dtype == np.int32:
+                return np.ascontiguousarray(ids), []
+            big = (ids < -2**31) | (ids > 2**31 - 1)
+            if not big.any():
+                return np.ascontiguousarray(ids.astype(np.int32)), []
+            host = ids
+        else:
+            import torch
+            if ids.dtype == torch.int32:
+                return ids.contiguous(), []
+            if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+                raise TypeError("ids must be an integer tensor, not %s" % ids.dtype)
+            ids = ids.to(torch.int64)
+            big = (ids < -2**31) | (ids > 2**31 - 1)
+            if not bool(big.any()):
+                return ids.to(torch.int32).contiguous(), []
+            host = ids.cpu().numpy()
+        offs = np.asarray(offsets(), dtype=np.uint64)
+        lo, hi = int(offs[0]), int(offs[-1])
+        if np.any(offs[1:] < offs[:-1]) or hi > len(host):
+            raise ValueError(_offsets_error(len(host)))
+        seen = np.asarray(host[lo:hi], dtype=np.int64)
+        V = self.vocab_size()
+        bad = np.flatnonzero(((seen < 0) | (seen >= V)) & ~np.isin(seen, np.asarray(ignore, dtype=np.int64)))
+        if len(bad):
+            raise ValueError("id must be in the range [0, vocab_size - 1]. Current value: vocab_size = %d; id=%d;"
+                             % (V, int(seen[bad[0]])))
+        if xp is np:
+            return np.ascontiguousarray(np.where(big, -1, ids).astype(np.int32)), [-1]
+        return torch.where(big, torch.full_like(ids, -1), ids).to(torch.int32).contiguous(), [-1]
+
+    def _decode_device(self, ids, offsets, ignore, out):
+        import torch
+        from .distributed import _DevView
+        L = _lib.lib()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if type(ids).__module__.startswith("torch"):
+            d_ids = ids.to(dev)
+        else:
+            d_ids = torch.from_numpy(np.ascontiguousarray(ids)).to(dev)
+        if type(offsets).__module__.startswith("torch"):
+            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
+        else:
+            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
+        n = d_offs.numel() - 1
+        if n < 0:
+            raise ValueError("offsets must hold at least one value")
+        d_ids, extra = self._ids_int32(d_ids, lambda: d_offs.cpu().numpy().astype(np.uint64), ignore, torch)
+        ign = np.asarray([i for i in ignore if -2**31 <= i < 2**31] + extra, dtype=np.int32)
+        p_text, p_off, total = C.c_void_p(), C.c_void_p(), C.c_uint64(0)
+        torch.cuda.synchronize()   # the library runs on its own stream
+        with self._dev_lock:       # the result pointers are valid until the next decode on this handle: copy under the lock
+            rc = L.yttm_api_decode_device(self._h, d_ids.data_ptr(), d_ids.numel(), d_offs.data_ptr(), n, ign.ctypes.data,
+                                          len(ign), C.byref(p_text), C.byref(p_off), C.byref(total))
+            if rc != 0:
+                raise self._err()
+            if total.value:
+                text = torch.as_tensor(_DevView(p_text.value, total.value, "|u1"), device=dev).clone()
+            else:
+                text = torch.empty(0, dtype=torch.uint8, device=dev)
+            oo = torch.as_tensor(_DevView(p_off.value, n + 1, "<i8"), device=dev).clone()
+            torch.cuda.synchronize()
+        if out == "cuda":
+            return text, oo
+        if out == "torch":
+            return text.cpu(), oo.cpu()
+        return text.cpu().numpy(), oo.cpu().numpy().astype(np.uint64)
 
     # -- BPE-dropout stream ---------------------------------------------------------------------
     def dropout_seed(self, seed: int):
