@@ -52,6 +52,11 @@ def main():
     zc = _cases.zipf()
     long_word = b"".join(zc.sentences(12, 60, seed=6)).replace(b" ", b"")
     sents = _cases.zipf_sentences(150) + list(_cases.EDGE_SENTENCES) + [long_word, b"a" * 700 + b" " + b"a" * 700, long_word + b" x " + long_word]
+    # the word finder stages groups of sentences in 16 KB pieces: a sentence longer than a piece, a group of 1.5 KB
+    # sentences that spills over one; the dedup compares 16 bytes at a time: words of 15 .. 33 bytes, repeated
+    sents += [b" ".join(zc.sentences(300, 70, seed=8))]
+    sents += [b" ".join(zc.sentences(20, 75, seed=9 + k)) for k in range(14)]
+    sents += [b" ".join((long_word[:n] + b" ") * 3 for n in (15, 16, 17, 31, 32, 33)) + long_word[:33]]
     g, o = GpuEncoder(model), orc.encoder(model)
     # long_word and the 700-byte words are longer than 512 slots: they reach the block-per-word kernel
     assert g.encode(sents, bos=True, eos=True) == o.encode(sents, bos=True, eos=True)

@@ -4,10 +4,11 @@
 // 1455-1632) behind yttm_enc_run* of include/yttm_b200.h.  The reference gives each CPU thread a
 // contiguous range of sentences and runs a heap-driven merge loop per word.  Here the batch is
 // one flat byte buffer in HBM and the unit of parallel work is the WORD:
-//   find_words_vec_kernel       warp per 4 sentences: word starts (on raw bytes, see bpe_core.cuh) go to a global
-//                               work list in byte order; every sentence records its range of work items
+//   find_words_vec_kernel       block per group of sentences staged in shared memory: word starts (on raw bytes, see
+//                               bpe_core.cuh) go to a global work list in byte order, one reservation per group;
+//                               every sentence records its range of work items
 //   dropout = 0 (the ids of a word are a function of its bytes, so every distinct word is encoded once):
-//     dedup_words_kernel        elects one representative occurrence per distinct word
+//     dedup_words_kernel        elects one representative occurrence per distinct word (16-byte vector loads)
 //     encode_rep_words_kernel   one thread per representative: UTF-8 decode -> char ids (unknown runs collapse to
 //                               one pseudo token, bpe.cpp:1513-1533) -> min-rank merge loop, leftmost first
 //                               (MergeEvent2::operator< bpe.cpp:1475-1478)
@@ -75,30 +76,42 @@ struct EncArgs {
 // [base + 1 + rel ..], the slots base and base + len + 2 stay unused.
 __device__ __forceinline__ uint64_t sent_base(uint64_t start, uint64_t s) { return start + 3 * s; }
 
-// Word starts, FIND_SPW sentences per warp and round.  Pass 1 counts the word starts of each sentence, one atomicAdd
-// per BLOCK and round reserves a contiguous range of the work list (a single counter hammered once per warp was a
-// bottleneck), pass 2 writes the entries in byte order and every sentence's range of work items.  A lane owns FOUR
-// consecutive bytes - one aligned 32-bit load - and decides the word starts on a 12-byte register window (previous /
-// own / next word, the neighbours' by shuffle); the 4-bit flags of the first FIND_VEC_CACHE / FIND_SPW 128-byte chunks
-// of every sentence stay in one register for the write pass.  word_start_at(p) == space_before(p) && !space_at(p) on
-// raw bytes (a continuation byte is never a space), and the text bounds become sentinel bytes: 0x20 before the sentence
-// (space_before(lo) is true; E2 96 81 cannot match across lo), 0x00 at and after its end (E2 96 81 cannot match across hi).
-constexpr int FIND_VEC_CACHE = 8;
-// the four bytes at batch positions p .. p+3 (p may be negative or reach past the batch), sentinels applied
-__device__ __forceinline__ uint32_t find_vec_word(const uint8_t *s, int64_t p, int64_t lo, int64_t hi, int64_t n_total) {
-  if (p + 4 <= lo) return 0x20202020u;
-  if (p >= hi) return 0u;
-  uint32_t w = 0;
-  if (p >= 0 && p + 4 <= n_total) w = *reinterpret_cast<const uint32_t *>(s + p);  // p is address-aligned by construction
-  else
-    for (int k = 0; k < 4; k++)
-      if (p + k >= 0 && p + k < n_total) w |= (uint32_t)s[p + k] << (8 * k);
-  if (p < lo || p + 4 > hi)
-    for (int k = 0; k < 4; k++) {
-      if (p + k < lo) w = (w & ~(0xffu << (8 * k))) | (0x20u << (8 * k));
-      else if (p + k >= hi) w &= ~(0xffu << (8 * k));
-    }
-  return w;
+// exclusive sum of one value per thread over the block; *tot = block sum (starts with a barrier, so s_red may be reused
+// right after the previous call)
+__device__ __forceinline__ uint32_t long_block_scan_sum(uint32_t v, uint32_t *s_red, uint32_t *tot) {
+  const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  uint32_t x = v;
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if ((int)lane >= o) x += y; }
+  __syncthreads();
+  if (lane == 31) s_red[wid] = x;
+  __syncthreads();
+  uint32_t base = 0, all = 0;
+  for (unsigned i = 0; i < nw; i++) { const uint32_t w = s_red[i]; if (i < wid) base += w; all += w; }
+  *tot = all;
+  return base + x - v;
+}
+
+// Word starts: one block per GROUP of G consecutive sentences (G from the batch's mean sentence length, so that a
+// typical group fits one FIND_TILE-byte piece).  The block stages the group's bytes in shared memory with aligned
+// 16-byte loads (every byte is read from HBM once), each thread decides the word starts of FIND_BPT consecutive staged
+// bytes, one block-wide scan numbers them in byte order and ONE atomicAdd per group reserves the group's range of the
+// work list, so the words of every sentence are a contiguous run of work items.  A group longer than a piece (long
+// sentences) is streamed piece by piece twice: count, reserve, write.  word_start_at(p) == space_before(p) &&
+// !space_at(p) on raw bytes (a continuation byte is never a space); the sentence bounds inside a group come from a
+// shared bitmap of sentence starts: a sentence start is always preceded by a space, and an E2 96 81 across a sentence
+// start is a space unit on neither side.  The group's first byte and its end are sentence starts of the bitmap, so the
+// bytes outside the group decide nothing and no halo from neighbouring groups is needed.
+constexpr int FIND_T = 256;                   // threads per block
+constexpr int FIND_BPT = 64;                  // bytes per thread and piece (one 64-bit mask)
+constexpr int FIND_TILE = FIND_T * FIND_BPT;  // bytes per piece (16 KB)
+constexpr int FIND_HALO = 16;                 // staged bytes on either side of a piece (the rules look 3 back, 2 ahead)
+constexpr int FIND_BUF = FIND_TILE + 2 * FIND_HALO;
+constexpr uint32_t FIND_GMAX = 256;           // sentences per group at most
+static_assert(FIND_BPT == 64 && FIND_HALO % 32 == 16, "a thread's 64 bitmap bits start at bit 16 of a bitmap word");
+// set bits / lowest set bit (m != 0) of a thread's 64-bit mask, from the 32-bit intrinsics
+__device__ __forceinline__ uint32_t find_popc64(uint64_t m) { return __popc((uint32_t)m) + __popc((uint32_t)(m >> 32)); }
+__device__ __forceinline__ int find_low64(uint64_t m) {
+  return (uint32_t)m ? __ffs((int)(uint32_t)m) - 1 : 31 + __ffs((int)(uint32_t)(m >> 32));
 }
 // SWAR helpers on four bytes at once: high bit of every byte that is an ASCII space (0x20 or 0x09..0x0d) / equals v
 __device__ __forceinline__ uint32_t swar_eq(uint32_t w, uint32_t v4) {
@@ -114,108 +127,157 @@ __device__ __forceinline__ uint32_t swar_mask4(uint32_t hi) {  // 0x80 bits of f
   const uint32_t m = hi >> 7;
   return (m | (m >> 7) | (m >> 14) | (m >> 21)) & 15u;
 }
-// word-start flags (bit k = byte p + k) of the lane's four bytes
-__device__ __forceinline__ uint32_t find_vec_flags(const uint8_t *s, int64_t p, int64_t lo, int64_t hi, int64_t n_total,
-                                                   unsigned lane) {
-  const uint32_t c = find_vec_word(s, p, lo, hi, n_total);
-  uint32_t pv = __shfl_up_sync(0xffffffffu, c, 1), nx = __shfl_down_sync(0xffffffffu, c, 1);
-  if (lane == 0) pv = find_vec_word(s, p - 4, lo, hi, n_total);
-  if (lane == 31) nx = find_vec_word(s, p + 4, lo, hi, n_total);
-  uint32_t inside = 15u;   // bytes of this lane that belong to the sentence
-  if (p < lo) inside &= lo - p >= 4 ? 0u : 15u << (uint32_t)(lo - p);
-  if (p + 4 > hi) inside &= hi <= p ? 0u : 15u >> (uint32_t)(p + 4 - hi);
-  if (!((swar_eq(pv, 0xe2e2e2e2u) | swar_eq(c, 0xe2e2e2e2u) | swar_eq(nx, 0xe2e2e2e2u)) & 0x80808080u)) {
-    // fast path (no 0xE2 within four bytes either side, so no U+2581 can touch these positions): a word starts where an
-    // ASCII space (or the sentinel in front of the sentence) is followed by a non-space byte
-    const uint32_t sp = swar_mask4(swar_space(c)), sp_prev = swar_mask4(swar_space(pv)) >> 3;
-    return ((sp << 1) | sp_prev) & ~sp & inside & 15u;
-  }
-  const uint64_t X = (uint64_t)pv | ((uint64_t)c << 32), Y = (uint64_t)c | ((uint64_t)nx << 32);  // bytes p-4 .. p+3, p .. p+7
-  uint32_t f = 0;
-#pragma unroll
-  for (int k = 0; k < 4; k++) {
-    const uint32_t t = (uint32_t)(X >> (8 * (1 + k))), u = (uint32_t)(Y >> (8 * k));  // t: bytes p+k-3 .., u: bytes p+k ..
-    const bool before = is_space_byte((uint8_t)(t >> 16)) || (t & 0xffffffu) == 0x8196e2u;
-    const bool at = is_space_byte((uint8_t)u) || (u & 0xffffffu) == 0x8196e2u;
-    if (before && !at) f |= 1u << k;
-  }
-  return f & inside;
+// staged byte i: is it a space unit / does a space unit end right before it (sentence starts from the bitmap sb)
+__device__ __forceinline__ bool find_sbit(const uint32_t *sb, int i) { return (sb[i >> 5] >> (i & 31)) & 1u; }
+__device__ __forceinline__ bool find_at(const uint8_t *b, const uint32_t *sb, int i) {
+  return is_space_byte(b[i]) ||
+         (b[i] == 0xe2 && b[i + 1] == 0x96 && b[i + 2] == 0x81 && !find_sbit(sb, i + 1) && !find_sbit(sb, i + 2));
 }
-constexpr int FIND_SPW = 4;  // sentences per warp and round: one work-list reservation (atomic) per 32 sentences
-// (at least 4 blocks per SM, the occupancy it is measured at: left free, ptxas moves the counts to local memory)
-__global__ void __launch_bounds__(256, 4) find_words_vec_kernel(EncArgs a) {
-  __shared__ unsigned long long s_cnt[8 * FIND_SPW], s_base;
-  const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+__device__ __forceinline__ bool find_before(const uint8_t *b, const uint32_t *sb, int i) {
+  return find_sbit(sb, i) || is_space_byte(b[i - 1]) ||
+         (b[i - 3] == 0xe2 && b[i - 2] == 0x96 && b[i - 1] == 0x81 && !find_sbit(sb, i - 2) && !find_sbit(sb, i - 1));
+}
+
+// Stages the piece [pa, pa + FIND_TILE) of the group [gstart, gend), FIND_HALO bytes on either side (the address of
+// batch byte pa is 16-byte aligned), and the bitmap of the sentence starts among them; returns the word starts among
+// the thread's FIND_BPT bytes (bit j = batch byte pa + FIND_BPT * threadIdx.x + j).  Starts with a barrier: the
+// previous piece is done with the buffers.
+__device__ __forceinline__ uint64_t find_piece(const uint8_t *bytes, int64_t n_total, int64_t pa, int64_t gstart,
+                                               int64_t gend, const uint32_t *s_off, uint32_t ng, uint4 *s_buf,
+                                               uint32_t *s_sb) {
+  constexpr int NCH = FIND_BUF / 16, PER = (NCH + FIND_T - 1) / FIND_T;
+  const int64_t p0 = pa - FIND_HALO;  // batch position of staged byte 0
+  const int tid = (int)threadIdx.x;
+  __syncthreads();
+  uint4 v[PER];
+#pragma unroll
+  for (int r = 0; r < PER; r++) {  // every load first: PER 16-byte loads in flight per thread
+    const int j = tid + r * FIND_T;
+    const int64_t q = p0 + 16 * (int64_t)j;
+    v[r] = make_uint4(0u, 0u, 0u, 0u);
+    if (j < NCH && q + 16 > gstart && q < gend) {  // only chunks holding bytes of the group
+      if (q >= 0 && q + 16 <= n_total) {
+        v[r] = *reinterpret_cast<const uint4 *>(bytes + q);
+      } else {  // a chunk over an end of the batch: byte by byte, never outside it
+        uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
+#pragma unroll
+        for (int k = 0; k < 16; k++)
+          if (q + k >= 0 && q + k < n_total) {
+            const uint32_t b = (uint32_t)bytes[q + k] << (8 * (k & 3));
+            if (k < 4) w0 |= b; else if (k < 8) w1 |= b; else if (k < 12) w2 |= b; else w3 |= b;
+          }
+        v[r] = make_uint4(w0, w1, w2, w3);
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < PER; r++)
+    if (tid + r * FIND_T < NCH) s_buf[tid + r * FIND_T] = v[r];
+  for (int j = tid; j < FIND_BUF / 32 + 1; j += FIND_T) s_sb[j] = 0u;
+  __syncthreads();
+  for (uint32_t i = (uint32_t)tid; i <= ng; i += FIND_T) {
+    const int64_t x = (int64_t)s_off[i] - p0;
+    if (x >= 0 && x < FIND_BUF) atomicOr(s_sb + (x >> 5), 1u << (x & 31));
+  }
+  __syncthreads();
+  const int64_t lo = pa + FIND_BPT * (int64_t)tid;  // batch position of the thread's first byte
+  const int64_t b = gstart - lo, e = gend - lo;    // the group's bytes among the thread's: [bb, ee)
+  const int bb = b < 0 ? 0 : b > FIND_BPT ? FIND_BPT : (int)b, ee = e < 0 ? 0 : e > FIND_BPT ? FIND_BPT : (int)e;
+  if (ee <= bb) return 0;
+  const uint64_t inside = (ee - bb == 64 ? ~0ull : (1ull << (ee - bb)) - 1) << bb;
+  const int i0 = FIND_HALO + FIND_BPT * tid;  // staged index of the thread's first byte
+  const uint32_t prev = reinterpret_cast<const uint32_t *>(s_buf)[i0 / 4 - 1];
+  uint32_t e2 = swar_eq(prev, 0xe2e2e2e2u);
+  uint64_t sp = 0;
+#pragma unroll
+  for (int k = 0; k < FIND_BPT / 16; k++) {
+    const uint4 c = s_buf[i0 / 16 + k];
+    e2 |= swar_eq(c.x, 0xe2e2e2e2u) | swar_eq(c.y, 0xe2e2e2e2u) | swar_eq(c.z, 0xe2e2e2e2u) | swar_eq(c.w, 0xe2e2e2e2u);
+    sp |= (uint64_t)(swar_mask4(swar_space(c.x)) | swar_mask4(swar_space(c.y)) << 4 | swar_mask4(swar_space(c.z)) << 8 |
+                     swar_mask4(swar_space(c.w)) << 12) << (16 * k);
+  }
+  if (!(e2 & 0x80808080u)) {
+    // no 0xE2 from four bytes before on, so no U+2581 touches these bytes: a word starts where a sentence starts or an
+    // ASCII space is followed by a non-space byte
+    const uint32_t *sw = s_sb + (i0 >> 5);
+    const uint64_t starts = (uint64_t)(sw[0] >> 16) | ((uint64_t)sw[1] << 16) | ((uint64_t)sw[2] << 48);
+    return (starts | (sp << 1) | (swar_space(prev) >> 31)) & ~sp & inside;
+  }
+  const uint8_t *sbyte = reinterpret_cast<const uint8_t *>(s_buf);
+  uint64_t f = 0;
+  for (int j = bb; j < ee; j++)
+    if (find_before(sbyte, s_sb, i0 + j) && !find_at(sbyte, s_sb, i0 + j)) f |= 1ull << j;
+  return f;
+}
+
+// (4 blocks of 256 threads per SM, the occupancy it is built for: 2 x 16 KB of staged bytes per SM in flight)
+__global__ void __launch_bounds__(FIND_T, 4) find_words_vec_kernel(EncArgs a, uint32_t G) {
+  __shared__ uint4 s_buf[FIND_BUF / 16];
+  __shared__ uint32_t s_sb[FIND_BUF / 32 + 1];
+  __shared__ uint32_t s_off[FIND_GMAX + 1];  // the group's sentence starts (batch positions), s_off[ng] = its end
+  __shared__ uint32_t s_wb[FIND_GMAX + 1];   // words of the group in front of them
+  __shared__ uint32_t s_red[FIND_T / 32];
+  __shared__ unsigned long long s_base;
+  constexpr int64_t FAR = (int64_t)1 << 62;
+  const int tid = (int)threadIdx.x;
   const uint64_t o0 = a.offs[0];
   const int64_t n_total = (int64_t)(a.offs[a.n_sent] - o0);
-  const int64_t mis = (int64_t)(reinterpret_cast<uintptr_t>(a.bytes) & 3u);
-  constexpr uint64_t PER_ROUND = 8 * FIND_SPW;
-  for (uint64_t g = (uint64_t)blockIdx.x * PER_ROUND; g < a.n_sent; g += (uint64_t)gridDim.x * PER_ROUND) {  // block-uniform
-    int64_t lo[FIND_SPW], hi[FIND_SPW], start[FIND_SPW];
-    uint32_t cnt[FIND_SPW];
-    uint32_t cache = 0;  // flags of the first FIND_VEC_CACHE / FIND_SPW chunks of every sentence, 4 bits per chunk
-    constexpr int CPS = FIND_VEC_CACHE / FIND_SPW;  // cached chunks per sentence (2: a 128-byte sentence spans at most 2)
-#pragma unroll
-    for (int q = 0; q < FIND_SPW; q++) {
-      const uint64_t s = g + (uint64_t)wid * FIND_SPW + q;
-      lo[q] = hi[q] = start[q] = 0;
-      cnt[q] = 0;
-      if (s < a.n_sent) {  // warp-uniform
-        lo[q] = (int64_t)(a.offs[s] - o0);
-        hi[q] = (int64_t)(a.offs[s + 1] - o0);
-        start[q] = lo[q] - ((lo[q] + mis) & 3);  // the address of batch byte `start` is 4-byte aligned
-        uint32_t mine = 0;
-        int j = 0;
-        for (int64_t pw = start[q]; pw < hi[q]; pw += 128, j++) {  // warp-uniform
-          const uint32_t f = find_vec_flags(a.bytes, pw + 4 * lane, lo[q], hi[q], n_total, lane);
-          if (j < CPS) cache |= f << (4 * (q * CPS + j));
-          mine += __popc(f);
-        }
-        for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
-        cnt[q] = mine;
+  const int64_t mis = (int64_t)(reinterpret_cast<uintptr_t>(a.bytes) & 15u);
+  for (uint64_t g = (uint64_t)blockIdx.x * G; g < a.n_sent; g += (uint64_t)gridDim.x * G) {  // block-uniform
+    const uint32_t ng = (uint32_t)min((uint64_t)G, a.n_sent - g);
+    __syncthreads();  // the previous group is done with s_off / s_wb / s_base
+    for (uint32_t i = (uint32_t)tid; i <= ng; i += FIND_T) s_off[i] = (uint32_t)(a.offs[g + i] - o0);
+    __syncthreads();
+    const int64_t gstart = s_off[0], gend = s_off[ng];
+    const int64_t a0 = gstart - ((gstart + mis) & 15);  // the address of batch byte a0 is 16-byte aligned
+    const uint32_t np = gend - a0 > FIND_TILE ? (uint32_t)((gend - a0 + FIND_TILE - 1) / FIND_TILE) : 1u;
+    uint32_t tot;
+    if (np > 1) {  // a group longer than a piece: count, then reserve before the write pass
+      uint32_t total = 0;
+      for (uint32_t k = 0; k < np; k++) {
+        const uint64_t m = find_piece(a.bytes, n_total, a0 + (int64_t)k * FIND_TILE, gstart, gend, s_off, ng, s_buf, s_sb);
+        long_block_scan_sum(find_popc64(m), s_red, &tot);
+        total += tot;
       }
-      if (lane == 0) s_cnt[wid * FIND_SPW + q] = cnt[q];
+      if (tid == 0) s_base = total ? atomicAdd(a.n_words, (unsigned long long)total) : 0ull;
+    }
+    uint32_t run = 0;  // words of the group in the earlier pieces
+    for (uint32_t k = 0; k < np; k++) {
+      const int64_t pa = a0 + (int64_t)k * FIND_TILE;
+      uint64_t m = find_piece(a.bytes, n_total, pa, gstart, gend, s_off, ng, s_buf, s_sb);
+      uint32_t n = run + long_block_scan_sum(find_popc64(m), s_red, &tot);  // words of the group before mine
+      if (np == 1) {
+        if (tid == 0) s_base = tot ? atomicAdd(a.n_words, (unsigned long long)tot) : 0ull;
+        __syncthreads();
+      }
+      const unsigned long long base = s_base;
+      // the thread's bytes in order: a sentence start among them records the words in front of it, a word belongs to
+      // the sentence of the last start at or before it (the last thread of the last piece also takes the group's end)
+      const int64_t lo = pa + FIND_BPT * (int64_t)tid;
+      const int64_t lim = k + 1 == np && tid == FIND_T - 1 ? FAR : lo + FIND_BPT;
+      uint32_t i = 0, r = ng + 1;  // i = first sentence start at or after lo
+      while (i < r) {
+        const uint32_t mid = (i + r) >> 1;
+        if ((int64_t)s_off[mid] < lo) i = mid + 1; else r = mid;
+      }
+      while (true) {
+        const int64_t x = i <= ng ? (int64_t)s_off[i] : FAR;
+        const int64_t p = m ? lo + find_low64(m) : FAR;
+        if (x < lim && x <= p) { s_wb[i++] = n; continue; }
+        if (!m) break;
+        a.word_pos[base + n] = (uint32_t)p;
+        a.word_sent[base + n] = (uint32_t)(g + i - 1);
+        n++;
+        m &= m - 1;
+      }
+      run += tot;
     }
     __syncthreads();
-    if (wid == 0) {  // exclusive prefix of the 32 sentence counts + ONE reservation for the round
-      const unsigned long long c = s_cnt[lane];
-      unsigned long long x = c;
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-        if ((int)lane >= o) x += y;
-      }
-      s_cnt[lane] = x - c;
-      if (lane == 31) s_base = x ? atomicAdd(a.n_words, x) : 0ull;
+    const unsigned long long base = s_base;
+    for (uint32_t i = (uint32_t)tid; i < ng; i += FIND_T) {
+      a.sent_wbase[g + i] = (uint32_t)(base + s_wb[i]);
+      a.sent_wcnt[g + i] = s_wb[i + 1] - s_wb[i];
     }
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < FIND_SPW; q++) {
-      const uint64_t s = g + (uint64_t)wid * FIND_SPW + q;
-      if (s >= a.n_sent) continue;  // warp-uniform
-      unsigned long long idx = s_base + s_cnt[wid * FIND_SPW + q];
-      if (lane == 0) { a.sent_wbase[s] = (uint32_t)idx; a.sent_wcnt[s] = cnt[q]; }
-      if (!cnt[q]) continue;
-      const unsigned below = (1u << lane) - 1u;
-      int j = 0;
-      for (int64_t pw = start[q]; pw < hi[q]; pw += 128, j++) {
-        const int64_t p = pw + 4 * lane;
-        const uint32_t f = j < CPS ? (cache >> (4 * (q * CPS + j))) & 15u : find_vec_flags(a.bytes, p, lo[q], hi[q], n_total, lane);
-        const unsigned b0 = __ballot_sync(0xffffffffu, f & 1u), b1 = __ballot_sync(0xffffffffu, f & 2u),
-                       b2 = __ballot_sync(0xffffffffu, f & 4u), b3 = __ballot_sync(0xffffffffu, f & 8u);
-        // byte order: a lane's index = words in earlier lanes (all four bits) + its own lower bits
-        const unsigned all_below = __popc(b0 & below) + __popc(b1 & below) + __popc(b2 & below) + __popc(b3 & below);
-        unsigned long long i = idx + all_below;
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-          if ((f >> k) & 1u) {
-            a.word_pos[i] = (uint32_t)(p + k);
-            a.word_sent[i] = (uint32_t)s;
-            i++;
-          }
-        idx += __popc(b0) + __popc(b1) + __popc(b2) + __popc(b3);
-      }
-    }
-    __syncthreads();  // s_cnt / s_base are reused by the next round
   }
 }
 
@@ -286,19 +348,7 @@ __device__ __forceinline__ uint32_t long_block_min(uint32_t v, uint32_t *s_red) 
   for (unsigned i = 1; i < (blockDim.x >> 5); i++) r = min(r, s_red[i]);
   return r;
 }
-// exclusive sum and inclusive max of one value per thread over the block; *tot = block sum / block max
-__device__ __forceinline__ uint32_t long_block_scan_sum(uint32_t v, uint32_t *s_red, uint32_t *tot) {
-  const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  uint32_t x = v;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if ((int)lane >= o) x += y; }
-  __syncthreads();
-  if (lane == 31) s_red[wid] = x;
-  __syncthreads();
-  uint32_t base = 0, all = 0;
-  for (unsigned i = 0; i < nw; i++) { const uint32_t w = s_red[i]; if (i < wid) base += w; all += w; }
-  *tot = all;
-  return base + x - v;
-}
+// inclusive max of one value per thread over the block (long_block_scan_sum, above, is the exclusive sum)
 __device__ __forceinline__ uint32_t long_block_scan_max(uint32_t v, uint32_t *s_red) {
   const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   uint32_t x = v;
@@ -442,7 +492,7 @@ __global__ void __launch_bounds__(LONG_T) encode_long_words_kernel(EncArgs a, Lo
 // first byte of a space unit (never a continuation byte), INVALID_CP with length 1 in both cases (decode_unit), so
 // nothing outside the word enters.  Natural text repeats its words (the bench batch: 20 M occurrences of < 200 k
 // words), and the merge loop of encode_word is the expensive part of encoding a word.  Three launches:
-//   dedup_words_kernel       one thread per occurrence: end of the word + 64-bit FNV-1a/mix64 hash of its bytes; an
+//   dedup_words_kernel       one thread per occurrence: end of the word + 64-bit hash of its bytes; an
 //                            open-addressed table of (32-bit tag, work item) words, small enough to stay in L2, elects
 //                            the first occurrence that claims a slot as the word's representative; later occurrences
 //                            with the same tag compare BYTES with it (exactness never rests on the hash).  A word that
@@ -465,19 +515,95 @@ struct DedupArgs {
   uint32_t weak_tag;           // tests only: all tags equal, so every probe ends in the byte compare
 };
 
+// The words' bytes are read 16 at a time: aligned 16-byte loads (lanes whose words are neighbours share their lines)
+// and a shift that lines the bytes up, never a byte-serial gather.
+struct Chunk16 { uint64_t lo, hi; };  // 16 bytes, little-endian
+// the 16 bytes from batch position q (the address of byte q is 16-byte aligned); bytes outside the batch read as 0
+__device__ __forceinline__ Chunk16 dd_chunk(const uint8_t *s, int64_t q, int64_t n_total) {
+  if (q >= 0 && q + 16 <= n_total) {
+    const uint4 v = *reinterpret_cast<const uint4 *>(s + q);
+    return Chunk16{v.x | (uint64_t)v.y << 32, v.z | (uint64_t)v.w << 32};
+  }
+  Chunk16 c{0, 0};  // a chunk over an end of the batch: byte by byte, never outside it
+#pragma unroll
+  for (int k = 0; k < 16; k++)
+    if (q + k >= 0 && q + k < n_total) {
+      if (k < 8) c.lo |= (uint64_t)s[q + k] << (8 * k);
+      else c.hi |= (uint64_t)s[q + k] << (8 * (k - 8));
+    }
+  return c;
+}
+// bytes o .. o + n - 1 of the 32 bytes c0:c1 (o < 16, 1 <= n <= 16), zero above
+__device__ __forceinline__ Chunk16 dd_shift(Chunk16 c0, Chunk16 c1, uint32_t o, uint32_t n) {
+  const uint64_t x0 = o >= 8 ? c0.hi : c0.lo, x1 = o >= 8 ? c1.lo : c0.hi, x2 = o >= 8 ? c1.hi : c1.lo;
+  const uint32_t s = 8 * (o & 7);
+  Chunk16 r = s ? Chunk16{(x0 >> s) | (x1 << (64 - s)), (x1 >> s) | (x2 << (64 - s))} : Chunk16{x0, x1};
+  if (n <= 8) { r.hi = 0; if (n < 8) r.lo &= (1ull << (8 * n)) - 1; }
+  else if (n < 16) r.hi &= (1ull << (8 * (n - 8))) - 1;
+  return r;
+}
+// the n (1 .. 16) bytes at batch position p; mis = address of the batch & 15
+__device__ __forceinline__ Chunk16 dd_window(const uint8_t *s, int64_t p, uint32_t n, int64_t n_total, int64_t mis) {
+  const uint32_t o = (uint32_t)((p + mis) & 15);
+  const Chunk16 c0 = dd_chunk(s, p - o, n_total);
+  const Chunk16 c1 = o + n > 16 ? dd_chunk(s, p - o + 16, n_total) : Chunk16{0, 0};
+  return dd_shift(c0, c1, o, n);
+}
+// 16-bit masks of the bytes of a chunk that are ASCII spaces / equal a given byte (v4 = the byte four times)
+__device__ __forceinline__ uint32_t dd_space16(Chunk16 c) {
+  return swar_mask4(swar_space((uint32_t)c.lo)) | swar_mask4(swar_space((uint32_t)(c.lo >> 32))) << 4 |
+         swar_mask4(swar_space((uint32_t)c.hi)) << 8 | swar_mask4(swar_space((uint32_t)(c.hi >> 32))) << 12;
+}
+__device__ __forceinline__ uint32_t dd_eq16(Chunk16 c, uint32_t v4) {
+  return swar_mask4(swar_eq((uint32_t)c.lo, v4)) | swar_mask4(swar_eq((uint32_t)(c.lo >> 32), v4)) << 4 |
+         swar_mask4(swar_eq((uint32_t)c.hi, v4)) << 8 | swar_mask4(swar_eq((uint32_t)(c.hi >> 32), v4)) << 12;
+}
+__device__ __forceinline__ uint64_t dd_rotl(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
+
 __global__ void __launch_bounds__(128) dedup_words_kernel(EncArgs a, uint64_t n_words, DedupArgs d) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t o0 = a.offs[0];
+  const int64_t n_total = (int64_t)(a.offs[a.n_sent] - o0);
+  const int64_t mis = (int64_t)(reinterpret_cast<uintptr_t>(a.bytes) & 15u);
   for (uint64_t w0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); w0 < n_words; w0 += stride) {  // warp-uniform
     const uint64_t w = w0 + lane;
     bool is_rep = false;
     if (w < n_words) {
-      const uint64_t p0 = a.word_pos[w], hi = a.offs[(uint64_t)a.word_sent[w] + 1] - o0;
-      uint64_t q = p0, h = 0xcbf29ce484222325ull;
+      const int64_t p0 = a.word_pos[w], hi = (int64_t)(a.offs[(uint64_t)a.word_sent[w] + 1] - o0);
       uint32_t l;
-      while (q < hi && !space_at(a.bytes, q, hi, &l)) { h = (h ^ a.bytes[q]) * 0x100000001b3ull; q++; }
-      const uint64_t len = q - p0;
+      // ---- end of the word: the first space unit at or after p0, or hi; its first 3 chunks stay in registers
+      const uint32_t o = (uint32_t)((p0 + mis) & 15);
+      Chunk16 c0{0, 0}, c1{0, 0}, c2{0, 0};
+      int64_t end = hi;
+      for (int64_t q = p0 - o, k = 0; q < hi; q += 16, k++) {
+        const Chunk16 c = dd_chunk(a.bytes, q, n_total);
+        if (k == 0) c0 = c; else if (k == 1) c1 = c; else if (k == 2) c2 = c;
+        const int64_t lim = hi - q;  // bytes of the sentence in this chunk (if below 16)
+        uint32_t m = dd_space16(c);
+        const uint32_t e2 = dd_eq16(c, 0xe2e2e2e2u);
+        if (e2) {  // U+2581 = E2 96 81 inside the sentence; one starting in the last two bytes is checked byte by byte
+          const uint32_t whole = lim - 2 >= 14 ? 0x3fffu : lim - 2 <= 0 ? 0u : (1u << (lim - 2)) - 1;
+          m |= e2 & (dd_eq16(c, 0x96969696u) >> 1) & (dd_eq16(c, 0x81818181u) >> 2) & whole;
+          for (int j = 14; j < 16; j++)
+            if (((e2 >> j) & 1u) && j < lim && space_at(a.bytes, (uint64_t)(q + j), (uint64_t)hi, &l)) m |= 1u << j;
+        }
+        if (k == 0) m &= 0xffffu << o;
+        if (lim < 16) m &= (1u << lim) - 1;
+        if (m) { end = q + __ffs((int)m) - 1; break; }
+      }
+      const uint32_t len = (uint32_t)(end - p0);
+      // bytes 16 k .. of the word (n of them)
+      auto own = [&](uint32_t k, uint32_t n) {
+        return k == 0 ? dd_shift(c0, c1, o, n) : k == 1 ? dd_shift(c1, c2, o, n)
+                                                        : dd_window(a.bytes, p0 + 16 * (int64_t)k, n, n_total, mis);
+      };
+      uint64_t h = len * 0x9e3779b97f4a7c15ull;  // a function of the word's bytes only
+      for (uint32_t k = 0; 16ull * k < len; k++) {
+        const Chunk16 x = own(k, min(16u, len - 16 * k));
+        h = (dd_rotl(h, 23) ^ x.lo) * 0x9e3779b97f4a7c15ull;
+        h = (dd_rotl(h, 23) ^ x.hi) * 0xc2b2ae3d27d4eb4full;
+      }
       h = mix64(h);
       const uint32_t tag = d.weak_tag ? 7u : (uint32_t)(h >> 32);
       const unsigned long long mine = ((unsigned long long)tag << 32) | (uint32_t)w;
@@ -495,9 +621,12 @@ __global__ void __launch_bounds__(128) dedup_words_kernel(EncArgs a, uint64_t n_
         // Equal iff the len bytes match AND the word at p2 ends right after them.  No space unit can start inside the
         // matching bytes: an ASCII space or a whole E2 96 81 there would be one in this word too, and an E2 96 81 that
         // starts inside and ends beyond leaves a continuation byte at p2 + len, which the end check rejects.
-        bool same = true;
-        for (uint64_t i = 0; i < len; i++)
-          if (p2 + i >= hi2 || a.bytes[p2 + i] != a.bytes[p0 + i]) { same = false; break; }
+        bool same = p2 + len <= hi2;
+        for (uint32_t k = 0; same && 16ull * k < len; k++) {
+          const uint32_t n = min(16u, len - 16 * k);
+          const Chunk16 x = dd_window(a.bytes, (int64_t)p2 + 16 * (int64_t)k, n, n_total, mis), y = own(k, n);
+          same = x.lo == y.lo && x.hi == y.hi;
+        }
         if (same && p2 + len < hi2 && !space_at(a.bytes, p2 + len, hi2, &l)) same = false;  // the other word is longer
         if (same) { r = w2; is_rep = false; break; }
       }
@@ -664,8 +793,12 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   a.n_tok = nullptr;  // sized by the number of words, known after find_words_vec_kernel
   {
     ytc::timer_begin(c, "enc_find");
-    const uint64_t blocks = std::min<uint64_t>((n_sent + 8 * FIND_SPW - 1) / (8 * FIND_SPW), (uint64_t)c->n_sm * 8);
-    find_words_vec_kernel<<<(unsigned)std::max<uint64_t>(blocks, 1), 256, 0, c->stream>>>(a);
+    // sentences per group: a group of mean-length sentences fills about 3/4 of a piece, so that groups longer than a
+    // piece (two passes) stay rare
+    const uint64_t mean = std::max<uint64_t>(n_bytes / n_sent, 1);
+    const uint32_t G = (uint32_t)std::min<uint64_t>(FIND_GMAX, std::max<uint64_t>(FIND_TILE * 3 / 4 / mean, 1));
+    const uint64_t blocks = std::min<uint64_t>((n_sent + G - 1) / G, (uint64_t)c->n_sm * 4);
+    find_words_vec_kernel<<<(unsigned)std::max<uint64_t>(blocks, 1), FIND_T, 0, c->stream>>>(a, G);
     ytc::timer_end(c, "enc_find");
     c->launches++;
   }
