@@ -18,8 +18,7 @@ from youtokentome_b200 import synth  # noqa: E402
 
 KNOBS = ["YT_EMU_SMS", "YT_EMU_SCHED_SEED", "YTTM_FORCE_STREAM", "YTTM_STREAM_Q", "YTTM_STAGES", "YTTM_PAIR_CAP_FLOOR", "YTTM_DEFER_CAP",
          "YTTM_ENC_CHUNK_MB", "YTTM_ENC_DEDUP_SLOTS", "YTTM_ENC_DEDUP_WEAKTAG", "YTTM_XQ_SEG_CAP",
-         "YTTM_PAIR_MAX_LOAD_PCT", "YTTM_TRAIN_PINNED_H2D", "YTTM_TRAIN_PINNED_CHUNK_KB", "YTTM_LOOP_BLOCKS",
-         "YTTM_FRONT_TOP", "YTTM_NEWP_LIMIT", "YTTM_DRAIN_PLACES", "YTTM_TRAIN_PIPELINE", "YTTM_TRAIN_PIPELINE_PIECE_KB", "YTTM_LOOP_THREADS"]
+         "YTTM_PAIR_MAX_LOAD_PCT", "YTTM_FRONT_TOP", "YTTM_NEWP_LIMIT", "YTTM_DRAIN_PLACES", "YTTM_TRAIN_PIPELINE", "YTTM_TRAIN_PIPELINE_PIECE_KB", "YTTM_LOOP_THREADS"]
 
 
 def sentences(rng, text):
@@ -127,11 +126,6 @@ def main():
             env["YTTM_XQ_SEG_CAP"] = str(int(rng.choice([4, 8, 64])))   # exchange segments overflow -> rebuild path
         if rng.integers(0, 3) == 0:
             env["YTTM_PAIR_MAX_LOAD_PCT"] = str(int(rng.choice([30, 50, 90])))
-        if rng.integers(0, 3) == 0:   # corpus through the pinned staging buffers, tiny chunks
-            env["YTTM_TRAIN_PINNED_H2D"] = str(int(rng.integers(1, 6)))
-            env["YTTM_TRAIN_PINNED_CHUNK_KB"] = str(int(rng.choice([1, 2, 16])))
-        if rng.integers(0, 4) == 0:
-            env["YTTM_LOOP_BLOCKS"] = str(int(rng.integers(1, 4)))
         # round 2: the replicated front (refresh rate, lost rounds), the drain geometry, the pipelined ingest
         if rng.integers(0, 2):
             env["YTTM_FRONT_TOP"] = str(int(rng.integers(1, 7)))
@@ -139,11 +133,11 @@ def main():
             env["YTTM_NEWP_LIMIT"] = str(int(rng.choice([1, 2, 5, 20, 768])))
         if rng.integers(0, 2):
             env["YTTM_DRAIN_PLACES"] = str(int(rng.integers(1, 8)))
-        if rng.integers(0, 3) == 0 and "YTTM_TRAIN_PINNED_H2D" not in env:
+        if rng.integers(0, 3) == 0:
             env["YTTM_TRAIN_PIPELINE"] = "1"
             env["YTTM_TRAIN_PIPELINE_PIECE_KB"] = str(int(rng.choice([1, 3, 16])))
         if rng.integers(0, 3) == 0:
-            env["YTTM_LOOP_THREADS"] = str(int(rng.choice([64, 128, 256, 1024])))
+            env["YTTM_LOOP_THREADS"] = str(int(rng.choice([64, 128, 256])))
         for k in KNOBS:
             os.environ.pop(k, None)
         os.environ.update(env)

@@ -335,7 +335,7 @@ static Status train_on_buffer(const char *text, uint64_t n, int n_tokens, const 
   // a context fixes its launch geometry when it first trains: the knobs that shape it are part of the cache key, so a
   // changed setting takes effect in a running process (the A/B tools and the tests vary them between calls)
   std::string geometry;
-  for (const char *k : {"YTTM_STAGES", "YTTM_LOOP_THREADS", "YTTM_LOOP_BLOCKS", "YT_EMU_SMS"}) {
+  for (const char *k : {"YTTM_STAGES", "YTTM_LOOP_THREADS", "YT_EMU_SMS"}) {
     const char *v = std::getenv(k);
     geometry += v ? v : "";
     geometry += '|';

@@ -40,9 +40,8 @@ struct YtLoopCtl {
   uint32_t overflow;          // a probe sequence wrapped (fatal)
   unsigned long long dead;    // token slots tombstoned since the last compaction
   unsigned long long slots;   // token slots at the last compaction
-  unsigned long long t_phase[8];  // ns spent by block 0 in: [0] drain, [1] arg-max of its partition, [2] barrier 1, [3] apply, [4] barrier 2;
-                                  // with YTTM_DBG&8 also, over ALL blocks: [5] max apply, [6] mean apply, [7] max drain
-  unsigned long long blk[2][3];   // per-iteration scratch of [5..7] (double-buffered by iteration parity)
+  unsigned long long t_phase[4];  // ns spent by block 0 in: [0] drain (wait for the count words, entries, new pairs),
+                                  // [1] election (+ refreshes), [2] apply, [3] parked entries into its partition
   unsigned long long iters;       // iterations those times cover
   uint32_t xq_round;              // exchange rounds completed (same on every rank of the job)
   uint32_t stop_why;              // stop == 2: 1 partition nearly full, 2 exchange segment overflowed, 4 partition full, 8 load factor
@@ -107,7 +106,7 @@ struct yttm_ctx {
   int loop_smem = 0, loop_resident = 0, loop_stages = 2;
   uint32_t loop_tok_cap = 0, loop_word_cap = 0, loop_stream_q = 0, loop_stream_tok_cap = 0, loop_stream_word_cap = 0;
   int loop_blocks = 0, loop_threads = 0;
-  double loop_phase_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  double loop_phase_ms[4] = {0, 0, 0, 0};   // YtLoopCtl::t_phase of the last yttm_train_run
   uint64_t loop_iters = 0, loop_relaunches = 0, loop_sweeps = 0;
 
   yttm_train_stats stats{};

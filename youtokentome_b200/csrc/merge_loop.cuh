@@ -160,13 +160,6 @@ __device__ __forceinline__ void st_relaxed(unsigned long long *p, unsigned long 
   __atomic_store_n(p, v, __ATOMIC_RELAXED);
 #endif
 }
-__device__ __forceinline__ void fence_scope(bool sys) {
-#ifndef YT_SIMT_EMU
-  if (sys) __threadfence_system(); else __threadfence();
-#else
-  __atomic_thread_fence(__ATOMIC_SEQ_CST);
-#endif
-}
 
 // Token ids must fit 22 bits (the packed exchange entries below).
 constexpr uint32_t BB_ID_LIMIT = 1u << 22;
@@ -204,7 +197,6 @@ struct LoopArgs {
   uint32_t stream_tok_cap;     // STREAMING: token / word capacity of ONE pipeline stage
   uint32_t stream_word_cap;
   uint32_t n_stage;            // STREAMING: pipeline depth
-  uint32_t dbg;                // diagnostics (env YTTM_DBG): 1 = consumers skip the scan, 2 = scalar scan, 8 = per-block timers
   uint4 *defer;                // STREAMING: per-block lists of words to rewrite after the tile scan
   uint32_t defer_cap;          // entries per block
   uint32_t n_tiles;
@@ -227,7 +219,6 @@ struct LoopArgs {
   uint32_t newp_limit;               // keys the new-pair table takes per round (NEWP_LIMIT; tests: YTTM_NEWP_LIMIT)
   uint32_t drain_places;             // places per segment the drain covers with per-thread items (1 .. XQ_BOX); the rest of a
                                      // segment goes through the shared walk.  Host: as many as one trip of the items holds.
-  unsigned long long *dbg_blk;       // YTTM_DBG & 16: 8 accumulators per block (ns): poll bests, apply, wait counts (+ owner sweep), drain, cache, sweeps
 };
 
 struct Best { unsigned long long c, prio, slot; };
@@ -285,16 +276,6 @@ __device__ __forceinline__ void xq_store(const LoopArgs &a, const XqOut &o, uint
 #pragma unroll
   for (int d = 0; d < XQ_MAX_WORLD; d++)
     if ((uint32_t)d < a.xq.world) reinterpret_cast<uint4 *>(a.xq.base[d] + o.off)[i] = e;
-}
-// every lane of a warp may contribute one update (has == true)
-__device__ __forceinline__ void xq_push(const LoopArgs &a, const XqOut &o, bool has, unsigned long long key,
-                                        long long delta, unsigned lane) {
-  const unsigned m = __ballot_sync(0xffffffffu, has);
-  if (!m) return;
-  uint32_t base = 0;
-  if (lane == 0) base = atomicAdd(o.s_n, (uint32_t)__popc(m));
-  base = __shfl_sync(0xffffffffu, base, 0);
-  if (has) xq_store(a, o, base + __popc(m & ((1u << lane) - 1u)), key, delta);
 }
 // one thread on its own (scalar paths)
 __device__ __forceinline__ void xq_push1(const LoopArgs &a, const XqOut &o, unsigned long long key, long long delta) {
@@ -849,11 +830,6 @@ __device__ __forceinline__ void sweep_below(const LoopArgs &a, uint64_t pbase, u
   block_best(b, s_warp, s_out);
 }
 
-#ifndef YT_SIMT_EMU
-#define YT_NOINLINE __noinline__
-#else
-#define YT_NOINLINE
-#endif
 // A work item of the drain: place `e` of segment j = (sender rank sd, block b); e == ~0u: no item.  cnt_off / plc_off:
 // byte offsets of its count word (in this block's row) and of its place inside the sender's {XqHdr, segments} slot.
 struct DrainItem { uint32_t e, j, sd, cnt_off, plc_off; };
@@ -870,7 +846,7 @@ __device__ __forceinline__ DrainItem drain_item(const LoopArgs &a, uint32_t item
   d.plc_off = (uint32_t)(offsetof(XqHdr, places) + ((size_t)d.e * XQ_MAX_BLOCKS + b) * 16);
   return d;
 }
-// What a drained entry needs (merge_loop_body): the front, the round's new pairs, the parked list, the partition.
+// What a drained entry needs (merge_loop_kernel): the front, the round's new pairs, the parked list, the partition.
 struct FrontCtx {
   unsigned long long *fk, *fc, *nk, *nc, *ownk;
   long long *ownd;
@@ -923,7 +899,8 @@ __device__ __forceinline__ void front_flush(const FrontCtx &f, uint32_t n) {
   if (added) atomicAdd(f.s_occ, added);
 }
 
-__device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
+// 512 threads at most: 128 registers per thread (with 1024 threads and 64 registers the loop spilled and ran slower)
+__global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
   __shared__ Best s_warp[32];
   __shared__ Best s_bound, s_tmp;   // the bound of the front / scratch of a refresh
   __shared__ uint32_t s_dead;   // token slots of this block tombstoned in this launch
@@ -969,9 +946,7 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
   const uint64_t pbase = (uint64_t)blockIdx.x * R;  // this block's partition of the pair table
   const uint32_t n_done0 = a.ctl->n_done;
   uint32_t round = a.ctl->xq_round;                   // exchange rounds completed so far (same on every rank)
-  unsigned long long tacc0 = 0, tacc2 = 0, tacc3 = 0, tacc4 = 0, titers = 0;  // phase timers (block 0, thread 0)
-  const bool dbgb = (a.dbg & 16u) != 0 && threadIdx.x == 0;   // per-block phase accumulators (thread 0 of every block)
-  unsigned long long bacc[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, bt = 0;
+  unsigned long long tacc0 = 0, tacc1 = 0, tacc2 = 0, tacc3 = 0, titers = 0;  // phase timers (block 0, thread 0)
 
   // occupancy of this block's partition (keys never leave the table between rebuilds)
   {
@@ -1092,7 +1067,6 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
   for (uint32_t it = 0; it <= a.max_iters; ++it) {
     const uint32_t n_done = n_done0 + it;
     unsigned long long tq0 = gtid == 0 ? gtimer() : 0, tq1 = 0, tq2 = 0, tq2b = 0, tq3 = 0;
-    if (dbgb) bt = gtimer();
     // ---------------- uniform exit checks: the flags every block read off the last round's count words
     const uint32_t xf = s_xf;
     {
@@ -1131,7 +1105,6 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
       a.ctl->n_done = n_done + 1;
     }
     if (gtid == 0) tq1 = gtimer();
-    if (dbgb) { const unsigned long long t = gtimer(); bacc[0] += t - bt; bt = t; }
     // every occurrence of (x,y) is merged below and no count changes are emitted for it: the front drops it here, its
     // owner parks the matching update of the partition (the front's count is exact)
     if (threadIdx.x == 0) {   // (no barrier needed behind this: the apply phase touches none of it)
@@ -1236,37 +1209,27 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
             if (slot < a.defer_cap) defer[slot] = make_uint4(d0.x + lo, obase + o, wcap, 0u);
             else s_direct = 1;  // list full: the direct pass below picks the rest up
           };
-          if (a.dbg & 1u) {
-          } else if (a.dbg & 2u) {
-            for (uint32_t base = cw * 32; base < span; base += ncw * 32) {
-              const uint32_t i = base + lane;
-              const bool hit = i + 1 < span && tk[i] == op.x && tk[i + 1] == op.y;
-              if (!__ballot_sync(0xffffffffu, hit)) continue;
-              if (hit) report(i);
-            }
-          } else {
-            // eight tokens per lane from two 16-byte shared loads; the token after them comes from the
-            // next lane.  p = position in the aligned window; occurrence p is inside the tile iff
-            // head <= p and p + 1 < total (a word-initial token is never y, so none straddles tiles).
-            // 8 tokens per lane: a scalar scan left most of the HBM bandwidth unused.
-            const uint32_t total = head + span;
-            for (uint32_t base = cw * 256; base < total; base += ncw * 256) {
-              const uint32_t p = base + lane * 8;
-              uint4 v = make_uint4(~0u, ~0u, ~0u, ~0u), u = v;
-              if (p < total) v = *reinterpret_cast<const uint4 *>(stg + p);
-              if (p + 4 < total) u = *reinterpret_cast<const uint4 *>(stg + p + 4);
-              uint32_t nxt = __shfl_down_sync(0xffffffffu, v.x, 1);
-              if (lane == 31) nxt = p + 8 < total ? stg[p + 8] : ~0u;
-              uint32_t m = (v.x == op.x && v.y == op.y ? 1u : 0u) | (v.y == op.x && v.z == op.y ? 2u : 0u) |
-                           (v.z == op.x && v.w == op.y ? 4u : 0u) | (v.w == op.x && u.x == op.y ? 8u : 0u) |
-                           (u.x == op.x && u.y == op.y ? 16u : 0u) | (u.y == op.x && u.z == op.y ? 32u : 0u) |
-                           (u.z == op.x && u.w == op.y ? 64u : 0u) | (u.w == op.x && nxt == op.y ? 128u : 0u);
-              if (!__ballot_sync(0xffffffffu, m)) continue;
-              while (m) {
-                const uint32_t pk = p + (uint32_t)__ffs(m) - 1u;
-                m &= m - 1u;
-                if (pk >= head && pk + 1 < total) report(pk - head);
-              }
+          // eight tokens per lane from two 16-byte shared loads; the token after them comes from the
+          // next lane.  p = position in the aligned window; occurrence p is inside the tile iff
+          // head <= p and p + 1 < total (a word-initial token is never y, so none straddles tiles).
+          // 8 tokens per lane: a scalar scan left most of the HBM bandwidth unused.
+          const uint32_t total = head + span;
+          for (uint32_t base = cw * 256; base < total; base += ncw * 256) {
+            const uint32_t p = base + lane * 8;
+            uint4 v = make_uint4(~0u, ~0u, ~0u, ~0u), u = v;
+            if (p < total) v = *reinterpret_cast<const uint4 *>(stg + p);
+            if (p + 4 < total) u = *reinterpret_cast<const uint4 *>(stg + p + 4);
+            uint32_t nxt = __shfl_down_sync(0xffffffffu, v.x, 1);
+            if (lane == 31) nxt = p + 8 < total ? stg[p + 8] : ~0u;
+            uint32_t m = (v.x == op.x && v.y == op.y ? 1u : 0u) | (v.y == op.x && v.z == op.y ? 2u : 0u) |
+                         (v.z == op.x && v.w == op.y ? 4u : 0u) | (v.w == op.x && u.x == op.y ? 8u : 0u) |
+                         (u.x == op.x && u.y == op.y ? 16u : 0u) | (u.y == op.x && u.z == op.y ? 32u : 0u) |
+                         (u.z == op.x && u.w == op.y ? 64u : 0u) | (u.w == op.x && nxt == op.y ? 128u : 0u);
+            if (!__ballot_sync(0xffffffffu, m)) continue;
+            while (m) {
+              const uint32_t pk = p + (uint32_t)__ffs(m) - 1u;
+              m &= m - 1u;
+              if (pk >= head && pk + 1 < total) report(pk - head);
             }
           }
           __syncwarp();
@@ -1316,14 +1279,12 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
       if (threadIdx.x == 0) s_xf = 0;   // accumulator of the poll below
     }
     if (gtid == 0) tq2 = gtimer();
-    if (dbgb) { const unsigned long long t = gtimer(); bacc[1] += t - bt; bt = t; }
     round = nround;
     // ---------------- while the other blocks finish their apply phase: the parked entries of the previous round (and
     // the consumed pair) go into this block's partition
     flush_own();
     if (threadIdx.x == 0) s_out_n = 0;   // (read by all before flush_own's barriers; next used in the next apply phase)
     if (gtid == 0) tq2b = gtimer();
-    if (dbgb) { const unsigned long long t = gtimer(); bacc[2] += t - bt; bt = t; }
     // ---------------- drain: the count changes of this merge, from every block of every GPU.  Thread j polls the count
     // word of segment j (barrier and count fetch in one) and, when the segment is short, fetches and handles its entries
     // right away — no block barrier sits between the arrival of a count word and the loads of its entries; longer
@@ -1342,16 +1303,6 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
           else if (gtimer() - t0 > a.spin_limit_ns) loop_trap();
         }
       };
-      if (a.dbg & 16u) {   // diagnostic: when have ALL count words arrived (hop + skew of the apply phases)?
-        for (uint32_t j = threadIdx.x; j < nseg; j += blockDim.x) {
-          const uint32_t sd = j / a.xq.nblocks, b = j - sd * a.xq.nblocks;
-          XqHdr *hh = xq_hdr(a.xq, a.xq.me, parity, sd);
-          const unsigned long long *cwp = sd == a.xq.me ? xq_cnt(hh, blockIdx.x, b) : &hh->shared[b];
-          for (uint32_t spin = 0; (uint32_t)(ld_relaxed_any(cwp, sys) >> 32) != round; spin++) spin_check(spin);
-        }
-        __syncthreads();
-        if (dbgb) bacc[6] += gtimer() - bt;
-      }
       // One work item per (place e, segment j), numbered place-major: item = e * nseg + j.  The thread of an item polls
       // the count word of segment j in this block's row and loads place e of that segment from the matrix — consecutive
       // lanes touch consecutive words / slots, and the entries of a round spread over the whole block.  No barrier between
@@ -1403,7 +1354,6 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
             unsigned long long key = 0;
             long long delta = 0;
             for (uint32_t spin = 0; !xq_unpack(e0, e1, stamp, &key, &delta); spin++) {   // the count word overtook the entry
-              if (dbgb) bacc[11] += 1;
               spin_check(spin);
               ld_relaxed2(ep[k], &e0, &e1, sys);
             }
@@ -1412,11 +1362,7 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
         }
       }
       if (flags) atomicOr(&s_xf, flags);
-      if (dbgb) bacc[8] += gtimer() - bt;    // thread 0 is through with its own segment
-      const int anybig = __syncthreads_or((int)big);
-      if (dbgb) bacc[9] += gtimer() - bt;    // every thread is
-      if (anybig) {   // block-uniform
-        if (dbgb) bacc[7] += 1;
+      if (__syncthreads_or((int)big)) {   // block-uniform
         xq_prefix(a, s_pref, s_scan);
         const uint32_t total = s_pref[nseg];
         for (uint32_t i = threadIdx.x; i < total; i += blockDim.x) {
@@ -1428,7 +1374,6 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
       }
     }
     __syncthreads();
-    if (dbgb) { const unsigned long long t = gtimer(); bacc[3] += t - bt; bt = t; }
     // ---- the new token's pairs: those not below the bound join the front — or, in a round with more of them than
     // the table takes, all of them stay outside and the bound rises to the largest sketch bucket (front_take)
     if (s_nocc) {   // block-uniform (read after the barrier); 0: the round had no new pair
@@ -1461,12 +1406,11 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
       }
     }
     __syncthreads();
-    if (dbgb) { const unsigned long long t = gtimer(); bacc[4] += t - bt; bt = t; }
     if (gtid == 0) {
       tq3 = gtimer();
-      tacc2 += tq1 - tq0;   // election from the front (+ refreshes)
-      tacc3 += tq2 - tq1;   // apply
-      tacc4 += tq2b - tq2;  // partition update + wait for the slowest block's count word
+      tacc1 += tq1 - tq0;   // election from the front (+ refreshes)
+      tacc2 += tq2 - tq1;   // apply
+      tacc3 += tq2b - tq2;  // parked entries -> partition
       tacc0 += tq3 - tq2b;  // drain + new pairs
       titers += 1;
     }
@@ -1474,13 +1418,9 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
   flush_own();   // every exit path: the partition is complete again
   if (threadIdx.x == 0 && s_povf) atomicExch(a.tab.overflow, 1u);
   if (gtid == 0 && n_refresh) atomicAdd(&a.ctl->n_sweeps, (unsigned long long)n_refresh);
-  if (dbgb && a.dbg_blk) {
-    bacc[5] = n_refresh;
-    for (int k = 0; k < 16; k++) a.dbg_blk[16 * blockIdx.x + k] += bacc[k];
-  }
   if (gtid == 0) {
     a.ctl->xq_round = round;
-    a.ctl->t_phase[0] += tacc0; a.ctl->t_phase[2] += tacc2; a.ctl->t_phase[3] += tacc3; a.ctl->t_phase[4] += tacc4;
+    a.ctl->t_phase[0] += tacc0; a.ctl->t_phase[1] += tacc1; a.ctl->t_phase[2] += tacc2; a.ctl->t_phase[3] += tacc3;
     a.ctl->iters += titers;
   }
   // resident tiles go back to HBM on every exit path
@@ -1490,9 +1430,6 @@ __device__ __forceinline__ void merge_loop_body(const LoopArgs &a) {
     for (uint32_t i = threadIdx.x; i < span; i += blockDim.x) a.tok[o0 + i] = stok[i];
   }
 }
-__global__ void __launch_bounds__(1024, 1) merge_loop_kernel(LoopArgs a) { merge_loop_body(a); }
-// the same loop compiled for at most 512 threads per block (128 registers per thread instead of 64)
-__global__ void __launch_bounds__(512, 1) merge_loop_kernel_512(LoopArgs a) { merge_loop_body(a); }
 
 // ---- exchange rounds outside the loop (multi-GPU table build): one block per partition -----------
 // xq_publish_table_kernel: block b enumerates the live (key, count) pairs of partition b of a SNAPSHOT of the local

@@ -20,7 +20,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <thread>
 #include <unistd.h>
 
 #include "common.cuh"
@@ -588,17 +587,14 @@ int ensure_loop_geometry(yttm_ctx *c) {
     c->loop_stream_tok_cap = (per_stage - c->loop_stream_word_cap) & ~3u;
   }
   YT_CUDA(c, cudaFuncSetAttribute(merge_loop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
-  YT_CUDA(c, cudaFuncSetAttribute(merge_loop_kernel_512, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
   int threads = 512, per_sm = 0;   // H100, 100 MB Zipf: 8.1 us per merge with 512 threads (128 registers), 11.3 with 1024 (64, spills)
-  if (const char *e = std::getenv("YTTM_LOOP_THREADS")) threads = std::max(64, std::min(1024, std::atoi(e) / 32 * 32));
-  YT_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, threads <= 512 ? merge_loop_kernel_512 : merge_loop_kernel, threads, dyn));
+  // tests: smaller blocks change how the scans and the drain split their work (512 at most: the kernel's launch bounds)
+  if (const char *e = std::getenv("YTTM_LOOP_THREADS")) threads = std::max(64, std::min(512, std::atoi(e) / 32 * 32));
+  YT_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, merge_loop_kernel, threads, dyn));
   if (per_sm < 1) YT_FAIL(c, "merge_loop_kernel does not fit on an SM");
   c->loop_threads = threads;
   // (a refresh of the front takes FRONT_TOP pairs from every block's partition and must leave room for new pairs)
-  int blocks = std::min(std::min(c->n_sm, XQ_MAX_BLOCKS), (int)(FRONT_FILL / FRONT_TOP));
-  // A/B knob: fewer blocks make the two grid barriers and the winner reduce cheaper and the per-block partition /
-  // tile larger (the tile planner falls back to STREAMING by itself if the words no longer fit)
-  if (const char *e = std::getenv("YTTM_LOOP_BLOCKS")) blocks = std::max(1, std::min(blocks, std::atoi(e)));
+  const int blocks = std::min(std::min(c->n_sm, XQ_MAX_BLOCKS), (int)(FRONT_FILL / FRONT_TOP));
   if (c->xq_nblocks && (int)c->xq_nblocks != blocks) YT_FAIL(c, "merge loop geometry differs from the exchange buffer's");
   c->loop_blocks = blocks;
   return 0;
@@ -787,8 +783,6 @@ int plan_tiles(yttm_ctx *c, LoopArgs *a) {
   a->defer = nullptr;
   a->defer_cap = 0;
   a->n_stage = (uint32_t)c->loop_stages;
-  a->dbg = 0;
-  if (const char *e = std::getenv("YTTM_DBG")) a->dbg = (uint32_t)std::atoi(e);
   c->loop_resident = 0;
   if (c->n_words == 0 || c->n_slots == 0) return 0;
   YT_CUDA(c, c->counters.reserve(64));
@@ -905,9 +899,8 @@ const char *yttm_last_error(const yttm_ctx *c) { return c ? c->err.c_str() : g_y
 double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
   // block 0's share of a merge (merge_loop.cuh): drain = wait for the count words + entries + new pairs; elect = front
   // scan (+ refreshes); apply = token scan + rewrites + count word; partition = parked entries into the table
-  static const char *ph[] = {"loop_drain", "loop_unused1", "loop_elect", "loop_apply", "loop_partition",
-                             "loop_unused5", "loop_unused6", "loop_unused7"};
-  for (int i = 0; i < 8; i++)
+  static const char *ph[] = {"loop_drain", "loop_elect", "loop_apply", "loop_partition"};
+  for (int i = 0; i < 4; i++)
     if (!std::strcmp(stage, ph[i])) return c->loop_phase_ms[i];
   if (!std::strcmp(stage, "loop_iters")) return (double)c->loop_iters;
   if (!std::strcmp(stage, "loop_refreshes")) return (double)c->loop_sweeps;
@@ -917,45 +910,6 @@ double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
   return ytc::timer_ms(const_cast<yttm_ctx *>(c), stage);
 }
 uint64_t yttm_launch_count(const yttm_ctx *c) { return c->launches; }
-
-// EXPERIMENTAL (env YTTM_TRAIN_PINNED_H2D=<host threads>, off by default until measured; SURVEY 8f-1): the
-// corpus comes from PAGEABLE host memory, which cudaMemcpyAsync stages through the driver's own bounce buffer at
-// ~10 GB/s (9.4 ms for 100 MB measured, ~1 s for 10 GB).  Here `threads` host threads copy 32 MB slices into one of two
-// pinned staging buffers while the DMA engine drains the other one; an event per buffer guards its reuse.
-static int staged_h2d(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n, int threads) {
-  constexpr uint64_t CH_MAX = 32ull << 20;
-  uint64_t CH = CH_MAX;  // tests: YTTM_TRAIN_PINNED_CHUNK_KB makes small corpora span several chunks
-  if (const char *e = std::getenv("YTTM_TRAIN_PINNED_CHUNK_KB")) CH = std::min<uint64_t>(CH_MAX, (uint64_t)std::max(1, std::atoi(e)) << 10);
-  struct Stage { void *pin[2] = {nullptr, nullptr}; cudaEvent_t ev[2] = {nullptr, nullptr}; };
-  static thread_local Stage st;  // kept for the life of the host thread, like the training context itself
-  for (int k = 0; k < 2; k++)
-    if (!st.pin[k]) {
-      YT_CUDA(c, cudaHostAlloc(&st.pin[k], CH_MAX, cudaHostAllocDefault));
-      YT_CUDA(c, cudaEventCreateWithFlags(&st.ev[k], cudaEventDisableTiming));
-    }
-  bool used[2] = {false, false};
-  int k = 0;
-  for (uint64_t off = 0; off < n; off += CH, k ^= 1) {
-    const uint64_t len = std::min<uint64_t>(CH, n - off);
-    if (used[k]) YT_CUDA(c, cudaEventSynchronize(st.ev[k]));  // the copy out of this buffer has finished
-    const uint64_t per = (len + (uint64_t)threads - 1) / (uint64_t)threads;
-    char *buf = static_cast<char *>(st.pin[k]);  // a local copy: `st` is thread_local, a worker would see its own (empty) one
-    const char *from = src + off;
-    std::vector<std::thread> pool;
-    for (int t = 1; t < threads; t++) {
-      const uint64_t lo = std::min<uint64_t>(len, (uint64_t)t * per), hi = std::min<uint64_t>(len, lo + per);
-      if (hi > lo) pool.emplace_back([=]() { std::memcpy(buf + lo, from + lo, hi - lo); });
-    }
-    std::memcpy(buf, from, std::min<uint64_t>(len, per));
-    for (auto &th : pool) th.join();
-    YT_CUDA(c, cudaMemcpyAsync(dst + off, st.pin[k], len, cudaMemcpyHostToDevice, c->stream));
-    YT_CUDA(c, cudaEventRecord(st.ev[k], c->stream));
-    used[k] = true;
-  }
-  for (int j = 0; j < 2; j++)
-    if (used[j]) YT_CUDA(c, cudaEventSynchronize(st.ev[j]));  // the staging buffers are free again when we return
-  return 0;
-}
 
 // The corpus comes from pageable host memory at ~11 GB/s, and the two byte passes over it (code point histogram, word
 // split + dedup) need neither each other nor the alphabet: the text is copied in pieces that END WITH an ASCII space or
@@ -1017,17 +971,13 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
   uint8_t *base = c->text_buf.as<uint8_t>();
   YT_CUDA(c, cudaMemsetAsync(base, ' ', 16, c->stream));
   YT_CUDA(c, cudaMemsetAsync(base + 16 + n, ' ', 32, c->stream));
-  int staged = 0;
-  if (const char *e = std::getenv("YTTM_TRAIN_PINNED_H2D")) staged = std::max(0, std::min(64, std::atoi(e)));
-  c->timers["h2d_variant"].ms = (float)staged;  // yttm_stage_ms(ctx, "h2d_variant")
   c->d_text = base + 16;
   c->text_external = false;
   c->pipe_hist = false;
   c->pipe_wtab_cap = 0;
   uint64_t pipe_min = 64ull << 20;   // below this the passes are too short to be worth a second stream
   if (const char *e = std::getenv("YTTM_TRAIN_PIPELINE")) pipe_min = std::atoi(e) > 0 ? (uint64_t)std::atoi(e) : ~0ull;   // bytes; 0 = off
-  if (n && staged) { if (staged_h2d(c, base + 16, bytes, n, staged)) return 1; }
-  else if (n >= pipe_min) { if (pipelined_load(c, base + 16, bytes, n)) return 1; }
+  if (n >= pipe_min) { if (pipelined_load(c, base + 16, bytes, n)) return 1; }
   else if (n) YT_CUDA(c, cudaMemcpyAsync(base + 16, bytes, n, cudaMemcpyHostToDevice, c->stream));
   ytc::timer_end(c, "h2d");
   if (c->pipe_hist) {   // the kernels of the last pieces: everything after this call sees them done
@@ -1497,8 +1447,7 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
   YT_CUDA(c, cudaMemcpyAsync(&h, ctl, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   YT_CUDA(c, cudaStreamSynchronize(c->stream));
   h.n_done = 0; h.stop = 0; h.stop_why = 0; h.iters = 0; h.n_sweeps = 0;
-  for (int i = 0; i < 8; i++) h.t_phase[i] = 0;
-  for (int i = 0; i < 6; i++) (&h.blk[0][0])[i] = 0;
+  for (int i = 0; i < 4; i++) h.t_phase[i] = 0;
   YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
   c->loop_relaunches = 0;
   ytc::timer_begin(c, "merge_loop");
@@ -1519,12 +1468,6 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
     a.max_total = max_merges;
     a.max_iters = max_merges;
     a.part_limit = (uint32_t)(((uint64_t)c->p_rmask + 1) * pair_max_load_pct() / 100);  // rebuild above this partition load (default 1/2)
-    a.dbg_blk = nullptr;
-    if (a.dbg & 16u) {   // diagnostic: where do the blocks spend a merge?  (printed to stderr after the run)
-      if (!c->scratch_cnt.p || c->scratch_cnt.cap < (size_t)c->loop_blocks * 128) YT_CUDA(c, c->scratch_cnt.reserve((size_t)c->loop_blocks * 128));
-      if (c->loop_relaunches == 0) YT_CUDA(c, cudaMemsetAsync(c->scratch_cnt.p, 0, (size_t)c->loop_blocks * 128, c->stream));
-      a.dbg_blk = c->scratch_cnt.as<unsigned long long>();
-    }
     a.front_top = 4;   // smaller front: shorter probes and scans, but more refreshes (A/B: YTTM_FRONT_TOP)
     if (const char *e = std::getenv("YTTM_FRONT_TOP")) a.front_top = (uint32_t)std::max(1, std::min((int)FRONT_TOP, std::atoi(e)));
     {  // as many places per segment as ONE trip of the drain's items holds (1 GPU: all 7; 8 GPUs: 1)
@@ -1535,12 +1478,11 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
     a.newp_limit = NEWP_LIMIT;
     if (const char *e = std::getenv("YTTM_NEWP_LIMIT")) a.newp_limit = (uint32_t)std::max(1, std::min((int)NEWP_LIMIT, std::atoi(e)));
     a.dead_min_slots = 4096;
-    if (const char *e = std::getenv("YTTM_DEAD_MIN_SLOTS")) a.dead_min_slots = (uint32_t)std::max(0, std::atoi(e));
     YT_CUDA(c, cudaMemsetAsync(c->frontbuf.p, 0, front_buf_words((uint32_t)c->loop_blocks) * 8, c->stream));  // refresh numbers restart at 1
 #ifndef YT_SIMT_EMU
     void *args[] = {&a};
-    YT_CUDA(c, cudaLaunchCooperativeKernel(c->loop_threads <= 512 ? (void *)merge_loop_kernel_512 : (void *)merge_loop_kernel,
-                                           dim3(c->loop_blocks), dim3(c->loop_threads), args, (size_t)c->loop_smem, c->stream));
+    YT_CUDA(c, cudaLaunchCooperativeKernel((void *)merge_loop_kernel, dim3(c->loop_blocks), dim3(c->loop_threads), args,
+                                           (size_t)c->loop_smem, c->stream));
 #else  // tests/emul/simt: every block on its own OS thread, grid.sync() = pthread barrier
     emu::launch_cooperative((unsigned)c->loop_blocks, (unsigned)c->loop_threads, (size_t)c->loop_smem,
                             [=]() { merge_loop_kernel(a); });
@@ -1568,30 +1510,7 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
     YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
   }
   ytc::timer_end(c, "merge_loop");
-  if (const char *e = std::getenv("YTTM_DBG")) {
-    if ((std::atoi(e) & 16) && h.iters) {
-      std::vector<unsigned long long> blk((size_t)c->loop_blocks * 16);
-      YT_CUDA(c, cudaMemcpyAsync(blk.data(), c->scratch_cnt.p, blk.size() * 8, cudaMemcpyDeviceToHost, c->stream));
-      YT_CUDA(c, cudaStreamSynchronize(c->stream));
-      static const char *nm[] = {"elect(+refresh)", "apply", "partition_update", "wait_counts+drain", "new_pairs", "refreshes", "  of it: until all count words are in", "rounds with a shared (long) segment",
-                                 "  .. thread 0 done with its segment", "  .. all threads done", "", "entry re-loads of thread 0 [count]"};
-      const double it = (double)h.iters;
-      for (int k = 0; k < 12; k++) {
-        if (!nm[k][0]) continue;
-        double mn = 1e30, mx = 0, sum = 0;
-        int imn = 0, imx = 0;
-        for (int b = 0; b < c->loop_blocks; b++) {
-          const double v = (double)blk[(size_t)b * 16 + k] / (k == 5 ? 1.0 : it) * (k == 5 || k == 7 || k == 11 ? 1.0 : 1e-3);
-          sum += v;
-          if (v < mn) { mn = v; imn = b; }
-          if (v > mx) { mx = v; imx = b; }
-        }
-        std::fprintf(stderr, "YTTM_DBG16 %-36s per merge: mean %8.3f  min %8.3f (block %d)  max %8.3f (block %d)%s\n", nm[k],
-                     sum / c->loop_blocks, mn, imn, mx, imx, k == 5 ? "  [count per run]" : k == 7 ? "  [fraction]" : " us");
-      }
-    }
-  }
-  for (int i = 0; i < 8; i++) c->loop_phase_ms[i] = (double)h.t_phase[i] * 1e-6;
+  for (int i = 0; i < 4; i++) c->loop_phase_ms[i] = (double)h.t_phase[i] * 1e-6;
   c->loop_iters = h.iters;
   c->loop_sweeps = h.n_sweeps;
   *n_done_out = h.n_done;
