@@ -2,6 +2,7 @@
 bench.main() unchanged on the CPU emulator build of the kernels (torch.cuda stubbed, workload shrunk).  The numbers are
 meaningless here; the keys, their types and the internal consistency of the line are what the driver depends on."""
 import json
+import math
 import os
 import subprocess
 import sys
@@ -9,6 +10,11 @@ import sys
 import pytest
 
 from _bind import ROOT, have_reference
+
+
+def _half_unit_4g(x):
+    """Half a unit in the 4th significant digit of x: the most a value printed as "%.4g" is off."""
+    return 0.5 * 10.0 ** (math.floor(math.log10(abs(x))) - 3)
 
 
 def test_bench_line_contract_on_the_emulator(tmp_path):
@@ -31,7 +37,11 @@ def test_bench_line_contract_on_the_emulator(tmp_path):
     assert set(d["e2e"]) >= {"value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"} and d["e2e"]["h2d_bytes_per_step"] > 0
     rf = d["roofline"]
     assert set(rf) >= {"bound", "achieved", "peak", "unit", "frac", "traffic"} and rf["bound"] == "hbm"
-    assert abs(rf["frac"] - rf["achieved"] / rf["peak"]) < 1e-9
+    # frac is achieved / peak: both are printed to 4 significant digits, so some rate must round to `achieved` while
+    # that rate / peak rounds to `frac` (a fixed absolute tolerance fails at random once the rate reaches 0.01 GB/s)
+    a, f, p = rf["achieved"], rf["frac"], rf["peak"]
+    ha, hf = _half_unit_4g(a) * (1 + 1e-12), _half_unit_4g(f) * (1 + 1e-12)
+    assert a > 0 and f > 0 and (a - ha) / p <= f + hf and (a + ha) / p >= f - hf, (a, f, p)
     cb = d["cpu_baseline"]
     assert set(cb) >= {"value", "unit", "cores", "kind", "sample"} and cb["kind"] in ("reference", "port") and cb["ids_equal_on_sample"]
     assert abs(d["ms_per_step"] * d["value"] / 1e3 - d["config"]["sentences_per_gpu"] / 1e6) < 1e-6   # value = S / t

@@ -1,8 +1,7 @@
 """Parity of hot path (a): the CUDA trainer (through the C ABI) against the oracle — rules and
 char2id bit-exact (the assertion of stress_test.cpp:433-434) — and against oracle/_ref where
-it is present.  All tests need a GPU."""
-import ctypes as C
-
+it is present.  All tests need a GPU.  The byte passes and the initial pair table alone are checked field by field
+in tests/test_train_front_gpu.py."""
 import numpy as np
 import pytest
 
@@ -94,57 +93,6 @@ def test_zipf_medium_vs_reference(product, checkers):
     ref.train(text, m_r, 8000, 0.9995, n_threads=8)
     m_g = gpu_train(text, 8000, 0.9995)
     assert read_model(m_r) == read_model(m_g)
-
-
-def test_initial_pair_table(product, oracle):
-    """The pair-count scan kernel alone: table after build == counts recomputed in numpy."""
-    from youtokentome_b200 import _lib
-    L = _lib.lib()
-    text = _cases.zipf().text(100_000)
-    ctx = C.c_void_p()
-    assert L.yttm_ctx_create(0, C.byref(ctx)) == 0
-    try:
-        dl, nd = C.c_uint64(0), C.c_uint64(0)
-        assert L.yttm_train_load_corpus(ctx, C.cast(C.c_char_p(text), C.c_void_p), len(text), 0) == 0
-        assert L.yttm_train_char_hist(ctx, C.byref(dl), C.byref(nd)) == 0
-        cps = np.zeros(nd.value, dtype=np.uint32)
-        cnt = np.zeros(nd.value, dtype=np.uint64)
-        L.yttm_train_get_char_hist(ctx, cps.ctypes.data, cnt.ctypes.data)
-        # reference-free check of the histogram
-        import collections
-        want = collections.Counter(ch for ch in text.decode() if not ch.isspace())
-        assert {chr(c): int(n) for c, n in zip(cps, cnt)} == dict(want)
-        assert dl.value == len(text.decode())
-        ids = np.arange(5, 5 + len(cps), dtype=np.uint32)
-        kc = np.concatenate([cps, [9601]]).astype(np.uint32)
-        ki = np.concatenate([ids, [4]]).astype(np.uint32)
-        assert L.yttm_train_set_alphabet(ctx, kc.ctypes.data, ki.ctypes.data, len(kc), 4) == 0
-        st = _lib.TrainStats()
-        assert L.yttm_train_build(ctx, C.byref(st)) == 0, L.yttm_last_error(ctx)
-        keys = np.zeros(st.n_pairs + 16, dtype=np.uint64)
-        cts = np.zeros(st.n_pairs + 16, dtype=np.uint64)
-        n = C.c_uint64(0)
-        assert L.yttm_train_dump_pairs(ctx, keys.ctypes.data, cts.ctypes.data, len(keys), C.byref(n)) == 0
-        got = {int(k): int(c) for k, c in zip(keys[:n.value], cts[:n.value])}
-        cp2id = {int(c): int(i) for c, i in zip(kc, ki)}
-        want = collections.Counter()
-        for w in text.decode().split():
-            t = [4] + [cp2id[ord(ch)] for ch in w]
-            i = 0
-            while i < len(t):
-                j = i
-                while j < len(t) and t[j] == t[i]:
-                    j += 1
-                if j - i >= 2:
-                    want[(t[i] << 32) | t[i]] += (j - i) // 2
-                if j < len(t):
-                    want[(t[i] << 32) | t[j]] += 1
-                i = j
-        assert got == dict(want)
-        assert st.n_words == len(text.decode().split())
-        assert st.n_unique == len(set(w for w in text.decode().split()))
-    finally:
-        L.yttm_ctx_destroy(ctx)
 
 
 @pytest.mark.parametrize("q", ["64", "1000"])
