@@ -164,6 +164,29 @@ class BaseEncoder {
                               const int32_t **d_ids, const uint64_t **d_id_offsets, uint64_t *total_ids, bool bos = false,
                               bool eos = false, bool reverse = false, double dropout_prob = 0) const;
 
+  // encode_packed_into plus the source bytes of every id: spans[2j], spans[2j+1] = [start, end) of id j in the
+  // coordinates of offsets (yttm_enc_run_spans in yttm_b200.h says which bytes an id covers).  spans holds
+  // 2 * ids_cap values.  With dropout, advances the same sentence counter as encode_packed.
+  Status encode_spans_into(const char *bytes, const uint64_t *offsets, uint64_t n_sentences, int32_t *ids, uint64_t ids_cap,
+                           uint64_t *id_offsets, uint64_t *spans, uint64_t *total_ids, bool bos = false, bool eos = false,
+                           bool reverse = false, double dropout_prob = 0) const;
+  Status encode_spans_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sentences,
+                             const int32_t **d_ids, const uint64_t **d_id_offsets, const uint64_t **d_spans,
+                             uint64_t *total_ids, bool bos = false, bool eos = false, bool reverse = false,
+                             double dropout_prob = 0) const;
+  // encode_as_subwords of a packed batch on the GPU, the pieces back to back: piece k = pieces[piece_offsets[k],
+  // piece_offsets[k+1]), the pieces of sentence i = [sent_offsets[i], sent_offsets[i+1]).  Status code 2 (nothing
+  // written, *n_pieces / *n_bytes = sizes needed) when pieces_cap (piece_offsets holds pieces_cap + 1) or bytes_cap
+  // is too small.
+  Status encode_subwords_into(const char *bytes, const uint64_t *offsets, uint64_t n_sentences, uint8_t *pieces,
+                              uint64_t bytes_cap, uint64_t *piece_offsets, uint64_t pieces_cap, uint64_t *sent_offsets,
+                              uint64_t *n_pieces, uint64_t *n_bytes, bool bos = false, bool eos = false, bool reverse = false,
+                              double dropout_prob = 0) const;
+  Status encode_subwords_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sentences,
+                                const uint8_t **d_pieces, const uint64_t **d_piece_offsets, const uint64_t **d_sent_offsets,
+                                uint64_t *n_pieces, uint64_t *n_piece_bytes, bool bos = false, bool eos = false,
+                                bool reverse = false, double dropout_prob = 0) const;
+
   // decode() of a packed batch on the GPU: sentence i = ids[offsets[i], offsets[i+1]), text i =
   // text[text_offsets[i], text_offsets[i+1]).  Status code 2 (nothing written, *total_bytes = size needed) when
   // text_cap is too small.

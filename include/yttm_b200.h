@@ -29,8 +29,8 @@ const char *yttm_last_error(const yttm_ctx *ctx); /* ctx may be NULL: error of t
 int yttm_device_count(void);
 
 /* cudaEvent milliseconds of the last call of the named stage ("char_hist", "word_count",
- * "tokenise", "pair_hist", "merge_loop", "encode", "h2d", "d2h", "decode", "dec_count", "dec_scan",
- * "dec_emit", "dec_e2e"); < 0 if unknown. */
+ * "tokenise", "pair_hist", "merge_loop", "encode", "h2d", "d2h", "enc_spans", "enc_subwords", "decode", "dec_count",
+ * "dec_scan", "dec_emit", "dec_e2e"); < 0 if unknown. */
 double yttm_stage_ms(const yttm_ctx *ctx, const char *stage);
 /* number of kernel launches issued by this context so far (bench.py: gpu_launches) */
 uint64_t yttm_launch_count(const yttm_ctx *ctx);
@@ -163,6 +163,38 @@ int yttm_enc_run_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_of
                         uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                         uint64_t first_sentence_index, const int32_t **d_out_ids, const uint64_t **d_out_offsets,
                         uint64_t *out_n);
+
+/* ---- source spans and subword pieces of an encode ---------------------------------------------------------------
+ * Same batches, arguments, checks and ids as yttm_enc_run / yttm_enc_run_device, plus the bytes every id came from.
+ * Span of id j = (spans[2j], spans[2j+1]) = [start, end) in the coordinates of offsets (sentence i is
+ * [offsets[i], offsets[i+1]) of them, also for the device forms whose d_bytes is the first byte of sentence 0):
+ *   an ordinary id covers a run of valid units (code points, or invalid bytes) of its word: from the first byte of its
+ *   first valid unit to the end of its last; an invalid unit between two of its units lies inside, any other in no span;
+ *   <UNK> covers its maximal run of out-of-alphabet units the same way; a word-initial U+2581 no rule merged covers no
+ *   unit: its span is empty and sits where the next id's span starts; <BOS> = [offsets[i], offsets[i]), <EOS> =
+ *   [offsets[i+1], offsets[i+1]); with reverse the (id, span) pairs are reversed together.
+ * The first spans / subwords call of an encoder builds its piece table (host work + one upload). */
+int yttm_enc_run_spans(yttm_enc *enc, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                       int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, int32_t *out_ids,
+                       uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_spans /* 2 * out_cap */, uint64_t *out_n);
+/* *d_out_* point into library-owned memory, complete when the call returns and valid until the next encode call */
+int yttm_enc_run_spans_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                              uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                              uint64_t first_sentence_index, const int32_t **d_out_ids, const uint64_t **d_out_offsets,
+                              const uint64_t **d_out_spans, uint64_t *out_n);
+/* encode_as_subwords (bpe.cpp:1757) of a batch: one piece per id, piece k = pieces[piece_offsets[k],
+ * piece_offsets[k+1]) (UTF-8): the recipe of an ordinary id with its leading U+2581 kept, "<BOS>" / "<EOS>", and for
+ * <UNK> the characters of its run (its span's bytes without invalid units).  The pieces of sentence i are
+ * [sent_offsets[i], sent_offsets[i+1]).  piece_offsets has *n_pieces + 1 entries, sent_offsets n_sent + 1.  Returns 2
+ * with *n_pieces / *n_piece_bytes = the sizes needed when pieces_cap or bytes_cap is too small (nothing written). */
+int yttm_enc_run_subwords(yttm_enc *enc, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                          int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, uint8_t *out_pieces,
+                          uint64_t bytes_cap, uint64_t *out_piece_offsets /* pieces_cap + 1 */, uint64_t pieces_cap,
+                          uint64_t *out_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes);
+int yttm_enc_run_subwords_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                 uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                                 uint64_t first_sentence_index, const uint8_t **d_pieces, const uint64_t **d_piece_offsets,
+                                 const uint64_t **d_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes);
 
 /* ---- decoding: BaseEncoder::decode (bpe.cpp:1843-1861 + id_to_subword :1774-1807) of a batch ---- */
 

@@ -58,6 +58,25 @@ void yttm_api_result_counts(void *handle, uint64_t *n_pieces, uint64_t *n_senten
 void yttm_api_result_text(void *handle, char *out);
 void yttm_api_result_offsets(void *handle, uint64_t *piece_off, uint64_t *sent_off);
 
+/* encode with the source span of every id (yttm_enc_run_spans of yttm_b200.h): spans_out holds 2 * ids_cap values,
+ * (start, end) per id in the coordinates of offsets; 0 ok, 1 error, 2 ids_cap too small (*total_ids = size needed) */
+int yttm_api_encode_spans_into(void *handle, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                               int reverse, double dropout, int32_t *ids_out, uint64_t ids_cap, uint64_t *offsets_out,
+                               uint64_t *spans_out, uint64_t *total_ids);
+int yttm_api_encode_spans_device(void *handle, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                 uint64_t n_sent, int bos, int eos, int reverse, double dropout, const int32_t **d_ids,
+                                 const uint64_t **d_id_offsets, const uint64_t **d_spans, uint64_t *total_ids);
+/* encode(output_type='subword') on the GPU (yttm_enc_run_subwords): the same pieces as yttm_api_encode_subwords, into
+ * caller-owned buffers; 0 ok, 1 error, 2 a capacity too small (*n_pieces / *n_bytes = sizes needed) */
+int yttm_api_encode_subwords_into(void *handle, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos,
+                                  int eos, int reverse, double dropout, uint8_t *pieces, uint64_t bytes_cap,
+                                  uint64_t *piece_offsets /* pieces_cap + 1 */, uint64_t pieces_cap,
+                                  uint64_t *sent_offsets /* n_sent + 1 */, uint64_t *n_pieces, uint64_t *n_bytes);
+int yttm_api_encode_subwords_device(void *handle, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                    uint64_t n_sent, int bos, int eos, int reverse, double dropout, const uint8_t **d_pieces,
+                                    const uint64_t **d_piece_offsets, const uint64_t **d_sent_offsets, uint64_t *n_pieces,
+                                    uint64_t *n_piece_bytes);
+
 /* yttm.pyx:136-158 decode: one piece per sentence; id_to_subword: one piece; vocab: vocab_size pieces */
 int64_t yttm_api_decode(void *handle, const int32_t *ids, const uint64_t *offsets, uint64_t n_sent,
                         const int32_t *ignore, uint64_t n_ignore);

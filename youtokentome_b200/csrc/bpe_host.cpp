@@ -568,6 +568,63 @@ Status BaseEncoder::encode_packed_device(const char *d_bytes, const uint64_t *d_
   return Status();
 }
 
+Status BaseEncoder::encode_spans_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, int32_t *ids,
+                                      uint64_t ids_cap, uint64_t *id_offsets, uint64_t *spans, uint64_t *total_ids, bool bos,
+                                      bool eos, bool reverse, double dropout_prob) const {
+  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
+  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
+  if (!device_status_.ok()) return device_status_;
+  *total_ids = 0;
+  int rc = yttm_enc_run_spans(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+                              sentence_counter_, ids, ids_cap, id_offsets, spans, total_ids);
+  if (rc == 2) return Status(2, "encode_spans_into: output buffer too small");
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
+Status BaseEncoder::encode_spans_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                                        const int32_t **d_ids, const uint64_t **d_id_offsets, const uint64_t **d_spans,
+                                        uint64_t *total_ids, bool bos, bool eos, bool reverse, double dropout_prob) const {
+  if (!device_status_.ok()) return device_status_;
+  int rc = yttm_enc_run_spans_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+                                     dropout_seed_, sentence_counter_, d_ids, d_id_offsets, d_spans, total_ids);
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
+Status BaseEncoder::encode_subwords_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, uint8_t *pieces,
+                                         uint64_t bytes_cap, uint64_t *piece_offsets, uint64_t pieces_cap,
+                                         uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes, bool bos, bool eos,
+                                         bool reverse, double dropout_prob) const {
+  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
+  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
+  if (!device_status_.ok()) return device_status_;
+  *n_pieces = 0;
+  *n_bytes = 0;
+  int rc = yttm_enc_run_subwords(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+                                 sentence_counter_, pieces, bytes_cap, piece_offsets, pieces_cap, sent_offsets, n_pieces,
+                                 n_bytes);
+  if (rc == 2) return Status(2, "encode_subwords_into: output buffer too small");
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
+Status BaseEncoder::encode_subwords_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                                           const uint8_t **d_pieces, const uint64_t **d_piece_offsets,
+                                           const uint64_t **d_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes,
+                                           bool bos, bool eos, bool reverse, double dropout_prob) const {
+  if (!device_status_.ok()) return device_status_;
+  int rc = yttm_enc_run_subwords_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+                                        dropout_seed_, sentence_counter_, d_pieces, d_piece_offsets, d_sent_offsets,
+                                        n_pieces, n_piece_bytes);
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
 Status BaseEncoder::decode_packed_into(const int32_t *ids, const uint64_t *offsets, uint64_t n_sent, const int32_t *ignore_ids,
                                        uint64_t n_ignore, uint8_t *text, uint64_t text_cap, uint64_t *text_offsets,
                                        uint64_t *total_bytes) const {

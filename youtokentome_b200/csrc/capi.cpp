@@ -165,6 +165,55 @@ int64_t yttm_api_encode_subwords(void *hv, const char *bytes, const uint64_t *of
   return (int64_t)g_res.text.size();
 }
 
+// Spans and subwords on the GPU: caller-owned host buffers (return code 2: a capacity too small, sizes needed in the
+// counts) or pointers into library-owned device memory valid until the next encode call on this handle.
+int yttm_api_encode_spans_into(void *hv, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                               int reverse, double dropout, int32_t *ids_out, uint64_t ids_cap, uint64_t *offsets_out,
+                               uint64_t *spans_out, uint64_t *total_ids) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->encode_spans_into(bytes, offsets, n_sent, ids_out, ids_cap, offsets_out, spans_out, total_ids,
+                                        bos != 0, eos != 0, reverse != 0, dropout);
+  if (st.code == 2) return 2;
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
+int yttm_api_encode_spans_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                                 int bos, int eos, int reverse, double dropout, const int32_t **d_ids,
+                                 const uint64_t **d_id_offsets, const uint64_t **d_spans, uint64_t *total_ids) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->encode_spans_device(d_bytes, d_offsets, n_bytes, n_sent, d_ids, d_id_offsets, d_spans, total_ids,
+                                          bos != 0, eos != 0, reverse != 0, dropout);
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
+int yttm_api_encode_subwords_into(void *hv, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                                  int reverse, double dropout, uint8_t *pieces, uint64_t bytes_cap, uint64_t *piece_offsets,
+                                  uint64_t pieces_cap, uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->encode_subwords_into(bytes, offsets, n_sent, pieces, bytes_cap, piece_offsets, pieces_cap, sent_offsets,
+                                           n_pieces, n_bytes, bos != 0, eos != 0, reverse != 0, dropout);
+  if (st.code == 2) return 2;
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
+int yttm_api_encode_subwords_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                    uint64_t n_sent, int bos, int eos, int reverse, double dropout, const uint8_t **d_pieces,
+                                    const uint64_t **d_piece_offsets, const uint64_t **d_sent_offsets, uint64_t *n_pieces,
+                                    uint64_t *n_piece_bytes) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->encode_subwords_device(d_bytes, d_offsets, n_bytes, n_sent, d_pieces, d_piece_offsets, d_sent_offsets,
+                                             n_pieces, n_piece_bytes, bos != 0, eos != 0, reverse != 0, dropout);
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
 void yttm_api_result_counts(void *, uint64_t *n_pieces, uint64_t *n_sentences) {
   *n_pieces = g_res.piece_off.size() - 1;
   *n_sentences = g_res.sent_off.size() - 1;

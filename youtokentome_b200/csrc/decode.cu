@@ -217,41 +217,55 @@ void yttm_dec_free(yttm_dec *d) {
   delete d;
 }
 
-namespace {
-
-// The piece of every id in [0, V): O(sum of piece bytes) host work and one upload.  The recipe of a rule's product is
-// the concatenation of its operands' recipes at the time of the rule (fill_from_state), a special id takes its token.
-int build_piece_table(yttm_enc *e) {
+// O(sum of piece bytes) host work.  The recipe of a rule's product is the concatenation of its operands' recipes at the
+// time of the rule (fill_from_state), a special id takes its token.
+int yttm_model_pieces(yttm_enc *e, const char *who, std::vector<std::string> *raw_out, std::vector<uint8_t> *special_out) {
   yttm_ctx *c = e->ctx;
+  const std::string w = who;
   const uint64_t V = e->vocab;
-  if (V >= 0x7fffffffull) YT_FAIL(c, "decode: vocabulary too large");
-  std::vector<std::string> raw(V);
+  if (V >= 0x7fffffffull) YT_FAIL(c, w + ": vocabulary too large");
+  std::vector<std::string> &raw = *raw_out;
+  raw.assign(V, std::string());
   std::vector<uint8_t> have(V, 0);
   for (size_t i = 0; i < e->h_char_cp.size(); i++) {
     const uint32_t id = e->h_char_id[i];
-    if (id >= V) YT_FAIL(c, "decode: model has a character id outside [0, vocab_size): " + std::to_string(id));
+    if (id >= V) YT_FAIL(c, w + ": model has a character id outside [0, vocab_size): " + std::to_string(id));
     raw[id].clear();
     append_utf8(e->h_char_cp[i], &raw[id]);
     have[id] = 1;
   }
   for (size_t i = 0; 3 * i + 2 < e->h_rules_xyz.size(); i++) {
     const uint32_t x = e->h_rules_xyz[3 * i], y = e->h_rules_xyz[3 * i + 1], z = e->h_rules_xyz[3 * i + 2];
-    if (x >= V || y >= V || z >= V) YT_FAIL(c, "decode: model has a rule id outside [0, vocab_size): rule " + std::to_string(i));
-    if (!have[x] || !have[y]) YT_FAIL(c, "decode: model rule " + std::to_string(i) + " uses an id without a piece");
-    if (raw[x].size() + raw[y].size() >= MAX_PIECE) YT_FAIL(c, "decode: model piece of id " + std::to_string(z) + " is over 128 MB");
+    if (x >= V || y >= V || z >= V) YT_FAIL(c, w + ": model has a rule id outside [0, vocab_size): rule " + std::to_string(i));
+    if (!have[x] || !have[y]) YT_FAIL(c, w + ": model rule " + std::to_string(i) + " uses an id without a piece");
+    if (raw[x].size() + raw[y].size() >= MAX_PIECE) YT_FAIL(c, w + ": model piece of id " + std::to_string(z) + " is over 128 MB");
     std::string r = raw[x] + raw[y];
     raw[z] = std::move(r);
     have[z] = 1;
   }
-  std::vector<uint8_t> special(V, 0);
+  std::vector<uint8_t> &special = *special_out;
+  special.assign(V, 0);
   const std::pair<int, const char *> sp[] = {{e->unk, "<UNK>"}, {e->pad, "<PAD>"}, {e->bos, "<BOS>"}, {e->eos, "<EOS>"}};
   for (auto &p : sp)
     if (p.first >= 0 && (uint64_t)p.first < V) { raw[p.first] = p.second; have[p.first] = 1; special[p.first] = 1; }
+  for (uint64_t i = 0; i < V; i++)
+    if (!have[i]) YT_FAIL(c, w + ": model has no piece for id " + std::to_string(i));
+  return 0;
+}
+
+namespace {
+
+// The decode piece of every id in [0, V) and one upload.
+int build_piece_table(yttm_enc *e) {
+  yttm_ctx *c = e->ctx;
+  const uint64_t V = e->vocab;
+  std::vector<std::string> raw;
+  std::vector<uint8_t> special;
+  if (yttm_model_pieces(e, "decode", &raw, &special)) return 1;
   const uint64_t n_bits = (V + 31) / 32;
   std::vector<uint32_t> off(V + 1), lead(n_bits, 0);
   uint64_t total = 0;
   for (uint64_t i = 0; i < V; i++) {
-    if (!have[i]) YT_FAIL(c, "decode: model has no piece for id " + std::to_string(i));
     if (!special[i] && raw[i].compare(0, 3, "\xe2\x96\x81") == 0) {  // replace_space: a leading U+2581 is one space
       raw[i].replace(0, 3, " ");
       lead[i >> 5] |= 1u << (i & 31);

@@ -18,6 +18,11 @@
 //                               bpe.cpp:1417-1453 with a counter-based generator)
 //   sentence_ids_kernel         ids per sentence; an exclusive scan turns them into output offsets
 //   emit_ids_kernel             warp per sentence: copies the ids of its words into the packed output
+// On request (yttm_enc_run_spans* / yttm_enc_run_subwords*) the same flow also gives the source span of every id and
+// the subword pieces:
+//   span_words_kernel           one thread per encoded word: the span of each of its ids relative to the word start
+//   emit_ids_kernel<true>       ... and the spans at the occurrences' positions
+//   sub_count_kernel / scan / sub_emit_kernel   one thread per id: piece lengths, offsets, piece bytes
 // The ids of a word are kept in its private slots of a scratch buffer (a word of k bytes owns k+1 slots), at a
 // position that is a pure function of its byte position, so no kernel depends on another block's progress.
 #include <algorithm>
@@ -703,8 +708,67 @@ __global__ void __launch_bounds__(256) sentence_ids_kernel(EncArgs a, const uint
   }
 }
 
+// ---- spans ------------------------------------------------------------------------------------------------------
+// The source bytes of every id: span_words_kernel walks the units of every encoded item (a representative, or every
+// occurrence with dropout) in step with its ids and writes each id's span relative to the word start into the slot
+// beside the id (rel, same indexing as slots).  The span of a word's ids is a function of the word's bytes and ids, so
+// the occurrences of a representative share it; emit_ids_kernel<true> adds the occurrence's position.
+//   ordinary id  covers units[id] valid units (its recipe without the word-initial U+2581); an invalid unit between
+//                two of them lies inside its span, one in front of its first unit lies in no span
+//   unk id       covers the maximal run of out-of-alphabet valid units that starts at the next valid unit
+//   units = 0    the word-initial "▁" no rule merged: the empty span at the next valid unit
+struct alignas(16) Span64 { unsigned long long lo, hi; };  // (start, end), one 16-byte store
+struct SpanOut {
+  uint2 *rel;                    // per slot: (start, end) relative to the word start
+  const uint32_t *units;         // per id
+  Span64 *spans;                 // per output id: (start, end) in the coordinates of offs
+};
+
+__global__ void __launch_bounds__(128) span_words_kernel(EncArgs a, const uint32_t *__restrict__ list,
+                                                         const unsigned long long *__restrict__ n_list, uint64_t n_items,
+                                                         SpanOut so) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t o0 = a.offs[0];
+  const uint64_t n = list ? *n_list : n_items;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const uint32_t w = list ? list[i] : (uint32_t)i;
+    const uint64_t p0 = a.word_pos[w], s = a.word_sent[w];
+    const uint64_t hi = a.offs[s + 1] - o0;
+    const uint64_t slot0 = p0 + 3 * s + 1;
+    const int32_t *t = a.slots + slot0;
+    uint2 *rel = so.rel + slot0;
+    const uint32_t n_tok = a.n_tok[w];
+    // the first valid unit at or after q inside the word: its start (hi if none), code point and length
+    auto next_valid = [&](uint64_t q, uint32_t *cp, uint32_t *l) {
+      while (q < hi && !space_at(a.bytes, q, hi, l)) {
+        *cp = decode_unit(a.bytes, q, hi, l);
+        if (*cp != INVALID_CP) return q;
+        q += *l;
+      }
+      return hi;
+    };
+    uint64_t q = p0;
+    for (uint32_t k = 0; k < n_tok; k++) {
+      const int32_t id = t[k];
+      uint32_t cp = 0, l = 0;
+      uint64_t u = next_valid(q, &cp, &l);
+      const uint64_t start = u;
+      uint64_t end = u;
+      if (id == a.unk_id) {
+        while (u < hi && a.cp2id[cp] == NO_ID) { end = u + l; u = next_valid(end, &cp, &l); }
+      } else {
+        for (uint32_t m = so.units[id]; m && u < hi; m--) { end = u + l; if (m > 1) u = next_valid(end, &cp, &l); }
+      }
+      q = end;
+      rel[k] = make_uint2((uint32_t)(start - p0), (uint32_t)(end - p0));
+    }
+  }
+}
+
+template <bool SPANS>
 __global__ void __launch_bounds__(256) emit_ids_kernel(EncArgs a, const uint32_t *__restrict__ rep,
-                                                       const unsigned long long *__restrict__ out_off, int32_t *__restrict__ out) {
+                                                       const unsigned long long *__restrict__ out_off, int32_t *__restrict__ out,
+                                                       SpanOut so) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
@@ -715,6 +779,11 @@ __global__ void __launch_bounds__(256) emit_ids_kernel(EncArgs a, const uint32_t
     if (lane == 0) {
       if (a.bos) out[at(0)] = a.bos_id;
       if (a.eos) out[at(total - 1)] = a.eos_id;
+      if constexpr (SPANS) {
+        const unsigned long long lo = a.offs[s], hi = a.offs[s + 1];
+        if (a.bos) so.spans[at(0)] = Span64{lo, lo};
+        if (a.eos) so.spans[at(total - 1)] = Span64{hi, hi};
+      }
     }
     unsigned long long pos = a.bos ? 1 : 0;
     for (uint32_t i0 = 0; i0 < nw; i0 += 32) {  // warp-uniform
@@ -731,12 +800,69 @@ __global__ void __launch_bounds__(256) emit_ids_kernel(EncArgs a, const uint32_t
       }
       const uint32_t all = __shfl_sync(0xffffffffu, x, 31);
       if (n) {
-        const int32_t *src = a.slots + ((uint64_t)a.word_pos[r] + 3ull * a.word_sent[r] + 1);
+        const uint64_t slot = (uint64_t)a.word_pos[r] + 3ull * a.word_sent[r] + 1;
+        const int32_t *src = a.slots + slot;
         const unsigned long long first = pos + (x - n);
         for (uint32_t k = 0; k < n; k++) out[at(first + k)] = src[k];
+        if constexpr (SPANS) {
+          const unsigned long long wp = a.offs[0] + a.word_pos[w0 + i];  // this occurrence's first byte
+          for (uint32_t k = 0; k < n; k++) {
+            const uint2 rs = so.rel[slot + k];
+            so.spans[at(first + k)] = Span64{wp + rs.x, wp + rs.y};
+          }
+        }
       }
       pos += all;
     }
+  }
+}
+
+// ---- subwords ---------------------------------------------------------------------------------------------------
+// One piece per output id: the model's piece of an ordinary id (recipe UTF-8, leading U+2581 kept) or of <BOS> / <EOS>,
+// and for <UNK> the characters of its run: the valid units of its span, copied from the source bytes.
+struct SubArgs {
+  const int32_t *ids;
+  const Span64 *spans;
+  uint64_t n;                  // ids
+  const uint8_t *bytes;        // batch bytes; span value v is batch byte v - offs[0]
+  const uint64_t *offs;
+  const uint32_t *piece_off;   // V + 1
+  const uint8_t *piece_bytes;
+  int32_t unk_id;
+};
+
+__global__ void __launch_bounds__(256) sub_count_kernel(SubArgs a, unsigned long long *__restrict__ len) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t o0 = a.offs[0];
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < a.n; j += stride) {
+    const int32_t id = a.ids[j];
+    if (id != a.unk_id) { len[j] = __ldg(a.piece_off + id + 1) - __ldg(a.piece_off + id); continue; }
+    const Span64 sp = a.spans[j];
+    unsigned long long m = 0;
+    uint32_t l;
+    for (uint64_t q = sp.lo - o0, e = sp.hi - o0; q < e; q += l)
+      if (decode_unit(a.bytes, q, e, &l) != INVALID_CP) m += l;
+    len[j] = m;
+  }
+}
+
+__global__ void __launch_bounds__(256) sub_emit_kernel(SubArgs a, const unsigned long long *__restrict__ off,
+                                                       uint8_t *__restrict__ out) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t o0 = a.offs[0];
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < a.n; j += stride) {
+    const int32_t id = a.ids[j];
+    uint8_t *dst = out + off[j];
+    if (id != a.unk_id) {
+      const uint32_t b = __ldg(a.piece_off + id), e = __ldg(a.piece_off + id + 1);
+      for (uint32_t k = b; k < e; k++) *dst++ = __ldg(a.piece_bytes + k);
+      continue;
+    }
+    const Span64 sp = a.spans[j];
+    uint32_t l;
+    for (uint64_t q = sp.lo - o0, e = sp.hi - o0; q < e; q += l)
+      if (decode_unit(a.bytes, q, e, &l) != INVALID_CP)
+        for (uint32_t k = 0; k < l; k++) *dst++ = a.bytes[q + k];
   }
 }
 
@@ -751,13 +877,60 @@ __global__ void __launch_bounds__(256) add_base_kernel(unsigned long long *__res
 
 namespace {
 
+// what an encode call computes: ids; ids + spans; ids + spans + subword pieces
+enum EncMode { ENC_IDS = 0, ENC_SPANS = 1, ENC_SUBWORDS = 2 };
+
+// The subword piece and the unit count of every id, one upload (the first spans / subwords call of an encoder).
+int build_sub_table(yttm_enc *e) {
+  yttm_ctx *c = e->ctx;
+  const uint64_t V = e->vocab;
+  std::vector<std::string> raw;
+  std::vector<uint8_t> special;
+  if (yttm_model_pieces(e, "encode", &raw, &special)) return 1;
+  std::vector<uint32_t> head(2 * V + 1);  // piece_off[V + 1] | units[V]
+  uint64_t total = 0;
+  for (uint64_t i = 0; i < V; i++) {
+    head[i] = (uint32_t)total;
+    total += raw[i].size();
+    if (total > 0xffffff00ull) YT_FAIL(c, "encode: piece table over 4 GB");
+    uint32_t u = 0;
+    if (!special[i]) {
+      for (unsigned char b : raw[i]) u += (b & 0xc0) != 0x80;  // code points of valid UTF-8
+      if (raw[i].compare(0, 3, "\xe2\x96\x81") == 0) u -= 1;    // the word-initial U+2581 covers no unit
+    }
+    head[V + 1 + i] = u;
+  }
+  head[V] = (uint32_t)total;
+  const uint64_t a_bytes = ((2 * V + 1) * 4 + 15) & ~15ull, size = a_bytes + total + 16;
+  std::vector<uint8_t> h(size, 0);
+  std::memcpy(h.data(), head.data(), head.size() * 4);
+  for (uint64_t i = 0; i < V; i++) std::memcpy(h.data() + a_bytes + head[i], raw[i].data(), raw[i].size());
+  YT_CUDA(c, e->sub_table.reserve(size));
+  YT_CUDA(c, cudaMemcpyAsync(e->sub_table.p, h.data(), size, cudaMemcpyHostToDevice, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  e->sub_piece_off = e->sub_table.as<uint32_t>();
+  e->sub_units = e->sub_piece_off + V + 1;
+  e->sub_bytes = e->sub_table.as<uint8_t>() + a_bytes;
+  return 0;
+}
+
+// Encodes one batch on the device.  mode >= ENC_SPANS also writes e->out_spans; ENC_SUBWORDS also the pieces
+// (e->sub_off: out_n + 1 byte offsets, e->sub_out: *out_bytes bytes).
 int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const uint64_t *d_offs, uint64_t n_bytes,
                uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence,
-               uint64_t *out_n) {
+               uint64_t *out_n, int mode = ENC_IDS, uint64_t *out_bytes = nullptr) {
   yttm_ctx *c = enc->ctx;
   if (n_bytes >= 0xfffffff0ull || n_sent >= 0xfffffff0ull)
     YT_FAIL(c, "encode batch too large: at most 2^32 bytes / sentences per call (split the batch)");
   const uint64_t n_slots = n_bytes + 3 * n_sent;
+  if (out_bytes) *out_bytes = 0;
+  SpanOut so{nullptr, nullptr, nullptr};
+  if (mode != ENC_IDS) {
+    if (!enc->sub_piece_off && build_sub_table(enc)) return 1;
+    YT_CUDA(c, e->rel.reserve((n_slots + 8) * 8));
+    so.rel = e->rel.as<uint2>();
+    so.units = enc->sub_units;
+  }
   YT_CUDA(c, e->slots.reserve((n_slots + 8) * 4));
   YT_CUDA(c, e->ranks.reserve((n_slots + 8) * 4));
   if (dropout > 0) YT_CUDA(c, e->aux.reserve((n_slots + 8) * 24));
@@ -847,9 +1020,21 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
       encode_long_words_kernel<<<(unsigned)c->n_sm, LONG_T, 0, c->stream>>>(a, ll);
       c->launches++;
       ytc::timer_end(c, "enc_rep");
+      if (mode != ENC_IDS) {
+        ytc::timer_begin(c, "enc_spans");
+        span_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, d.list, d.n_list, 0, so);
+        ytc::timer_end(c, "enc_spans");
+        c->launches++;
+      }
     } else {
       encode_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, n_words);
       c->launches++;
+      if (mode != ENC_IDS) {
+        ytc::timer_begin(c, "enc_spans");
+        span_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, nullptr, nullptr, n_words, so);
+        ytc::timer_end(c, "enc_spans");
+        c->launches++;
+      }
     }
     ytc::timer_end(c, "enc_words");
   }
@@ -870,15 +1055,166 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
                              c->stream));
   YT_CUDA(c, cudaStreamSynchronize(c->stream));
   YT_CUDA(c, e->out_ids.reserve((total + 8) * 4));
-  {
+  if (mode == ENC_IDS) {
     ytc::timer_begin(c, "enc_gather");
-    emit_ids_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a, d_rep, e->out_off.as<unsigned long long>(), e->out_ids.as<int32_t>());
+    emit_ids_kernel<false><<<(unsigned)sblocks, 256, 0, c->stream>>>(a, d_rep, e->out_off.as<unsigned long long>(),
+                                                                     e->out_ids.as<int32_t>(), so);
     ytc::timer_end(c, "enc_gather");
     c->launches++;
+  } else {
+    YT_CUDA(c, e->out_spans.reserve((total + 8) * 16));
+    so.spans = e->out_spans.as<Span64>();
+    ytc::timer_begin(c, "enc_gather");
+    emit_ids_kernel<true><<<(unsigned)sblocks, 256, 0, c->stream>>>(a, d_rep, e->out_off.as<unsigned long long>(),
+                                                                    e->out_ids.as<int32_t>(), so);
+    ytc::timer_end(c, "enc_gather");
+    c->launches++;
+  }
+  if (mode == ENC_SUBWORDS && total == 0) {
+    YT_CUDA(c, e->sub_off.reserve(16));
+    YT_CUDA(c, cudaMemsetAsync(e->sub_off.p, 0, 8, c->stream));
+  } else if (mode == ENC_SUBWORDS) {  // piece lengths -> exclusive scan -> piece bytes
+    SubArgs sa;
+    sa.ids = e->out_ids.as<int32_t>(); sa.spans = so.spans; sa.n = total;
+    sa.bytes = d_bytes; sa.offs = d_offs;
+    sa.piece_off = enc->sub_piece_off; sa.piece_bytes = enc->sub_bytes; sa.unk_id = enc->unk;
+    YT_CUDA(c, e->sub_len.reserve((total + 8) * 8));
+    YT_CUDA(c, e->sub_off.reserve((total + 8) * 8));
+    unsigned long long *sub_off = e->sub_off.as<unsigned long long>();
+    const uint64_t iblocks = std::max<uint64_t>(std::min<uint64_t>((total + 255) / 256, (uint64_t)c->n_sm * 8), 1);
+    ytc::timer_begin(c, "enc_subwords");
+    sub_count_kernel<<<(unsigned)iblocks, 256, 0, c->stream>>>(sa, e->sub_len.as<unsigned long long>());
+    c->launches++;
+    if (yttm_device_scan_u64(c, e->sub_len.as<unsigned long long>(), total, sub_off, d_total)) return 1;
+    unsigned long long n_piece_bytes = 0;
+    YT_CUDA(c, cudaMemcpyAsync(&n_piece_bytes, d_total, 8, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaMemcpyAsync(sub_off + total, d_total, 8, cudaMemcpyDeviceToDevice, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    YT_CUDA(c, e->sub_out.reserve(n_piece_bytes + 16));
+    sub_emit_kernel<<<(unsigned)iblocks, 256, 0, c->stream>>>(sa, sub_off, e->sub_out.as<uint8_t>());
+    c->launches++;
+    ytc::timer_end(c, "enc_subwords");
+    *out_bytes = n_piece_bytes;
   }
   ytc::timer_end(c, "encode");
   YT_CUDA(c, cudaGetLastError());
   *out_n = total;
+  return 0;
+}
+
+// Caller buffers of the host-buffer entry points; nullptr = not asked for.  ids_cap bounds ids / spans / pieces (one
+// piece per id), bytes_cap the piece bytes.
+struct HostOut {
+  int mode;
+  int32_t *ids;
+  uint64_t *spans;              // 2 per id
+  uint64_t ids_cap;
+  uint64_t *id_offsets;         // n_sent + 1
+  uint8_t *pieces;
+  uint64_t bytes_cap;
+  uint64_t *piece_offsets;      // n_pieces + 1
+};
+
+// The host-buffer form of enc_device: the batch is cut into chunks at sentence boundaries, chunk i runs in slot i & 1
+// while the copies of its neighbours overlap it.  Returns 2 with *out_n / *out_bytes = the sizes needed when a capacity
+// is too small.
+int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos,
+                 int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, const HostOut &o,
+                 uint64_t *out_n, uint64_t *out_bytes) {
+  yttm_ctx *c = e->ctx;
+  *out_n = 0;
+  if (out_bytes) *out_bytes = 0;
+  if (n_sent == 0) {
+    if (o.id_offsets) o.id_offsets[0] = 0;
+    if (o.piece_offsets) o.piece_offsets[0] = 0;
+    return 0;
+  }
+  if (!e->s_in) {
+    YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
+    YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; i++) {
+      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_in[i], cudaEventDisableTiming));
+      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming));
+      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming));
+    }
+  }
+  // chunks of about CHUNK bytes, cut at sentence boundaries; chunk i lives in slot i & 1
+  const uint64_t total_bytes = offsets[n_sent] - offsets[0];
+  uint64_t chunk_bytes = 32ull << 20;
+  if (const char *env = std::getenv("YTTM_ENC_CHUNK_MB")) chunk_bytes = (uint64_t)std::max(1, std::atoi(env)) << 20;
+  std::vector<uint64_t> cut(1, 0);  // sentence indices
+  while (cut.back() < n_sent) {
+    const uint64_t lo = cut.back();
+    const uint64_t want = offsets[lo] + chunk_bytes;
+    uint64_t hi = (uint64_t)(std::upper_bound(offsets + lo + 1, offsets + n_sent + 1, want) - offsets) - 1;
+    if (hi <= lo) hi = lo + 1;  // a single sentence longer than the chunk size
+    if (offsets[n_sent] - offsets[hi] < chunk_bytes / 4) hi = n_sent;  // no tiny tail chunk
+    cut.push_back(std::min<uint64_t>(hi, n_sent));
+  }
+  const size_t K = cut.size() - 1;
+  c->timers["enc_chunks"].ms = (float)K;  // yttm_stage_ms(ctx, "enc_chunks"): how many chunks the last call used
+  auto h2d = [&](size_t i) -> int {  // enqueue the input copies of chunk i on the copy-in stream
+    yttm_enc::Slot &sl = e->slot[i & 1];
+    const uint64_t lo = cut[i], hi = cut[i + 1], nb = offsets[hi] - offsets[lo];
+    YT_CUDA(c, sl.d_bytes.reserve(nb + 64));
+    YT_CUDA(c, sl.d_offs.reserve((hi - lo + 1) * 8));
+    if (i >= 2) YT_CUDA(c, cudaStreamWaitEvent(e->s_in, e->ev_done[i & 1], 0));  // kernels of chunk i-2 are done with it
+    if (nb) YT_CUDA(c, cudaMemcpyAsync(sl.d_bytes.p, bytes + offsets[lo], nb, cudaMemcpyHostToDevice, e->s_in));
+    YT_CUDA(c, cudaMemcpyAsync(sl.d_offs.p, offsets + lo, (hi - lo + 1) * 8, cudaMemcpyHostToDevice, e->s_in));
+    YT_CUDA(c, cudaEventRecord(e->ev_in[i & 1], e->s_in));
+    return 0;
+  };
+  ytc::timer_begin(c, "e2e");
+  if (h2d(0)) return 1;
+  uint64_t base = 0, bbase = 0;  // ids / piece bytes of the chunks before
+  int rc_small = 0;
+  for (size_t i = 0; i < K; i++) {
+    yttm_enc::Slot &sl = e->slot[i & 1];
+    const uint64_t lo = cut[i], hi = cut[i + 1], nb = offsets[hi] - offsets[lo];
+    if (i + 1 < K && h2d(i + 1)) return 1;
+    YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_in[i & 1], 0));
+    if (i >= 2) YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_out[i & 1], 0));  // results of chunk i-2 have left
+    uint64_t total = 0, tbytes = 0;
+    if (enc_device(e, &sl, sl.d_bytes.as<uint8_t>(), sl.d_offs.as<uint64_t>(), nb, hi - lo, bos, eos, reverse, dropout,
+                   seed, first_sentence_index + lo, &total, o.mode, &tbytes))
+      return 1;
+    if (base && hi > lo) {  // chunk-local offsets -> batch offsets
+      add_base_kernel<<<(unsigned)std::min<uint64_t>((hi - lo + 255) / 256, (uint64_t)c->n_sm * 4), 256, 0, c->stream>>>(
+          sl.out_off.as<unsigned long long>(), hi - lo, (unsigned long long)base);
+      c->launches++;
+    }
+    if (o.piece_offsets && bbase && total) {  // the same for the piece offsets (spans are batch coordinates already)
+      add_base_kernel<<<(unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)c->n_sm * 4), 256, 0, c->stream>>>(
+          sl.sub_off.as<unsigned long long>(), total, (unsigned long long)bbase);
+      c->launches++;
+    }
+    YT_CUDA(c, cudaEventRecord(e->ev_done[i & 1], c->stream));
+    if (base + total > o.ids_cap || bbase + tbytes > o.bytes_cap) rc_small = 2;
+    if (!rc_small) {
+      YT_CUDA(c, cudaStreamWaitEvent(e->s_out, e->ev_done[i & 1], 0));
+      if (total && o.ids)
+        YT_CUDA(c, cudaMemcpyAsync(o.ids + base, sl.out_ids.p, total * 4, cudaMemcpyDeviceToHost, e->s_out));
+      if (total && o.spans)
+        YT_CUDA(c, cudaMemcpyAsync(o.spans + 2 * base, sl.out_spans.p, total * 16, cudaMemcpyDeviceToHost, e->s_out));
+      if (total && o.piece_offsets)
+        YT_CUDA(c, cudaMemcpyAsync(o.piece_offsets + base, sl.sub_off.p, total * 8, cudaMemcpyDeviceToHost, e->s_out));
+      if (tbytes && o.pieces)
+        YT_CUDA(c, cudaMemcpyAsync(o.pieces + bbase, sl.sub_out.p, tbytes, cudaMemcpyDeviceToHost, e->s_out));
+      YT_CUDA(c, cudaMemcpyAsync(o.id_offsets + lo, sl.out_off.p, (hi - lo) * 8, cudaMemcpyDeviceToHost, e->s_out));
+      YT_CUDA(c, cudaEventRecord(e->ev_out[i & 1], e->s_out));
+    }
+    base += total;
+    bbase += tbytes;
+  }
+  YT_CUDA(c, cudaStreamSynchronize(e->s_out));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  ytc::timer_end(c, "e2e");
+  *out_n = base;
+  if (out_bytes) *out_bytes = bbase;
+  if (rc_small) { c->err = std::string(who) + ": output buffer too small"; return 2; }
+  o.id_offsets[n_sent] = base;
+  if (o.piece_offsets) o.piece_offsets[base] = bbase;
+  (void)total_bytes;
   return 0;
 }
 
@@ -940,6 +1276,7 @@ void yttm_enc_destroy(yttm_enc *e) {
   cudaSetDevice(e->ctx->device);
   e->cp2id.release();
   e->rules.release();
+  e->sub_table.release();
   yttm_dec_free(e->dec);
   for (int i = 0; i < 2; i++) {
     e->slot[i].release();
@@ -976,81 +1313,78 @@ int yttm_enc_run(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64
   YT_CUDA(c, cudaSetDevice(c->device));
   if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
   if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
-  *out_n = 0;
-  if (n_sent == 0) { if (out_offsets) out_offsets[0] = 0; return 0; }
-  if (!e->s_in) {
-    YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
-    YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_in[i], cudaEventDisableTiming));
-      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming));
-      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming));
-    }
-  }
-  // chunks of about CHUNK bytes, cut at sentence boundaries; chunk i lives in slot i & 1
-  const uint64_t total_bytes = offsets[n_sent] - offsets[0];
-  uint64_t chunk_bytes = 32ull << 20;
-  if (const char *env = std::getenv("YTTM_ENC_CHUNK_MB")) chunk_bytes = (uint64_t)std::max(1, std::atoi(env)) << 20;
-  std::vector<uint64_t> cut(1, 0);  // sentence indices
-  while (cut.back() < n_sent) {
-    const uint64_t lo = cut.back();
-    const uint64_t want = offsets[lo] + chunk_bytes;
-    uint64_t hi = (uint64_t)(std::upper_bound(offsets + lo + 1, offsets + n_sent + 1, want) - offsets) - 1;
-    if (hi <= lo) hi = lo + 1;  // a single sentence longer than the chunk size
-    if (offsets[n_sent] - offsets[hi] < chunk_bytes / 4) hi = n_sent;  // no tiny tail chunk
-    cut.push_back(std::min<uint64_t>(hi, n_sent));
-  }
-  const size_t K = cut.size() - 1;
-  c->timers["enc_chunks"].ms = (float)K;  // yttm_stage_ms(ctx, "enc_chunks"): how many chunks the last call used
-  auto h2d = [&](size_t i) -> int {  // enqueue the input copies of chunk i on the copy-in stream
-    yttm_enc::Slot &sl = e->slot[i & 1];
-    const uint64_t lo = cut[i], hi = cut[i + 1], nb = offsets[hi] - offsets[lo];
-    YT_CUDA(c, sl.d_bytes.reserve(nb + 64));
-    YT_CUDA(c, sl.d_offs.reserve((hi - lo + 1) * 8));
-    if (i >= 2) YT_CUDA(c, cudaStreamWaitEvent(e->s_in, e->ev_done[i & 1], 0));  // kernels of chunk i-2 are done with it
-    if (nb) YT_CUDA(c, cudaMemcpyAsync(sl.d_bytes.p, bytes + offsets[lo], nb, cudaMemcpyHostToDevice, e->s_in));
-    YT_CUDA(c, cudaMemcpyAsync(sl.d_offs.p, offsets + lo, (hi - lo + 1) * 8, cudaMemcpyHostToDevice, e->s_in));
-    YT_CUDA(c, cudaEventRecord(e->ev_in[i & 1], e->s_in));
-    return 0;
-  };
-  ytc::timer_begin(c, "e2e");
-  if (h2d(0)) return 1;
-  uint64_t base = 0;
-  int rc_small = 0;
-  for (size_t i = 0; i < K; i++) {
-    yttm_enc::Slot &sl = e->slot[i & 1];
-    const uint64_t lo = cut[i], hi = cut[i + 1], nb = offsets[hi] - offsets[lo];
-    if (i + 1 < K && h2d(i + 1)) return 1;
-    YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_in[i & 1], 0));
-    if (i >= 2) YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_out[i & 1], 0));  // results of chunk i-2 have left
-    uint64_t total = 0;
-    if (enc_device(e, &sl, sl.d_bytes.as<uint8_t>(), sl.d_offs.as<uint64_t>(), nb, hi - lo, bos, eos, reverse, dropout,
-                   seed, first_sentence_index + lo, &total))
-      return 1;
-    if (base && hi > lo) {  // chunk-local offsets -> batch offsets
-      add_base_kernel<<<(unsigned)std::min<uint64_t>((hi - lo + 255) / 256, (uint64_t)c->n_sm * 4), 256, 0, c->stream>>>(
-          sl.out_off.as<unsigned long long>(), hi - lo, (unsigned long long)base);
-      c->launches++;
-    }
-    YT_CUDA(c, cudaEventRecord(e->ev_done[i & 1], c->stream));
-    if (base + total > out_cap) rc_small = 2;
-    if (!rc_small) {
-      YT_CUDA(c, cudaStreamWaitEvent(e->s_out, e->ev_done[i & 1], 0));
-      if (total)
-        YT_CUDA(c, cudaMemcpyAsync(out_ids + base, sl.out_ids.p, total * 4, cudaMemcpyDeviceToHost, e->s_out));
-      YT_CUDA(c, cudaMemcpyAsync(out_offsets + lo, sl.out_off.p, (hi - lo) * 8, cudaMemcpyDeviceToHost, e->s_out));
-      YT_CUDA(c, cudaEventRecord(e->ev_out[i & 1], e->s_out));
-    }
-    base += total;
-  }
-  YT_CUDA(c, cudaStreamSynchronize(e->s_out));
-  YT_CUDA(c, cudaStreamSynchronize(c->stream));
-  ytc::timer_end(c, "e2e");
-  *out_n = base;
-  if (rc_small) { c->err = "yttm_enc_run: output buffer too small"; return 2; }
-  out_offsets[n_sent] = base;
-  (void)total_bytes;
+  const HostOut o{ENC_IDS, out_ids, nullptr, out_cap, out_offsets, nullptr, ~0ull, nullptr};
+  return enc_run_host(e, "yttm_enc_run", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed, first_sentence_index, o,
+                      out_n, nullptr);
+}
+
+// the checks every encode entry point makes before it runs
+#define YT_ENC_ENTRY(e, name)                                                                                         \
+  if (!e) { g_yttm_create_error = name ": null encoder handle (no CUDA device, or yttm_enc_create failed)"; return 1; } \
+  yttm_ctx *c = e->ctx;                                                                                                \
+  YT_CUDA(c, cudaSetDevice(c->device));                                                                                \
+  if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");                         \
+  if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
+
+int yttm_enc_run_spans_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                              int bos, int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index,
+                              const int32_t **d_out_ids, const uint64_t **d_out_offsets, const uint64_t **d_out_spans,
+                              uint64_t *out_n) {
+  YT_ENC_ENTRY(e, "yttm_enc_run_spans_device")
+  yttm_enc::Slot &sl = e->slot[0];
+  if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
+                 first_sentence_index, out_n, ENC_SPANS))
+    return 1;
+  YT_CUDA(c, sl.out_off.reserve(16));
+  YT_CUDA(c, sl.out_ids.reserve(16));
+  YT_CUDA(c, sl.out_spans.reserve(16));
+  if (n_sent == 0) YT_CUDA(c, cudaMemsetAsync(sl.out_off.p, 0, 8, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));  // the results are complete for readers on any stream
+  if (d_out_ids) *d_out_ids = sl.out_ids.as<int32_t>();
+  if (d_out_offsets) *d_out_offsets = sl.out_off.as<uint64_t>();
+  if (d_out_spans) *d_out_spans = sl.out_spans.as<uint64_t>();
   return 0;
 }
 
+int yttm_enc_run_spans(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                       int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, int32_t *out_ids,
+                       uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_spans, uint64_t *out_n) {
+  YT_ENC_ENTRY(e, "yttm_enc_run_spans")
+  const HostOut o{ENC_SPANS, out_ids, out_spans, out_cap, out_offsets, nullptr, ~0ull, nullptr};
+  return enc_run_host(e, "yttm_enc_run_spans", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
+                      first_sentence_index, o, out_n, nullptr);
+}
+
+int yttm_enc_run_subwords_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                 uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                                 uint64_t first_sentence_index, const uint8_t **d_pieces, const uint64_t **d_piece_offsets,
+                                 const uint64_t **d_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes) {
+  YT_ENC_ENTRY(e, "yttm_enc_run_subwords_device")
+  yttm_enc::Slot &sl = e->slot[0];
+  if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
+                 first_sentence_index, n_pieces, ENC_SUBWORDS, n_piece_bytes))
+    return 1;
+  YT_CUDA(c, sl.out_off.reserve(16));
+  YT_CUDA(c, sl.sub_off.reserve(16));
+  YT_CUDA(c, sl.sub_out.reserve(16));
+  if (n_sent == 0) {
+    YT_CUDA(c, cudaMemsetAsync(sl.out_off.p, 0, 8, c->stream));
+    YT_CUDA(c, cudaMemsetAsync(sl.sub_off.p, 0, 8, c->stream));
+  }
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (d_pieces) *d_pieces = sl.sub_out.as<uint8_t>();
+  if (d_piece_offsets) *d_piece_offsets = sl.sub_off.as<uint64_t>();
+  if (d_sent_offsets) *d_sent_offsets = sl.out_off.as<uint64_t>();
+  return 0;
+}
+
+int yttm_enc_run_subwords(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                          int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, uint8_t *out_pieces,
+                          uint64_t bytes_cap, uint64_t *out_piece_offsets, uint64_t pieces_cap, uint64_t *out_sent_offsets,
+                          uint64_t *n_pieces, uint64_t *n_piece_bytes) {
+  YT_ENC_ENTRY(e, "yttm_enc_run_subwords")
+  const HostOut o{ENC_SUBWORDS, nullptr, nullptr, pieces_cap, out_sent_offsets, out_pieces, bytes_cap, out_piece_offsets};
+  return enc_run_host(e, "yttm_enc_run_subwords", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
+                      first_sentence_index, o, n_pieces, n_piece_bytes);
+}
 }  // extern "C"

@@ -1,8 +1,9 @@
 """The reference's Python surface (youtokentome/youtokentome.py:1-99 + the Cython class
 youtokentome/cpp/yttm.pyx:52-181) over the CUDA library: same class, method names, argument
 meaning, return types and exceptions (ValueError(status.message), TypeError for bad argument
-types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path), `decode_packed` (its inverse,
-on the GPU) and `dropout_seed`."""
+types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path, optionally with the source byte
+span of every id), `encode_subwords_packed` (the subword pieces on the GPU), `decode_packed` (the inverse of
+`encode_packed`, on the GPU) and `dropout_seed`."""
 import ctypes as C
 import threading
 from collections.abc import Collection
@@ -25,6 +26,12 @@ def _pack(sentences):
     if enc:
         np.cumsum([len(b) for b in enc], out=offs[1:])
     return b"".join(enc), offs
+
+
+def _check_dropout(dropout_prob):  # yttm.pyx:92-93
+    if dropout_prob < 0 or dropout_prob > 1:
+        raise ValueError("dropout_prob value must be in the range [0, 1]. Current value of dropout_prob = " +
+                         str(dropout_prob))
 
 
 def _offsets_error(n_ids):  # the library's text for the same error
@@ -67,14 +74,21 @@ class BPE:
         return BPE(model=model, n_threads=n_threads)
 
     # -- encode ---------------------------------------------------------------------------------
-    def encode_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy"):
+    def encode_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy",
+                      with_spans=False):
         """Additive fast path (no Python lists; replaces the marshalling of yttm.pyx:96-107): sentence i =
         data[offsets[i]:offsets[i+1]].  `data`: bytes / numpy uint8 / torch uint8 tensor (CPU or CUDA); `offsets`:
         uint64 array (or int64 tensor).  Returns (ids int32, id_offsets) as
           out="numpy"  numpy arrays (one call into buffers allocated here),
           out="torch"  CPU torch tensors (pinned if the input was),
           out="cuda"   CUDA torch tensors: input uploaded if needed, results stay on the device
-                       (yttm_enc_run_device; nothing touches the host)."""
+                       (yttm_enc_run_device; nothing touches the host).
+        with_spans=True returns (ids, id_offsets, spans) with the same ids: spans[j] = (start, end) of the bytes id j
+        came from, in the coordinates of `offsets` (data[start:end]); shape (n_ids, 2), dtype and device of
+        id_offsets.  An id covers a run of its word's units (code points or invalid bytes) and the invalid bytes
+        between them; the word-initial "▁" and <BOS> / <EOS> have empty spans (yttm_enc_run_spans in yttm_b200.h)."""
+        if with_spans:
+            return self._encode_extra("spans", data, offsets, bos, eos, reverse, dropout_prob, out)
         L = _lib.lib()
         if out not in ("numpy", "torch", "cuda"):
             raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
@@ -145,6 +159,125 @@ class BPE:
             return ids.cpu(), oo.cpu()
         return ids.cpu().numpy(), oo.cpu().numpy().astype(np.uint64)
 
+    def encode_subwords_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy"):
+        """encode(output_type=SUBWORD) of a packed batch on the GPU (inputs as for encode_packed).  Returns
+        (piece_bytes uint8, piece_offsets, sentence_offsets): piece k = piece_bytes[piece_offsets[k]:piece_offsets[k+1]]
+        as UTF-8, the pieces of sentence i = [sentence_offsets[i], sentence_offsets[i+1]); offsets are uint64 numpy
+        arrays for out="numpy", int64 tensors for "torch" / "cuda"."""
+        return self._encode_extra("subwords", data, offsets, bos, eos, reverse, dropout_prob, out)
+
+    def _encode_extra(self, kind, data, offsets, bos, eos, reverse, dropout_prob, out):
+        """encode_packed(with_spans=True) / encode_subwords_packed."""
+        if out not in ("numpy", "torch", "cuda"):
+            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+        _check_dropout(dropout_prob)
+        is_torch = type(data).__module__.startswith("torch")
+        if out == "cuda" or (is_torch and data.is_cuda):
+            return self._encode_extra_device(kind, data, offsets, bos, eos, reverse, dropout_prob, out)
+        L = _lib.lib()
+        if is_torch:
+            keep = data = data.contiguous()
+            ptr, n_bytes = data.data_ptr(), data.numel()
+        elif isinstance(data, np.ndarray):
+            keep = data = np.ascontiguousarray(data)
+            ptr, n_bytes = data.ctypes.data, data.nbytes
+        else:
+            keep = data = bytes(data) if not isinstance(data, bytes) else data
+            ptr, n_bytes = C.cast(C.c_char_p(data), C.c_void_p), len(data)
+        if type(offsets).__module__.startswith("torch"):
+            offsets = offsets.cpu().numpy()
+        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
+        n = len(offsets) - 1
+        if n < 0:
+            raise ValueError("offsets must hold at least one value")
+        cap = int(n_bytes) + 3 * n + 16   # ids of a sentence of L bytes: at most L + 1 (+ <BOS> + <EOS>)
+        args = (self._h, ptr, offsets.ctypes.data, n, int(bos), int(eos), int(reverse), float(dropout_prob))
+        if kind == "spans":
+            total = C.c_uint64(0)
+            if out == "torch":
+                import torch
+                pin = is_torch and data.is_pinned()
+                ids = torch.empty(cap, dtype=torch.int32, pin_memory=pin)
+                oo = torch.empty(n + 1, dtype=torch.int64, pin_memory=pin)
+                spans = torch.empty((cap, 2), dtype=torch.int64, pin_memory=pin)
+                ptrs = ids.data_ptr(), oo.data_ptr(), spans.data_ptr()
+            else:
+                ids, oo = np.empty(cap, dtype=np.int32), np.empty(n + 1, dtype=np.uint64)
+                spans = np.empty((cap, 2), dtype=np.uint64)
+                ptrs = ids.ctypes.data, oo.ctypes.data, spans.ctypes.data
+            rc = L.yttm_api_encode_spans_into(*args, ptrs[0], cap, ptrs[1], ptrs[2], C.byref(total))
+            del keep
+            if rc != 0:
+                raise self._err()
+            return ids[:total.value], oo, spans[:total.value]
+        # a piece is its units' bytes plus a leading U+2581 (3 bytes, at most one per word) or "<BOS>" / "<EOS>"
+        bytes_cap = 4 * int(n_bytes) + 10 * n + 16
+        text = np.empty(bytes_cap, dtype=np.uint8)
+        po = np.empty(cap + 1, dtype=np.uint64)
+        so = np.empty(n + 1, dtype=np.uint64)
+        n_p, n_b = C.c_uint64(0), C.c_uint64(0)
+        rc = L.yttm_api_encode_subwords_into(*args, text.ctypes.data, bytes_cap, po.ctypes.data, cap, so.ctypes.data,
+                                             C.byref(n_p), C.byref(n_b))
+        del keep
+        if rc != 0:
+            raise self._err()
+        text, po = text[:n_b.value].copy(), po[:n_p.value + 1].copy()
+        if out == "torch":
+            import torch
+            return torch.from_numpy(text), torch.from_numpy(po.astype(np.int64)), torch.from_numpy(so.astype(np.int64))
+        return text, po, so
+
+    def _encode_extra_device(self, kind, data, offsets, bos, eos, reverse, dropout_prob, out):
+        import torch
+        from .distributed import _DevView
+        L = _lib.lib()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if type(data).__module__.startswith("torch"):
+            d_bytes = data.to(dev, non_blocking=True).contiguous()
+        else:
+            raw = data if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).tobytes()
+            d_bytes = (torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev) if raw
+                       else torch.empty(0, dtype=torch.uint8, device=dev))
+        if type(offsets).__module__.startswith("torch"):
+            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
+        else:
+            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
+        n = d_offs.numel() - 1
+        if n < 0:
+            raise ValueError("offsets must hold at least one value")
+        first, last = (int(v) for v in d_offs[[0, n]].cpu())
+        # the library reads sentence 0 at the byte pointer it gets: the byte at offsets[0]
+        args = (self._h, d_bytes.data_ptr() + first, d_offs.data_ptr(), last - first, n, int(bos), int(eos), int(reverse),
+                float(dropout_prob))
+        p = [C.c_void_p() for _ in range(3)]
+        n_a, n_b = C.c_uint64(0), C.c_uint64(0)
+
+        def view(ptr, k, ts):
+            if k == 0:
+                return torch.empty(0, dtype={"|u1": torch.uint8, "<i4": torch.int32, "<i8": torch.int64}[ts], device=dev)
+            return torch.as_tensor(_DevView(ptr.value, k, ts), device=dev).clone()
+
+        torch.cuda.synchronize()   # the library runs on its own stream
+        with self._dev_lock:       # the result pointers are valid until the next encode on this handle: copy under the lock
+            if kind == "spans":
+                rc = L.yttm_api_encode_spans_device(*args, C.byref(p[0]), C.byref(p[1]), C.byref(p[2]), C.byref(n_a))
+                if rc != 0:
+                    raise self._err()
+                res = (view(p[0], n_a.value, "<i4"), view(p[1], n + 1, "<i8"),
+                       view(p[2], 2 * n_a.value, "<i8").view(n_a.value, 2))
+            else:
+                rc = L.yttm_api_encode_subwords_device(*args, C.byref(p[0]), C.byref(p[1]), C.byref(p[2]), C.byref(n_a),
+                                                       C.byref(n_b))
+                if rc != 0:
+                    raise self._err()
+                res = (view(p[0], n_b.value, "|u1"), view(p[1], n_a.value + 1, "<i8"), view(p[2], n + 1, "<i8"))
+            torch.cuda.synchronize()
+        if out == "cuda":
+            return res
+        if out == "torch":
+            return tuple(t.cpu() for t in res)
+        return tuple(t.cpu().numpy() if t.dtype == torch.uint8 else t.cpu().numpy().astype(np.uint64) for t in res)
+
     def _pieces(self, need):
         """The calling thread's last length-framed piece list -> list of sentences, each a list of str."""
         L = _lib.lib()
@@ -163,9 +296,7 @@ class BPE:
                eos: bool = False, reverse: bool = False, dropout_prob: float = 0):
         if not isinstance(output_type, OutputType):
             raise TypeError("parameter output_type must be youtokentome.OutputType, not %s}" % str(type(output_type)))
-        if dropout_prob < 0 or dropout_prob > 1:  # yttm.pyx:92-93
-            raise ValueError("dropout_prob value must be in the range [0, 1]. Current value of dropout_prob = " +
-                             str(dropout_prob))
+        _check_dropout(dropout_prob)
         single = isinstance(sentences, str)
         if not single:
             assert isinstance(sentences, (list, tuple))
