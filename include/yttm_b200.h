@@ -79,7 +79,13 @@ int yttm_train_build(yttm_ctx *ctx, yttm_train_stats *stats);
 
 /* Multi-GPU word exchange (round 1, kept for callers that gather through the host): export this rank's unique
  * words (tokens, offsets[n_unique+1], freq) to host buffers, or import a concatenation of all ranks' exports and
- * rebuild the pair table from it (duplicates across ranks are harmless: statistics are additive). */
+ * rebuild the pair table from it (duplicates across ranks are harmless: statistics are additive).
+ * Preconditions of an imported word set, which words built by the trainer always meet:
+ *   - the first token of a word appears at no other position of any word (the role of U+2581: the STREAMING merge
+ *     loop relies on it, a pair never straddles two tiles);
+ *   - token ids and first_new_id + max_merges of the following yttm_train_run stay below 2^22;
+ *   - freq[i] x (tokens of word i) < 2^43: a count change travels through the merge loop as a signed 44-bit value
+ *     (checked: import_words fails otherwise).  Pair counts themselves are 64-bit. */
 int yttm_train_export_words(yttm_ctx *ctx, uint32_t *tokens, uint64_t tokens_cap, uint32_t *offsets,
                             uint64_t *freq, uint64_t words_cap, uint64_t *n_words, uint64_t *n_tokens);
 int yttm_train_import_words(yttm_ctx *ctx, const uint32_t *tokens, uint64_t n_tokens, const uint32_t *offsets,

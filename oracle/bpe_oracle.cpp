@@ -119,6 +119,68 @@ static void for_each_pair(const std::vector<uint32_t> &w, F f) {
 
 struct TrainStats { uint64_t data_len = 0, n_words = 0, n_unique = 0, n_tokens = 0, n_merges = 0; };
 
+struct MergeRule { uint32_t x, y, z; uint64_t cnt; };  // cnt: count of (x, y) at merge time
+
+// Phases 3-4 over a list of words (bpe.cpp:436-478, main :1121-1282, worker :601-811): pair counts under the run
+// rule weighted by wfreq, then up to max_merges merges with new ids first_new_id, first_new_id + 1, ...  `words` is
+// rewritten in place; *live receives the pair counts after the last merge (zero counts included).  Equal words may
+// appear more than once: their statistics add up.  A word of fewer than 2 tokens carries no pair.
+static void merge_words(std::vector<std::vector<uint32_t>> &words, const std::vector<uint64_t> &wfreq,
+                        uint32_t first_new_id, uint64_t max_merges, std::vector<MergeRule> *rules,
+                        std::unordered_map<uint64_t, uint64_t> *live) {
+  std::unordered_map<uint64_t, uint64_t> cnt;
+  std::unordered_map<uint64_t, std::vector<uint32_t>> where;  // pair -> words that (once) held it
+  std::set<Cand> order;                                        // all pairs with cnt > 0
+  for (uint32_t wi = 0; wi < words.size(); wi++) {
+    for_each_pair(words[wi], [&](uint64_t k, uint64_t c) {
+      cnt[k] += c * wfreq[wi];
+      auto &v = where[k];
+      if (v.empty() || v.back() != wi) v.push_back(wi);
+    });
+  }
+  for (auto &kv : cnt) order.insert({kv.second, (uint32_t)(kv.first >> 32), (uint32_t)kv.first});
+
+  auto add = [&](uint64_t k, int64_t d) {
+    if (d == 0) return;
+    uint64_t &c = cnt[k];
+    if (c) order.erase({c, (uint32_t)(k >> 32), (uint32_t)k});
+    c = (uint64_t)((int64_t)c + d);
+    if (c) order.insert({c, (uint32_t)(k >> 32), (uint32_t)k});
+  };
+
+  std::vector<uint32_t> nw;
+  std::unordered_map<uint64_t, int64_t> delta;  // count changes of one merge, applied before the next election
+  for (uint64_t m = 0; m < max_merges; m++) {
+    if (order.empty()) break;  // "WARNING merged only" (bpe.cpp:1137-1145)
+    Cand best = *order.rbegin();
+    uint32_t x = best.x, y = best.y, z = first_new_id + (uint32_t)m;
+    rules->push_back({x, y, z, best.cnt});
+    std::vector<uint32_t> affected;
+    affected.swap(where[key(x, y)]);
+    delta.clear();
+    for (uint32_t wi : affected) {
+      auto &w = words[wi];
+      nw.clear();
+      bool any = false;
+      for (size_t i = 0; i < w.size();) {  // greedy left to right (stress_test.cpp:181-188)
+        if (i + 1 < w.size() && w[i] == x && w[i + 1] == y) { nw.push_back(z); i += 2; any = true; }
+        else nw.push_back(w[i++]);
+      }
+      if (!any) continue;
+      int64_t f = (int64_t)wfreq[wi];
+      for_each_pair(w, [&](uint64_t k, uint64_t c) { delta[k] -= (int64_t)c * f; });
+      w = nw;
+      for_each_pair(w, [&](uint64_t k, uint64_t c) {
+        delta[k] += (int64_t)c * f;
+        auto &v = where[k];
+        if (v.empty() || v.back() != wi) v.push_back(wi);
+      });
+    }
+    for (auto &kv : delta) add(kv.first, kv.second);
+  }
+  if (live) live->swap(cnt);
+}
+
 // learn_bpe_from_string (bpe.cpp:859-1293) without the thread choreography.
 // Returns "" or an error message (bpe.cpp:1053-1062).
 static std::string train(const uint8_t *text, uint64_t n, int vocab_size, double coverage, Model *m, TrainStats *st) {
@@ -173,59 +235,13 @@ static std::string train(const uint8_t *text, uint64_t n, int vocab_size, double
   for (auto &kv : wmap) { words.push_back(kv.first); wfreq.push_back(kv.second); }
   wmap.clear();
 
-  // phase 3: pair counts + inverted index (bpe.cpp:436-478)
-  std::unordered_map<uint64_t, uint64_t> cnt;
-  std::unordered_map<uint64_t, std::vector<uint32_t>> where;  // pair -> words that (once) held it
-  std::set<Cand> order;                                        // all pairs with cnt > 0
   uint64_t ntok = 0;
-  for (uint32_t wi = 0; wi < words.size(); wi++) {
-    ntok += words[wi].size();
-    for_each_pair(words[wi], [&](uint64_t k, uint64_t c) {
-      cnt[k] += c * wfreq[wi];
-      auto &v = where[k];
-      if (v.empty() || v.back() != wi) v.push_back(wi);
-    });
-  }
-  for (auto &kv : cnt) order.insert({kv.second, (uint32_t)(kv.first >> 32), (uint32_t)kv.first});
+  for (auto &w : words) ntok += w.size();
   if (st) { st->data_len = data_len; st->n_unique = words.size(); st->n_tokens = ntok; }
 
-  auto add = [&](uint64_t k, int64_t d) {
-    if (d == 0) return;
-    uint64_t &c = cnt[k];
-    if (c) order.erase({c, (uint32_t)(k >> 32), (uint32_t)k});
-    c = (uint64_t)((int64_t)c + d);
-    if (c) order.insert({c, (uint32_t)(k >> 32), (uint32_t)k});
-  };
-
-  // phase 4: merge loop (bpe.cpp:1121-1282 main, :601-811 worker)
-  std::vector<Rule> rules;
-  std::vector<uint32_t> nw;
-  while ((int64_t)used < (int64_t)vocab_size) {
-    if (order.empty()) break;  // "WARNING merged only" (bpe.cpp:1137-1145)
-    Cand best = *order.rbegin();
-    uint32_t x = best.x, y = best.y, z = used++;
-    rules.push_back({x, y, z});
-    std::vector<uint32_t> affected;
-    affected.swap(where[key(x, y)]);
-    for (uint32_t wi : affected) {
-      auto &w = words[wi];
-      nw.clear();
-      bool any = false;
-      for (size_t i = 0; i < w.size();) {  // greedy left to right (stress_test.cpp:181-188)
-        if (i + 1 < w.size() && w[i] == x && w[i + 1] == y) { nw.push_back(z); i += 2; any = true; }
-        else nw.push_back(w[i++]);
-      }
-      if (!any) continue;
-      int64_t f = (int64_t)wfreq[wi];
-      for_each_pair(w, [&](uint64_t k, uint64_t c) { add(k, -(int64_t)c * f); });
-      w = nw;
-      for_each_pair(w, [&](uint64_t k, uint64_t c) {
-        add(k, (int64_t)c * f);
-        auto &v = where[k];
-        if (v.empty() || v.back() != wi) v.push_back(wi);
-      });
-    }
-  }
+  // phases 3-4: pair counts + merge loop
+  std::vector<MergeRule> rules;
+  merge_words(words, wfreq, used, vocab_size > (int)used ? (uint64_t)(vocab_size - (int)used) : 0, &rules, nullptr);
   if (st) st->n_merges = rules.size();
 
   // rename_tokens (bpe.cpp:814-837)
@@ -389,6 +405,13 @@ void set_err(char *err, int errlen, const std::string &s) {
   if (err && errlen > 0) { std::strncpy(err, s.c_str(), errlen - 1); err[errlen - 1] = 0; }
 }
 struct Handle { orc::Model m; std::vector<int32_t> ids; std::vector<uint64_t> offs; };
+// what the last orc_train_words left behind (orc_words_state)
+struct WordsState {
+  std::vector<std::vector<uint32_t>> words;
+  std::vector<uint64_t> wfreq;
+  std::unordered_map<uint64_t, uint64_t> live;
+};
+WordsState g_words;
 }  // namespace
 
 extern "C" {
@@ -404,6 +427,52 @@ int orc_train_memory(const char *text, uint64_t n, const char *model_path, int v
   if (stats5) { stats5[0] = st.data_len; stats5[1] = st.n_words; stats5[2] = st.n_unique; stats5[3] = st.n_tokens; stats5[4] = st.n_merges; }
   if (!e.empty()) { set_err(err, errlen, e); return 1; }
   if (model_path && *model_path && !orc::save(m, model_path)) { set_err(err, errlen, "cannot write model"); return 1; }
+  return 0;
+}
+
+// The merge loop of training on given words (the words-in form of phases 3-4): word i = tokens[offsets[i],
+// offsets[i+1]) with frequency freq[i].  Up to max_merges rules (x, y, z) into out_rules (3 per merge) and the
+// count of (x, y) at merge time into out_freqs; *n_done = merges made.  The words and the pair table after the
+// merges stay for orc_words_state.
+int orc_train_words(const uint32_t *tokens, uint64_t n_tokens, const uint32_t *offsets, const uint64_t *freq,
+                    uint64_t n_words, uint32_t first_new_id, uint32_t max_merges, uint32_t *out_rules,
+                    uint64_t *out_freqs, uint32_t *n_done) {
+  g_words = WordsState();
+  g_words.words.resize(n_words);
+  g_words.wfreq.assign(freq, freq + n_words);
+  for (uint64_t i = 0; i < n_words; i++) {
+    if (offsets[i] > offsets[i + 1] || offsets[i + 1] > n_tokens) return 1;
+    g_words.words[i].assign(tokens + offsets[i], tokens + offsets[i + 1]);
+  }
+  std::vector<orc::MergeRule> rules;
+  orc::merge_words(g_words.words, g_words.wfreq, first_new_id, max_merges, &rules, &g_words.live);
+  for (size_t i = 0; i < rules.size(); i++) {
+    out_rules[3 * i] = rules[i].x; out_rules[3 * i + 1] = rules[i].y; out_rules[3 * i + 2] = rules[i].z;
+    out_freqs[i] = rules[i].cnt;
+  }
+  *n_done = (uint32_t)rules.size();
+  return 0;
+}
+
+// State after the last orc_train_words: its words (same order, with their frequencies) and the live pair table
+// (key = x << 32 | y, count > 0).  With tokens == nullptr only the sizes are returned.
+int orc_words_state(uint32_t *tokens, uint64_t *offsets, uint64_t *freq, uint64_t *keys, uint64_t *counts,
+                    uint64_t *n_words, uint64_t *n_tokens, uint64_t *n_pairs) {
+  uint64_t nt = 0, np = 0;
+  for (auto &w : g_words.words) nt += w.size();
+  for (auto &kv : g_words.live) np += kv.second != 0;
+  *n_words = g_words.words.size(); *n_tokens = nt; *n_pairs = np;
+  if (!tokens) return 0;
+  uint64_t p = 0;
+  for (size_t i = 0; i < g_words.words.size(); i++) {
+    offsets[i] = p;
+    for (uint32_t t : g_words.words[i]) tokens[p++] = t;
+    freq[i] = g_words.wfreq[i];
+  }
+  offsets[g_words.words.size()] = p;
+  uint64_t q = 0;
+  for (auto &kv : g_words.live)
+    if (kv.second) { keys[q] = kv.first; counts[q] = kv.second; q++; }
   return 0;
 }
 

@@ -182,7 +182,38 @@ class Oracle:
                                        C.c_double, C.c_uint64, C.c_uint64, C.POINTER(C.c_double),
                                        C.POINTER(C.c_uint64), C.c_char_p, C.c_int]
         lib.orc_result_ids.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.orc_train_words.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                        C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)]
+        lib.orc_words_state.argtypes = [C.c_void_p] * 5 + [C.POINTER(C.c_uint64)] * 3
         self.last_stats = None
+
+    def train_words(self, tokens, offsets, freq, first_new_id, max_merges):
+        """The merge loop on given words (word i = tokens[offsets[i]:offsets[i+1]], frequency freq[i]) ->
+        list of (x, y, z, count at merge time)."""
+        tokens = np.ascontiguousarray(tokens, dtype=np.uint32)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint32)
+        freq = np.ascontiguousarray(freq, dtype=np.uint64)
+        rules = np.zeros(3 * max(max_merges, 1), dtype=np.uint32)
+        cnts = np.zeros(max(max_merges, 1), dtype=np.uint64)
+        nd = C.c_uint32(0)
+        assert self.lib.orc_train_words(tokens.ctypes.data, len(tokens), offsets.ctypes.data, freq.ctypes.data,
+                                        len(freq), first_new_id, max_merges, rules.ctypes.data, cnts.ctypes.data,
+                                        C.byref(nd)) == 0, "orc_train_words: bad offsets"
+        return [tuple(int(v) for v in rules[3 * i:3 * i + 3]) + (int(cnts[i]),) for i in range(nd.value)]
+
+    def words_state(self):
+        """After train_words: (tokens uint32, offsets uint64[n+1], freq uint64, keys uint64, counts uint64) — the words
+        and the live pair table (key = x << 32 | y, count > 0)."""
+        nw, nt, npr = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self.lib.orc_words_state(None, None, None, None, None, C.byref(nw), C.byref(nt), C.byref(npr))
+        tok = np.zeros(nt.value + 1, dtype=np.uint32)
+        off = np.zeros(nw.value + 1, dtype=np.uint64)
+        frq = np.zeros(nw.value + 1, dtype=np.uint64)
+        keys = np.zeros(npr.value + 1, dtype=np.uint64)
+        cnts = np.zeros(npr.value + 1, dtype=np.uint64)
+        self.lib.orc_words_state(tok.ctypes.data, off.ctypes.data, frq.ctypes.data, keys.ctypes.data, cnts.ctypes.data,
+                                 C.byref(nw), C.byref(nt), C.byref(npr))
+        return tok[:nt.value], off, frq[:nw.value], keys[:npr.value], cnts[:npr.value]
 
     def train(self, text, model_path, vocab_size, coverage=1.0, pad=0, unk=1, bos=2, eos=3):
         err = C.create_string_buffer(ERRLEN)

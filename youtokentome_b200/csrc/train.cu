@@ -1344,6 +1344,12 @@ int yttm_train_import_words(yttm_ctx *c, const uint32_t *tokens, uint64_t n_toke
                             const uint64_t *freq, uint64_t n_words, yttm_train_stats *stats) {
   YT_CUDA(c, cudaSetDevice(c->device));
   if (n_tokens >= 0xfffffff0ull) YT_FAIL(c, "import_words: too many tokens");
+  // a count change of the merge loop is freq x (pairs of a word) in a signed 44-bit field (xq_pack)
+  for (uint64_t i = 0; i < n_words; i++) {
+    const uint64_t len = offsets[i + 1] - offsets[i];
+    if (len && freq[i] >= (1ull << 43) / len)
+      YT_FAIL(c, "import_words: word " + std::to_string(i) + ": frequency x tokens must stay below 2^43");
+  }
   c->cur = 0;
   YT_CUDA(c, c->tok[0].reserve((n_tokens + 4) * 4));
   YT_CUDA(c, c->off[0].reserve((n_words + 2) * 4));
@@ -1450,6 +1456,19 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
   for (int i = 0; i < 4; i++) h.t_phase[i] = 0;
   YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
   c->loop_relaunches = 0;
+  // compact the words and rebuild the table from them: the counts are stale (reason & 2: lost count changes), a
+  // partition ran full (reason & 4: grow) or is over the load limit (reason & 1)
+  auto rebuild = [&](uint32_t reason) -> int {
+    if (compact_words(c)) return 1;
+    const uint32_t keep_done = h.n_done;
+    // dead keys vanish in the rebuild, so the table usually keeps its size; it grows when a partition filled up
+    const uint64_t want = (reason & 4u) ? c->pcap * 2 : c->pcap / 2;
+    if (rebuild_pair_table(c, std::max<uint64_t>(want, pair_cap_floor()))) return 1;
+    YT_CUDA(c, cudaMemcpyAsync(&h, ctl, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    h.n_done = keep_done;
+    return 0;
+  };
   ytc::timer_begin(c, "merge_loop");
   while (h.n_done < max_merges && h.stop != 1) {
     LoopArgs a{};
@@ -1491,20 +1510,25 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
     YT_CUDA(c, cudaMemcpyAsync(&h, ctl, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
     YT_CUDA(c, cudaStreamSynchronize(c->stream));
     c->loop_relaunches++;
-    if (h.stop == 1 || h.n_done >= max_merges) break;
+    if (h.stop == 1 || h.n_done >= max_merges) {
+      // The last merge of the call may have lost count changes (or an update of a full partition): the kernel reports
+      // that at its exit check as stop_why, behind "done".  Rebuild now, so that the table this call leaves behind
+      // (yttm_train_dump_pairs, the next yttm_train_run) is exact.
+      if (h.stop_why & 6u) {
+        const uint32_t keep_stop = h.stop;
+        if (rebuild(h.stop_why)) return 1;
+        h.stop = keep_stop; h.stop_why = 0; h.overflow = 0; h.dead = 0; h.slots = c->n_slots;
+        YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
+      }
+      break;
+    }
     if (h.stop != 2 && h.stop != 3) YT_FAIL(c, "merge loop left without a reason (internal error)");
     // stop == 3: compaction wanted (by some rank); stop == 2: the table wants a rebuild.  Every rank of a job
     // leaves at the same merge for the same reason (merge_loop.cuh), so the steps below run in lockstep.
-    const uint32_t why = h.stop, reason = h.stop_why;
-    if (compact_words(c)) return 1;
-    if (why == 2) {
-      const uint32_t keep_done = h.n_done;
-      // dead keys vanish in the rebuild, so the table usually keeps its size; it grows when a partition filled up
-      const uint64_t want = (reason & 4u) ? c->pcap * 2 : c->pcap / 2;
-      if (rebuild_pair_table(c, std::max<uint64_t>(want, pair_cap_floor()))) return 1;
-      YT_CUDA(c, cudaMemcpyAsync(&h, ctl, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
-      YT_CUDA(c, cudaStreamSynchronize(c->stream));
-      h.n_done = keep_done;
+    if (h.stop == 2) {
+      if (rebuild(h.stop_why)) return 1;
+    } else if (compact_words(c)) {
+      return 1;
     }
     h.stop = 0; h.stop_why = 0; h.overflow = 0; h.dead = 0; h.slots = c->n_slots;
     YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
