@@ -164,7 +164,8 @@ int yttm_enc_run(yttm_enc *enc, const char *bytes, const uint64_t *offsets, uint
                  uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_n);
 
 /* Same with DEVICE-resident input (d_bytes, d_offsets) and results left on the device:
- * *d_out_ids / *d_out_offsets point into library-owned memory valid until the next call. */
+ * *d_out_ids / *d_out_offsets point into library-owned memory valid until the next call.  The ids are reserved before
+ * they are counted, at n_bytes + (1 + bos + eos) * n_sent ids of 4 bytes (the most a batch can produce). */
 int yttm_enc_run_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
                         uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                         uint64_t first_sentence_index, const int32_t **d_out_ids, const uint64_t **d_out_offsets,
@@ -183,7 +184,9 @@ int yttm_enc_run_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_of
 int yttm_enc_run_spans(yttm_enc *enc, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
                        int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, int32_t *out_ids,
                        uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_spans /* 2 * out_cap */, uint64_t *out_n);
-/* *d_out_* point into library-owned memory, complete when the call returns and valid until the next encode call */
+/* *d_out_* point into library-owned memory, complete when the call returns and valid until the next encode call.  The
+ * ids and spans are reserved before they are counted, at n_bytes + (1 + bos + eos) * n_sent ids: 20 bytes per id
+ * (about 2.6 GB for 128 MB of input), so split batches that do not fit the device at that bound. */
 int yttm_enc_run_spans_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
                               uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                               uint64_t first_sentence_index, const int32_t **d_out_ids, const uint64_t **d_out_offsets,

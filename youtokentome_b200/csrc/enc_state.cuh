@@ -29,14 +29,14 @@ struct yttm_enc {
   // per-call device buffers: two sets, so that the host-buffer entry point can pipeline chunks
   // (H2D of chunk i+1 and D2H of chunk i-1 overlap the kernels of chunk i)
   struct Slot {
-    ytc::DevBuf d_bytes, d_offs, slots, ranks, aux, wpos, wsent, nids, out_off, out_ids, counter, longw;
+    ytc::DevBuf d_bytes, d_offs, slots, ranks, aux, wpos, wsent, lookback, out_off, out_ids, counter, longw;
     ytc::DevBuf dd_tab, dd_rep, dd_list;  // word dedup
-    ytc::DevBuf swb, swc, ntok;            // per-sentence word ranges, per-word id counts
+    ytc::DevBuf swb, swc, rec;             // per-sentence word ranges, per-word records (id count, first ids)
     ytc::DevBuf rel, out_spans;            // spans: per-slot span relative to the word start, (start, end) per id
     ytc::DevBuf sub_len, sub_off, sub_out; // subwords: piece length per id, piece offsets, piece bytes
     void release() {
-      ytc::DevBuf *b[] = {&d_bytes, &d_offs, &slots, &ranks, &aux, &wpos, &wsent, &nids, &out_off, &out_ids, &counter, &longw,
-                          &dd_tab, &dd_rep, &dd_list, &swb, &swc, &ntok, &rel, &out_spans, &sub_len, &sub_off, &sub_out};
+      ytc::DevBuf *b[] = {&d_bytes, &d_offs, &slots, &ranks, &aux, &wpos, &wsent, &lookback, &out_off, &out_ids, &counter, &longw,
+                          &dd_tab, &dd_rep, &dd_list, &swb, &swc, &rec, &rel, &out_spans, &sub_len, &sub_off, &sub_out};
       for (auto *x : b) x->release();
     }
   } slot[2];

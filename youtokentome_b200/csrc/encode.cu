@@ -16,8 +16,9 @@
 //   dropout > 0 (every occurrence draws for itself):
 //     encode_words_kernel       one thread per occurrence, the same merge loop with BPE-dropout (DropoutQueue
 //                               bpe.cpp:1417-1453 with a counter-based generator)
-//   sentence_ids_kernel         ids per sentence; an exclusive scan turns them into output offsets
-//   emit_ids_kernel             warp per sentence: copies the ids of its words into the packed output
+//   every encoded item leaves a 16-byte record (id count, first three ids), so most words are served by one load
+//   emit_ids_kernel             single pass, block per tile of 256 sentences: id counts from the records, the tile's
+//                               output offset by a decoupled look-back over the earlier tiles, then offsets and ids
 // On request (yttm_enc_run_spans* / yttm_enc_run_subwords*) the same flow also gives the source span of every id and
 // the subword pieces:
 //   span_words_kernel           one thread per encoded word: the span of each of its ids relative to the word start
@@ -64,10 +65,10 @@ struct EncArgs {
   uint32_t *word_pos;        // work list: byte position of the word start (relative to the batch)
   uint32_t *word_sent;       //            sentence index inside the batch
   unsigned long long *n_words;
-  unsigned long long *n_ids;  // per sentence (uint64 so the generic scan applies)
   uint32_t *sent_wbase;       // first work item / number of work items of every sentence
   uint32_t *sent_wcnt;
-  uint32_t *n_tok;            // per encoded work item (every representative, or every word with dropout): number of ids
+  uint4 *rec;                 // per encoded work item (every representative, or every word with dropout): (number of
+                              // ids, first three ids), so that a word of at most 3 ids is one 16-byte load (put_rec)
   const uint32_t *cp2id;
   RuleTab rt;
   uint32_t space_id;
@@ -80,6 +81,11 @@ struct EncArgs {
 // word's first byte): base(s) = start(s) + 3 s ; the tokens of the sentence's words sit at
 // [base + 1 + rel ..], the slots base and base + len + 2 stay unused.
 __device__ __forceinline__ uint64_t sent_base(uint64_t start, uint64_t s) { return start + 3 * s; }
+
+// the record of an encoded item from its n final ids t[0 ..] (ids past n read as 0)
+__device__ __forceinline__ void put_rec(uint4 *rec, uint64_t w, uint32_t n, const int32_t *t) {
+  rec[w] = make_uint4(n, n > 0 ? (uint32_t)t[0] : 0u, n > 1 ? (uint32_t)t[1] : 0u, n > 2 ? (uint32_t)t[2] : 0u);
+}
 
 // exclusive sum of one value per thread over the block; *tot = block sum (starts with a barrier, so s_red may be reused
 // right after the previous call)
@@ -319,7 +325,7 @@ __global__ void __launch_bounds__(128) encode_words_kernel(EncArgs a, uint64_t n
       for (uint32_t i = 0; i < n; i++)
         if ((uint32_t)t[i] & UNK_FLAG) t[i] = a.unk_id;
     }
-    a.n_tok[w] = n;
+    put_rec(a.rec, w, n, t);
   }
 }
 
@@ -487,7 +493,8 @@ __global__ void __launch_bounds__(LONG_T) encode_long_words_kernel(EncArgs a, Lo
       const uint32_t v = t[i];
       t[i] = (v & UNK_FLAG) ? (uint32_t)a.unk_id : v;
     }
-    if (threadIdx.x == 0) a.n_tok[ll.item[w]] = n_out;
+    __syncthreads();  // t[0 .. 2] are final
+    if (threadIdx.x == 0) put_rec(a.rec, ll.item[w], n_out, reinterpret_cast<const int32_t *>(t));
     __syncthreads();
   }
 }
@@ -506,7 +513,7 @@ __global__ void __launch_bounds__(LONG_T) encode_long_words_kernel(EncArgs a, Lo
 //   encode_rep_words_kernel  the per-word body, over the representatives only (list length read on the device);
 //                            representatives of more than LONG_W slots go to the list of encode_long_words_kernel
 //   encode_long_words_kernel a block per long representative
-// emit_ids_kernel then copies the ids of a representative to every occurrence.  The slot of the first token of work
+// emit_ids_kernel then copies the ids of a representative (its record, or its slots) to every occurrence.  The slot of the first token of work
 // item w is word_pos[w] + 3 word_sent[w] + 1 (sent_base(): the sentence start cancels), so a copy needs no sentence
 // offsets.
 constexpr unsigned long long DEDUP_EMPTY = ~0ull;
@@ -664,7 +671,7 @@ __global__ void __launch_bounds__(128) encode_rep_words_kernel(EncArgs a, DedupA
     uint32_t l;
     while (q < hi && !space_at(a.bytes, q, hi, &l)) q++;
     uint32_t owned = (uint32_t)(q - p0) + 1, n;
-    if (owned > LONG_W) {  // a whole block will take it (encode_long_words_kernel sets n_tok)
+    if (owned > LONG_W) {  // a whole block will take it (encode_long_words_kernel writes its record)
       const unsigned long long k = atomicAdd(ll.n, 1ull);
       if (k < ll.cap) { ll.pos[k] = (uint32_t)p0; ll.sent[k] = (uint32_t)s; ll.end[k] = (uint32_t)q; ll.item[k] = w; continue; }
     }
@@ -680,31 +687,7 @@ __global__ void __launch_bounds__(128) encode_rep_words_kernel(EncArgs a, DedupA
       for (uint32_t k = 0; k < n; k++)
         if ((uint32_t)t[k] & UNK_FLAG) t[k] = a.unk_id;
     }
-    a.n_tok[w] = n;
-  }
-}
-
-// ---- output ---------------------------------------------------------------------------------------------------
-// The words of sentence s are the work items [sent_wbase[s], + sent_wcnt[s]) in byte order (find_words_vec_kernel); the
-// ids of work item w are the n_tok[r] values at slot(word_pos[r] + 3 word_sent[r] + 1) of its representative r = rep[w]
-// (r = w with dropout).  Two warp-per-sentence kernels take the ids from the encoded words straight to the packed
-// output, without compacting the slot buffer:
-//   sentence_ids_kernel   n_ids[s] = bos + eos + sum of n_tok over the sentence's words
-//   emit_ids_kernel       every lane takes one word, a warp scan gives its place, ids are copied from the
-//                         representative (reverse = mirrored index)
-__global__ void __launch_bounds__(256) sentence_ids_kernel(EncArgs a, const uint32_t *__restrict__ rep) {
-  const unsigned lane = threadIdx.x & 31;
-  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-  for (uint64_t s = warp; s < a.n_sent; s += nwarps) {
-    const uint32_t w0 = a.sent_wbase[s], nw = a.sent_wcnt[s];
-    uint32_t sum = 0;
-    for (uint32_t i = lane; i < nw; i += 32) {
-      const uint32_t w = w0 + i;
-      sum += a.n_tok[rep ? rep[w] : w];
-    }
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if (lane == 0) a.n_ids[s] = (unsigned long long)sum + (a.bos ? 1 : 0) + (a.eos ? 1 : 0);
+    put_rec(a.rec, w, n, t);
   }
 }
 
@@ -737,7 +720,7 @@ __global__ void __launch_bounds__(128) span_words_kernel(EncArgs a, const uint32
     const uint64_t slot0 = p0 + 3 * s + 1;
     const int32_t *t = a.slots + slot0;
     uint2 *rel = so.rel + slot0;
-    const uint32_t n_tok = a.n_tok[w];
+    const uint32_t n_tok = a.rec[w].x;
     // the first valid unit at or after q inside the word: its start (hi if none), code point and length
     auto next_valid = [&](uint64_t q, uint32_t *cp, uint32_t *l) {
       while (q < hi && !space_at(a.bytes, q, hi, l)) {
@@ -765,55 +748,167 @@ __global__ void __launch_bounds__(128) span_words_kernel(EncArgs a, const uint32
   }
 }
 
+// ---- output ---------------------------------------------------------------------------------------------------
+// The words of sentence s are the work items [sent_wbase[s], + sent_wcnt[s]) in byte order (find_words_vec_kernel); the
+// ids of work item w are those of its representative r = rep[w] (r = w with dropout): rec[r].x of them, the first three
+// in rec[r] itself, all of them at slot(word_pos[r] + 3 word_sent[r] + 1).  One single-pass kernel takes them from the
+// encoded words straight to the packed output, without compacting the slot buffer and without a host round trip:
+//   emit_ids_kernel   a block per tile of EMIT_T consecutive sentences, taken in ticket order: the ids of the tile's
+//                     sentences (a thread per word), a decoupled look-back over the earlier tiles for the tile's output
+//                     offset, then out_off and the ids (and the spans), a thread per word again.  The last tile writes
+//                     out_off[n_sent] and the batch's total.
+// Tiles publish one 64-bit word each: flag bits over a 62-bit id count, so value and flag are never seen apart and
+// no fence is needed.  Only the order of the look-back words matters: nothing else a block writes is read in the launch.
+constexpr int EMIT_T = 256;                                  // threads per block = sentences per tile
+constexpr unsigned long long LB_AGG = 1ull << 62;            // the tile's own id count
+constexpr unsigned long long LB_PRE = 1ull << 63;            // ids of the tiles up to and including this one
+constexpr unsigned long long LB_VAL = LB_AGG - 1;            // (0 = not published yet)
+struct EmitArgs {
+  const uint32_t *rep;         // null with dropout (every word represents itself)
+  unsigned long long *tiles;   // look-back word per tile, zeroed before the launch
+  unsigned long long *ticket;  // zeroed before the launch
+  unsigned long long *total;   // ids of the batch (the last tile)
+  unsigned long long *out_off; // n_sent + 1
+  int32_t *out;
+};
+
+// exclusive sum over the block of EMIT_T threads; *tot = block sum (starts with a barrier, like long_block_scan_sum)
+__device__ __forceinline__ unsigned long long emit_block_scan(unsigned long long v, unsigned long long *s_red,
+                                                              unsigned long long *tot) {
+  const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  unsigned long long x = v;
+  for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if ((int)lane >= o) x += y; }
+  __syncthreads();
+  if (lane == 31) s_red[wid] = x;
+  __syncthreads();
+  unsigned long long base = 0, all = 0;
+  for (unsigned i = 0; i < EMIT_T / 32; i++) { const unsigned long long w = s_red[i]; if (i < wid) base += w; all += w; }
+  *tot = all;
+  return base + x - v;
+}
+
 template <bool SPANS>
-__global__ void __launch_bounds__(256) emit_ids_kernel(EncArgs a, const uint32_t *__restrict__ rep,
-                                                       const unsigned long long *__restrict__ out_off, int32_t *__restrict__ out,
-                                                       SpanOut so) {
-  const unsigned lane = threadIdx.x & 31;
-  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-  for (uint64_t s = warp; s < a.n_sent; s += nwarps) {
-    const uint32_t w0 = a.sent_wbase[s], nw = a.sent_wcnt[s];
-    const unsigned long long ob = out_off[s], total = a.n_ids[s];
-    auto at = [&](unsigned long long j) { return ob + (a.reverse ? total - 1 - j : j); };
-    if (lane == 0) {
-      if (a.bos) out[at(0)] = a.bos_id;
-      if (a.eos) out[at(total - 1)] = a.eos_id;
-      if constexpr (SPANS) {
-        const unsigned long long lo = a.offs[s], hi = a.offs[s + 1];
-        if (a.bos) so.spans[at(0)] = Span64{lo, lo};
-        if (a.eos) so.spans[at(total - 1)] = Span64{hi, hi};
+__global__ void __launch_bounds__(EMIT_T) emit_ids_kernel(EncArgs a, EmitArgs e, SpanOut so) {
+  __shared__ uint32_t s_wb[EMIT_T];             // first work item of each sentence of the tile
+  __shared__ uint32_t s_wofs[EMIT_T + 1];       // words of the tile in front of each sentence
+  __shared__ uint32_t s_ids[EMIT_T];            // ids of each sentence's words
+  __shared__ unsigned long long s_off[EMIT_T];  // ids of the tile in front of each sentence
+  __shared__ unsigned long long s_red[EMIT_T / 32];
+  __shared__ unsigned long long s_tile, s_base;
+  const uint32_t tid = threadIdx.x;
+  if (tid == 0) s_tile = atomicAdd(e.ticket, 1ull);  // blocks do not start in blockIdx order
+  s_ids[tid] = 0;
+  __syncthreads();
+  const uint64_t tile = s_tile, s0 = tile * EMIT_T;
+  const uint32_t ns = (uint32_t)min((uint64_t)EMIT_T, a.n_sent - s0);
+  const uint32_t be = (a.bos ? 1u : 0u) + (a.eos ? 1u : 0u);
+  const uint32_t *rep = e.rep;
+  uint32_t wc = 0;
+  if (tid < ns) { s_wb[tid] = a.sent_wbase[s0 + tid]; wc = a.sent_wcnt[s0 + tid]; }
+  unsigned long long tw;
+  const uint32_t wofs = (uint32_t)emit_block_scan(wc, s_red, &tw);
+  const uint32_t n_tw = (uint32_t)tw;  // words of the tile
+  if (tid < ns) s_wofs[tid] = wofs;
+  if (tid == 0) s_wofs[ns] = n_tw;
+  __syncthreads();
+  // the tile's j-th word: its sentence k (the last one with s_wofs[k] <= j: empty sentences in front of it share its
+  // s_wofs) and its work item
+  auto word = [&](uint32_t j, uint32_t *k) {
+    uint32_t lo = 0, hi = ns;
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (s_wofs[mid] <= j) lo = mid; else hi = mid; }
+    *k = lo;
+    return s_wb[lo] + (j - s_wofs[lo]);
+  };
+  for (uint32_t j = tid; j < n_tw; j += EMIT_T) {
+    uint32_t k;
+    const uint32_t w = word(j, &k);
+    atomicAdd(&s_ids[k], a.rec[rep ? rep[w] : w].x);
+  }
+  __syncthreads();
+  const uint32_t cnt = tid < ns ? s_ids[tid] + be : 0u;  // ids of my sentence
+  unsigned long long agg;
+  const unsigned long long off = emit_block_scan(cnt, s_red, &agg);
+  // ---- decoupled look-back (warp 0): the ids of the tiles in front of this one
+  if (tid < 32) {
+    unsigned long long excl = 0;
+    if (tile > 0) {
+      if (tid == 0) *(volatile unsigned long long *)(e.tiles + tile) = LB_AGG | agg;
+      for (int64_t look = (int64_t)tile - 1;; look -= 32) {
+        const int64_t i = look - (int64_t)tid;
+        unsigned long long v;
+        do {  // the 32 tiles in front, nearest first (before tile 0: an inclusive prefix of 0)
+          v = LB_PRE;
+          if (i >= 0) v = *(volatile unsigned long long *)(e.tiles + i);
+        } while (__ballot_sync(0xffffffffu, v == 0));
+        const unsigned pm = __ballot_sync(0xffffffffu, (v & LB_PRE) != 0);
+        const unsigned take = pm ? ((pm & (0u - pm)) << 1) - 1u : 0xffffffffu;  // up to the nearest inclusive prefix
+        unsigned long long x = ((take >> tid) & 1u) ? (v & LB_VAL) : 0ull;
+        for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+        excl += x;
+        if (pm) break;
       }
     }
-    unsigned long long pos = a.bos ? 1 : 0;
-    for (uint32_t i0 = 0; i0 < nw; i0 += 32) {  // warp-uniform
-      const uint32_t i = i0 + lane;
-      uint32_t r = 0, n = 0;
-      if (i < nw) {
-        r = rep ? rep[w0 + i] : w0 + i;
-        n = a.n_tok[r];
-      }
-      uint32_t x = n;
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-        if ((int)lane >= o) x += y;
-      }
-      const uint32_t all = __shfl_sync(0xffffffffu, x, 31);
-      if (n) {
-        const uint64_t slot = (uint64_t)a.word_pos[r] + 3ull * a.word_sent[r] + 1;
+    if (tid == 0) {
+      *(volatile unsigned long long *)(e.tiles + tile) = LB_PRE | (excl + agg);
+      s_base = excl;
+    }
+  }
+  if (tid < ns) s_off[tid] = off;
+  __syncthreads();
+  const unsigned long long base = s_base;
+  if (tile + 1 == gridDim.x && tid == 0) { e.out_off[a.n_sent] = base + agg; *e.total = base + agg; }
+  if (tid < ns) {
+    const uint64_t s = s0 + tid;
+    const unsigned long long ob = base + off;
+    e.out_off[s] = ob;
+    const unsigned long long first = ob + (a.reverse ? cnt - 1 : 0), last = ob + (a.reverse ? 0 : cnt - 1);
+    if (a.bos) e.out[first] = a.bos_id;
+    if (a.eos) e.out[last] = a.eos_id;
+    if constexpr (SPANS) {
+      const unsigned long long lo = a.offs[s], hi = a.offs[s + 1];
+      if (a.bos) so.spans[first] = Span64{lo, lo};
+      if (a.eos) so.spans[last] = Span64{hi, hi};
+    }
+  }
+  // ---- the words' ids, EMIT_T words at a time in order: a block scan places them
+  unsigned long long carry = 0;  // ids of the tile's words before the chunk
+  for (uint32_t j0 = 0; j0 < n_tw; j0 += EMIT_T) {  // block-uniform
+    const uint32_t j = j0 + tid;
+    uint32_t k = 0, w = 0, r = 0;
+    uint4 rc = make_uint4(0u, 0u, 0u, 0u);
+    if (j < n_tw) {
+      w = word(j, &k);
+      r = rep ? rep[w] : w;
+      rc = a.rec[r];
+    }
+    unsigned long long chunk;
+    const unsigned long long x = emit_block_scan(rc.x, s_red, &chunk);
+    const uint32_t n = rc.x;
+    if (n) {
+      // place of the word's first id in its sentence: the ids of the tile's words before it, the bos / eos of the
+      // tile's sentences before it and its own bos, less the sentence's offset in the tile
+      const unsigned long long p = carry + x + (unsigned long long)be * k + (a.bos ? 1 : 0) - s_off[k];
+      const unsigned long long ob = base + s_off[k], last = s_ids[k] + be - 1;
+      auto at = [&](unsigned long long jj) { return ob + (a.reverse ? last - jj : jj); };
+      uint64_t slot = 0;
+      if (SPANS || n > 3) slot = (uint64_t)a.word_pos[r] + 3ull * a.word_sent[r] + 1;
+      if (n <= 3) {
+        e.out[at(p)] = (int32_t)rc.y;
+        if (n > 1) e.out[at(p + 1)] = (int32_t)rc.z;
+        if (n > 2) e.out[at(p + 2)] = (int32_t)rc.w;
+      } else {
         const int32_t *src = a.slots + slot;
-        const unsigned long long first = pos + (x - n);
-        for (uint32_t k = 0; k < n; k++) out[at(first + k)] = src[k];
-        if constexpr (SPANS) {
-          const unsigned long long wp = a.offs[0] + a.word_pos[w0 + i];  // this occurrence's first byte
-          for (uint32_t k = 0; k < n; k++) {
-            const uint2 rs = so.rel[slot + k];
-            so.spans[at(first + k)] = Span64{wp + rs.x, wp + rs.y};
-          }
+        for (uint32_t q = 0; q < n; q++) e.out[at(p + q)] = src[q];
+      }
+      if constexpr (SPANS) {
+        const unsigned long long wp = a.offs[0] + a.word_pos[w];  // this occurrence's first byte
+        for (uint32_t q = 0; q < n; q++) {
+          const uint2 rs = so.rel[slot + q];
+          so.spans[at(p + q)] = Span64{wp + rs.x, wp + rs.y};
         }
       }
-      pos += all;
     }
+    carry += chunk;
   }
 }
 
@@ -937,7 +1032,8 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   const uint64_t max_words = n_bytes / 2 + n_sent + 8;
   YT_CUDA(c, e->wpos.reserve(max_words * 4));
   YT_CUDA(c, e->wsent.reserve(max_words * 4));
-  YT_CUDA(c, e->nids.reserve((n_sent + 1) * 8));
+  const uint64_t n_tiles = (n_sent + EMIT_T - 1) / EMIT_T;
+  YT_CUDA(c, e->lookback.reserve((n_tiles + 1) * 8));
   YT_CUDA(c, e->out_off.reserve((n_sent + 2) * 8));
   YT_CUDA(c, e->counter.reserve(64));
   YT_CUDA(c, cudaMemsetAsync(e->counter.p, 0, 64, c->stream));
@@ -947,7 +1043,6 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   a.aux = dropout > 0 ? e->aux.as<uint32_t>() : nullptr;
   a.word_pos = e->wpos.as<uint32_t>(); a.word_sent = e->wsent.as<uint32_t>();
   a.n_words = e->counter.as<unsigned long long>();
-  a.n_ids = e->nids.as<unsigned long long>();
   a.cp2id = enc->cp2id.as<uint32_t>();
   a.rt.slots = enc->rules.as<uint4>(); a.rt.mask = enc->rule_mask;
   a.space_id = enc->space_id;
@@ -963,7 +1058,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   YT_CUDA(c, e->swc.reserve((n_sent + 1) * 4));
   a.sent_wbase = e->swb.as<uint32_t>();
   a.sent_wcnt = e->swc.as<uint32_t>();
-  a.n_tok = nullptr;  // sized by the number of words, known after find_words_vec_kernel
+  a.rec = nullptr;  // sized by the number of words, known after find_words_vec_kernel
   {
     ytc::timer_begin(c, "enc_find");
     // sentences per group: a group of mean-length sentences fills about 3/4 of a piece, so that groups longer than a
@@ -982,8 +1077,8 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   if (n_words) {
     uint64_t blocks = std::min<uint64_t>((n_words + 127) / 128, (uint64_t)c->n_sm * 16);
     ytc::timer_begin(c, "enc_words");
-    YT_CUDA(c, e->ntok.reserve(n_words * 4 + 16));
-    a.n_tok = e->ntok.as<uint32_t>();
+    YT_CUDA(c, e->rec.reserve(n_words * 16 + 16));
+    a.rec = e->rec.as<uint4>();
     if (a.drop_thresh == 0) {
       // words of more than LONG_W slots get a whole block each (a 16 KB word takes seconds on one thread)
       const uint32_t cap = (uint32_t)(n_bytes / LONG_W + 16);
@@ -1038,38 +1133,28 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
     }
     ytc::timer_end(c, "enc_words");
   }
-  const uint64_t sblocks = std::max<uint64_t>(std::min<uint64_t>((n_sent + 7) / 8, (uint64_t)c->n_sm * 8), 1);
-  {  // per-sentence id counts from the words' token counts
-    ytc::timer_begin(c, "enc_count");
-    sentence_ids_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a, d_rep);
-    ytc::timer_end(c, "enc_count");
-    c->launches++;
+  // The output is reserved at a bound, so that the emit needs no count from the host first: a sentence of len bytes
+  // has at most len + 1 + bos + eos ids (a word of k bytes has at most k + 1 ids, and its words are separated by at least
+  // one byte each).
+  const uint64_t id_cap = n_bytes + (1ull + (bos ? 1 : 0) + (eos ? 1 : 0)) * n_sent;
+  YT_CUDA(c, e->out_ids.reserve((id_cap + 8) * 4));
+  if (mode != ENC_IDS) {
+    YT_CUDA(c, e->out_spans.reserve((id_cap + 8) * 16));
+    so.spans = e->out_spans.as<Span64>();
   }
-  // exclusive scan of the per-sentence id counts -> output offsets
-  ytc::timer_begin(c, "enc_scan");
-  if (yttm_device_scan_u64(c, a.n_ids, n_sent, e->out_off.as<unsigned long long>(), d_total)) return 1;
-  ytc::timer_end(c, "enc_scan");
+  YT_CUDA(c, cudaMemsetAsync(e->lookback.p, 0, n_tiles * 8, c->stream));
+  EmitArgs ea;
+  ea.rep = d_rep; ea.tiles = e->lookback.as<unsigned long long>();
+  ea.ticket = e->counter.as<unsigned long long>() + 3;  // zeroed with the other counters above
+  ea.total = d_total; ea.out_off = e->out_off.as<unsigned long long>(); ea.out = e->out_ids.as<int32_t>();
+  ytc::timer_begin(c, "enc_gather");
+  if (mode == ENC_IDS) emit_ids_kernel<false><<<(unsigned)n_tiles, EMIT_T, 0, c->stream>>>(a, ea, so);
+  else emit_ids_kernel<true><<<(unsigned)n_tiles, EMIT_T, 0, c->stream>>>(a, ea, so);
+  ytc::timer_end(c, "enc_gather");
+  c->launches++;
   unsigned long long total = 0;
   YT_CUDA(c, cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, c->stream));
-  YT_CUDA(c, cudaMemcpyAsync(e->out_off.as<unsigned long long>() + n_sent, d_total, 8, cudaMemcpyDeviceToDevice,
-                             c->stream));
   YT_CUDA(c, cudaStreamSynchronize(c->stream));
-  YT_CUDA(c, e->out_ids.reserve((total + 8) * 4));
-  if (mode == ENC_IDS) {
-    ytc::timer_begin(c, "enc_gather");
-    emit_ids_kernel<false><<<(unsigned)sblocks, 256, 0, c->stream>>>(a, d_rep, e->out_off.as<unsigned long long>(),
-                                                                     e->out_ids.as<int32_t>(), so);
-    ytc::timer_end(c, "enc_gather");
-    c->launches++;
-  } else {
-    YT_CUDA(c, e->out_spans.reserve((total + 8) * 16));
-    so.spans = e->out_spans.as<Span64>();
-    ytc::timer_begin(c, "enc_gather");
-    emit_ids_kernel<true><<<(unsigned)sblocks, 256, 0, c->stream>>>(a, d_rep, e->out_off.as<unsigned long long>(),
-                                                                    e->out_ids.as<int32_t>(), so);
-    ytc::timer_end(c, "enc_gather");
-    c->launches++;
-  }
   if (mode == ENC_SUBWORDS && total == 0) {
     YT_CUDA(c, e->sub_off.reserve(16));
     YT_CUDA(c, cudaMemsetAsync(e->sub_off.p, 0, 8, c->stream));
