@@ -12,6 +12,7 @@ import pytest
 
 import _cases
 import test_encode_gpu as EG
+import test_encode_words_gpu as WG
 import test_train_gpu as TG
 from _bind import tmp_model_path
 from youtokentome_b200 import _lib, synth
@@ -23,6 +24,7 @@ def emu(monkeypatch):
     L = emu_lib()
     monkeypatch.setattr(_lib, "_lib", L)  # what _lib.lib() hands to tests/_gpu.py and to the Python BPE class
     monkeypatch.setenv("YT_EMU_SMS", "2")
+    monkeypatch.setattr(WG, "_cache", {})   # the shared bodies keep encoders: they belong to the library that made them
     return L
 
 
@@ -174,37 +176,13 @@ def test_encode_unicode_long_words_dropout(emu, oracle):
 def test_encode_special_id_layouts(emu, oracle, special):
     """Special ids below, between and above the ids of the characters and rules (the product of rule k is the k-th
     free id): with and without dropout."""
-    m = tmp_model_path("orc")
-    oracle.train(_cases.dirty_zipf_text(), m, 1200, 1.0, **special)
-    sents = _cases.zipf_sentences(300) + _cases.EDGE_SENTENCES
-    g, o = EG.GpuEncoder(m), oracle.encoder(m)
-    kws = [dict(), dict(reverse=True)] + ([dict(eos=True)] if special.get("eos", 3) != -1 else [])
-    for kw in kws:
-        assert g.encode(sents, **kw) == o.encode(sents, **kw)
-    assert g.encode(sents, dropout=0.4, seed=11) == o.encode(sents, dropout=0.4, seed=11)
+    WG.check_special_id_layouts(oracle, special)
 
 
 def test_encode_rule_products_are_read_from_the_model(emu, oracle, tmp_path):
     """A model whose rule products are NOT the k-th free id (two product ids swapped by hand): the encoder takes the
     id a rule produces from the model, never from the rule's rank."""
-    from _bind import read_model
-    m = tmp_model_path("orc")
-    oracle.train(synth.readme_corpus(n_lines=200), m, 60, 1.0)
-    c2i, rules, special = read_model(m)
-    a, b = rules[5][2], rules[9][2]
-    swap = {a: b, b: a}
-    rules2 = [tuple(swap.get(v, v) for v in r) for r in rules]
-    m2 = str(tmp_path / "swapped.yttm")
-    with open(m2, "w") as f:
-        f.write("%d %d\n" % (len(c2i), len(rules2)))
-        for cp, i in c2i.items():
-            f.write("%d %d\n" % (cp, i))
-        for r in rules2:
-            f.write("%d %d %d\n" % r)
-        f.write("%d %d %d %d\n" % special)
-    sents = [synth.readme_corpus(n_lines=3, seed=4), b"abab cdcd abcd", b"dddd aaaa"]
-    g = EG.GpuEncoder(m2)
-    assert g.encode(sents) == oracle.encoder(m2).encode(sents)
+    WG.check_rule_products_are_read_from_the_model(oracle, tmp_path)
 
 
 def test_encode_chunked_pipeline(emu, oracle, monkeypatch):
