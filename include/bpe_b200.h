@@ -174,6 +174,20 @@ class BaseEncoder {
                              const int32_t **d_ids, const uint64_t **d_id_offsets, const uint64_t **d_spans,
                              uint64_t *total_ids, bool bos = false, bool eos = false, bool reverse = false,
                              double dropout_prob = 0) const;
+  // encode_packed as rows of an [n_sentences, width] matrix (yttm_enc_run_padded in yttm_b200.h gives the definition):
+  // ids holds n_sentences * width cells, lengths n_sentences, spans (nullptr = not asked for) 2 * n_sentences * width.
+  // width >= max(1, bos + eos).  pad_id = kModelPad takes the model's pad id (an error if the model has none).  With
+  // dropout, advances the same sentence counter as encode_packed.
+  static constexpr int64_t kModelPad = INT64_MIN;
+  Status encode_padded_into(const char *bytes, const uint64_t *offsets, uint64_t n_sentences, uint64_t width, int32_t *ids,
+                            uint64_t *lengths, uint64_t *spans, bool bos = false, bool eos = false, bool reverse = false,
+                            double dropout_prob = 0, int64_t pad_id = kModelPad) const;
+  // DEVICE-resident input; width = 0 takes the longest row, *out_width = the width used.  *d_ids / *d_lengths /
+  // *d_spans (with_spans) point into library-owned memory that stays valid until the next encode call on this object.
+  Status encode_padded_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sentences,
+                              uint64_t width, bool with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
+                              const uint64_t **d_spans, uint32_t *out_width, bool bos = false, bool eos = false,
+                              bool reverse = false, double dropout_prob = 0, int64_t pad_id = kModelPad) const;
   // encode_as_subwords of a packed batch on the GPU, the pieces back to back: piece k = pieces[piece_offsets[k],
   // piece_offsets[k+1]), the pieces of sentence i = [sent_offsets[i], sent_offsets[i+1]).  Status code 2 (nothing
   // written, *n_pieces / *n_bytes = sizes needed) when pieces_cap (piece_offsets holds pieces_cap + 1) or bytes_cap
@@ -225,6 +239,7 @@ class BaseEncoder {
 
  private:
   Status init_device();
+  Status resolve_pad(int64_t pad_id, int32_t *out) const;  // encode_padded_*: kModelPad -> the model's pad id
   mutable yttm_ctx *ctx_ = nullptr;
   mutable yttm_enc *enc_ = nullptr;
   mutable uint64_t dropout_seed_ = 5489;  // std::mt19937's default seed, for flavour

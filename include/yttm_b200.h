@@ -191,6 +191,31 @@ int yttm_enc_run_spans_device(yttm_enc *enc, const char *d_bytes, const uint64_t
                               uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                               uint64_t first_sentence_index, const int32_t **d_out_ids, const uint64_t **d_out_offsets,
                               const uint64_t **d_out_spans, uint64_t *out_n);
+/* ---- padded rows of an encode ----------------------------------------------------------------------------------
+ * Same batches, arguments, checks and dropout stream as yttm_enc_run; sentence i becomes row i of an n_sent x width
+ * matrix (row i = ids[i * width, (i + 1) * width)).  With c_i = the ids yttm_enc_run gives sentence i with
+ * bos = eos = reverse = 0 and K = width - bos - eos:
+ *   row_i = [<BOS>]? + c_i[:K] + [<EOS>]?   (truncation drops ids from the end of the content; <BOS> / <EOS> stay),
+ *   reversed as a whole after the truncation with reverse;  lengths[i] = len(row_i);  cells [lengths[i], width) hold
+ *   pad_id.  With spans, a kept id has the span yttm_enc_run_spans gives it and a pad cell the empty span
+ *   [offsets[i+1], offsets[i+1]) (spans[2 (i width + j)], spans[2 (i width + j) + 1] for cell j of row i).
+ * Only the n_sent x width cells are reserved on the device (20 bytes per cell with spans), never the packed bound; a
+ * request that does not fit fails with an error.  HOST buffers: width >= max(1, bos + eos) and below 2^31; out_ids holds
+ * n_sent * width ids, out_lengths n_sent values, out_spans (NULL = not asked for) 2 * n_sent * width values.  The
+ * batch runs in chunks whose rows are copied straight to their place. */
+int yttm_enc_run_padded(yttm_enc *enc, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                        int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, uint64_t width,
+                        int32_t pad_id, int32_t *out_ids /* n_sent * width */, uint64_t *out_lengths /* n_sent */,
+                        uint64_t *out_spans /* NULL or 2 * n_sent * width */);
+/* DEVICE-resident input; width = 0 takes the longest row of the batch, max_i(|c_i| + bos + eos) (0 when every row is
+ * empty), at the cost of one counting pass and one 8-byte read-back; *out_width = the width used.  *d_ids /
+ * *d_lengths / *d_spans (with_spans, else NULL) point into library-owned memory, complete when the call returns and
+ * valid until the next encode call. */
+int yttm_enc_run_padded_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                               uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                               uint64_t first_sentence_index, uint64_t width /* 0 = longest */, int32_t pad_id,
+                               int with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
+                               const uint64_t **d_spans, uint32_t *out_width);
 /* encode_as_subwords (bpe.cpp:1757) of a batch: one piece per id, piece k = pieces[piece_offsets[k],
  * piece_offsets[k+1]) (UTF-8): the recipe of an ordinary id with its leading U+2581 kept, "<BOS>" / "<EOS>", and for
  * <UNK> the characters of its run (its span's bytes without invalid units).  The pieces of sentence i are

@@ -66,6 +66,18 @@ int yttm_api_encode_spans_into(void *handle, const char *bytes, const uint64_t *
 int yttm_api_encode_spans_device(void *handle, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
                                  uint64_t n_sent, int bos, int eos, int reverse, double dropout, const int32_t **d_ids,
                                  const uint64_t **d_id_offsets, const uint64_t **d_spans, uint64_t *total_ids);
+/* encode as padded rows (yttm_enc_run_padded of yttm_b200.h): ids_out holds n_sent * width ids, lengths_out n_sent
+ * values, spans_out (may be NULL) 2 * n_sent * width; pad_id = YTTM_PAD_FROM_MODEL takes the model's pad id (an error
+ * if the model has none), any other value must fit in int32.  The device form takes width = 0 for the longest row and
+ * sets *out_width; its results are library-owned device memory valid until the next encode call.  0 ok, 1 error. */
+#define YTTM_PAD_FROM_MODEL INT64_MIN
+int yttm_api_encode_padded_into(void *handle, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                                int reverse, double dropout, uint64_t width, int64_t pad_id, int32_t *ids_out,
+                                uint64_t *lengths_out, uint64_t *spans_out);
+int yttm_api_encode_padded_device(void *handle, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                  uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t width,
+                                  int64_t pad_id, int with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
+                                  const uint64_t **d_spans, uint32_t *out_width);
 /* encode(output_type='subword') on the GPU (yttm_enc_run_subwords): the same pieces as yttm_api_encode_subwords, into
  * caller-owned buffers; 0 ok, 1 error, 2 a capacity too small (*n_pieces / *n_bytes = sizes needed) */
 int yttm_api_encode_subwords_into(void *handle, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos,

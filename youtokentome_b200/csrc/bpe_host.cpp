@@ -594,6 +594,51 @@ Status BaseEncoder::encode_spans_device(const char *d_bytes, const uint64_t *d_o
   return Status();
 }
 
+Status BaseEncoder::resolve_pad(int64_t pad_id, int32_t *out) const {
+  if (pad_id == kModelPad) {
+    if (bpe_state.special_tokens.pad_id == -1)
+      return Status(1, "Can't pad: model was trained without <PAD> (pad_id = -1); pass a pad id.");
+    *out = bpe_state.special_tokens.pad_id;
+    return Status();
+  }
+  if (pad_id < INT32_MIN || pad_id > INT32_MAX)
+    return Status(1, "pad_id must fit in int32. Current value of pad_id = " + std::to_string(pad_id));
+  *out = (int32_t)pad_id;
+  return Status();
+}
+
+Status BaseEncoder::encode_padded_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, uint64_t width,
+                                       int32_t *ids, uint64_t *lengths, uint64_t *spans, bool bos, bool eos, bool reverse,
+                                       double dropout_prob, int64_t pad_id) const {
+  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
+  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
+  int32_t pad = 0;
+  Status ps = resolve_pad(pad_id, &pad);
+  if (!ps.ok()) return ps;
+  if (!device_status_.ok()) return device_status_;
+  int rc = yttm_enc_run_padded(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+                               sentence_counter_, width, pad, ids, lengths, spans);
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
+Status BaseEncoder::encode_padded_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                                         uint64_t width, bool with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
+                                         const uint64_t **d_spans, uint32_t *out_width, bool bos, bool eos, bool reverse,
+                                         double dropout_prob, int64_t pad_id) const {
+  int32_t pad = 0;
+  Status ps = resolve_pad(pad_id, &pad);
+  if (!ps.ok()) return ps;
+  if (!device_status_.ok()) return device_status_;
+  int rc = yttm_enc_run_padded_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+                                      dropout_seed_, sentence_counter_, width, pad, with_spans, d_ids, d_lengths, d_spans,
+                                      out_width);
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
 Status BaseEncoder::encode_subwords_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, uint8_t *pieces,
                                          uint64_t bytes_cap, uint64_t *piece_offsets, uint64_t pieces_cap,
                                          uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes, bool bos, bool eos,

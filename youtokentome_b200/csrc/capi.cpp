@@ -190,6 +190,30 @@ int yttm_api_encode_spans_device(void *hv, const char *d_bytes, const uint64_t *
   return 0;
 }
 
+// Padded rows (yttm_enc_run_padded*): pad_id = YTTM_PAD_FROM_MODEL takes the model's pad id
+int yttm_api_encode_padded_into(void *hv, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                                int reverse, double dropout, uint64_t width, int64_t pad_id, int32_t *ids_out,
+                                uint64_t *lengths_out, uint64_t *spans_out) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->encode_padded_into(bytes, offsets, n_sent, width, ids_out, lengths_out, spans_out, bos != 0, eos != 0,
+                                         reverse != 0, dropout, pad_id);
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
+int yttm_api_encode_padded_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                                  int bos, int eos, int reverse, double dropout, uint64_t width, int64_t pad_id, int with_spans,
+                                  const int32_t **d_ids, const uint64_t **d_lengths, const uint64_t **d_spans,
+                                  uint32_t *out_width) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  Status st = h->enc->encode_padded_device(d_bytes, d_offsets, n_bytes, n_sent, width, with_spans != 0, d_ids, d_lengths,
+                                           d_spans, out_width, bos != 0, eos != 0, reverse != 0, dropout, pad_id);
+  if (!st.ok()) return fail(h, st.message);
+  return 0;
+}
+
 int yttm_api_encode_subwords_into(void *hv, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
                                   int reverse, double dropout, uint8_t *pieces, uint64_t bytes_cap, uint64_t *piece_offsets,
                                   uint64_t pieces_cap, uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes) {

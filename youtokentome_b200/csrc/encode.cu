@@ -19,6 +19,9 @@
 //   every encoded item leaves a 16-byte record (id count, first three ids), so most words are served by one load
 //   emit_ids_kernel             single pass, block per tile of 256 sentences: id counts from the records, the tile's
 //                               output offset by a decoupled look-back over the earlier tiles, then offsets and ids
+// yttm_enc_run_padded* replace it with
+//   emit_padded_kernel          block per tile of 256 sentences, row i of an [n_sent, L] matrix at i L: the tiles need
+//                               nothing from each other (no look-back); a counting form finds L when it is not given
 // On request (yttm_enc_run_spans* / yttm_enc_run_subwords*) the same flow also gives the source span of every id and
 // the subword pieces:
 //   span_words_kernel           one thread per encoded word: the span of each of its ids relative to the word start
@@ -912,6 +915,153 @@ __global__ void __launch_bounds__(EMIT_T) emit_ids_kernel(EncArgs a, EmitArgs e,
   }
 }
 
+// ---- padded output ----------------------------------------------------------------------------------------------
+// encode_padded: sentence i becomes row i of an [n_sent, L] matrix instead of a run of the packed output.  With
+// c = its content ids (the packed ids without <BOS> / <EOS>) and K = L - bos - eos, the row is
+// [<BOS>]? c[:K] [<EOS>]?, reversed as a whole with reverse, and its cells [len, L) hold the pad id.  Row i starts at
+// i L, so a tile needs nothing from the other tiles: no ticket, no look-back, no total.
+//   emit_padded_kernel<SPANS, false>  a block per tile of EMIT_T consecutive sentences: content ids per sentence from
+//                                     the records (a thread per word), lengths, the pad cells of the tile's rows (one
+//                                     contiguous range of out), then the kept ids of every word (a thread per word)
+//   emit_padded_kernel<false, true>   only the counts: the longest row of the batch (L not given)
+// A word whose ids start at or past column K is skipped without reading its slots; a word that straddles the cut
+// copies its kept ids only.
+struct PadArgs {
+  const uint32_t *rep;           // null with dropout (every word represents itself)
+  int32_t *out;                  // n_sent x width
+  unsigned long long *lengths;   // n_sent
+  unsigned long long *max_len;   // counting form: the longest row (zeroed before the launch)
+  uint64_t width;
+  int32_t pad_id;
+};
+
+template <bool SPANS, bool COUNT>
+__global__ void __launch_bounds__(EMIT_T) emit_padded_kernel(EncArgs a, PadArgs p, SpanOut so) {
+  __shared__ uint32_t s_wb[EMIT_T];              // first work item of each sentence of the tile
+  __shared__ uint32_t s_wofs[EMIT_T + 1];        // words of the tile in front of each sentence
+  __shared__ uint32_t s_ids[EMIT_T];             // content ids of each sentence
+  __shared__ uint32_t s_len[EMIT_T];             // row length of each sentence
+  __shared__ unsigned long long s_cofs[EMIT_T];  // content ids of the tile in front of each sentence
+  __shared__ unsigned long long s_red[EMIT_T / 32];
+  const uint32_t tid = threadIdx.x;
+  const uint64_t s0 = (uint64_t)blockIdx.x * EMIT_T;
+  const uint32_t ns = (uint32_t)min((uint64_t)EMIT_T, a.n_sent - s0);
+  const uint32_t be = (a.bos ? 1u : 0u) + (a.eos ? 1u : 0u);
+  const uint32_t *rep = p.rep;
+  s_ids[tid] = 0;
+  uint32_t wc = 0;
+  if (tid < ns) { s_wb[tid] = a.sent_wbase[s0 + tid]; wc = a.sent_wcnt[s0 + tid]; }
+  unsigned long long tw;
+  const uint32_t wofs = (uint32_t)emit_block_scan(wc, s_red, &tw);
+  const uint32_t n_tw = (uint32_t)tw;  // words of the tile
+  if (tid < ns) s_wofs[tid] = wofs;
+  if (tid == 0) s_wofs[ns] = n_tw;
+  __syncthreads();
+  auto word = [&](uint32_t j, uint32_t *k) {  // the tile's j-th word: its sentence k and its work item
+    uint32_t lo = 0, hi = ns;
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (s_wofs[mid] <= j) lo = mid; else hi = mid; }
+    *k = lo;
+    return s_wb[lo] + (j - s_wofs[lo]);
+  };
+  for (uint32_t j = tid; j < n_tw; j += EMIT_T) {
+    uint32_t k;
+    const uint32_t w = word(j, &k);
+    atomicAdd(&s_ids[k], a.rec[rep ? rep[w] : w].x);
+  }
+  __syncthreads();
+  const uint32_t cnt = tid < ns ? s_ids[tid] : 0u;
+  if constexpr (COUNT) {
+    unsigned long long m = tid < ns ? (unsigned long long)cnt + be : 0ull;
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((tid & 31) == 0) s_red[tid >> 5] = m;
+    __syncthreads();
+    if (tid == 0) {
+      for (int i = 1; i < EMIT_T / 32; i++) m = max(m, s_red[i]);
+      atomicMax(p.max_len, m);
+    }
+    return;
+  }
+  const uint64_t L = p.width, K = L - be;  // L >= bos + eos (checked by the host)
+  const uint32_t len = tid < ns ? (uint32_t)(min((uint64_t)cnt, K) + be) : 0u;
+  unsigned long long tot;
+  const unsigned long long cofs = emit_block_scan(cnt, s_red, &tot);
+  if (tid < ns) {
+    const uint64_t s = s0 + tid;
+    s_cofs[tid] = cofs;
+    s_len[tid] = len;
+    p.lengths[s] = len;
+    if (len) {
+      const uint64_t row = s * L, first = row + (a.reverse ? len - 1 : 0), last = row + (a.reverse ? 0 : len - 1);
+      if (a.bos) p.out[first] = a.bos_id;
+      if (a.eos) p.out[last] = a.eos_id;
+      if constexpr (SPANS) {
+        const unsigned long long lo = a.offs[s], hi = a.offs[s + 1];
+        if (a.bos) so.spans[first] = Span64{lo, lo};
+        if (a.eos) so.spans[last] = Span64{hi, hi};
+      }
+    }
+  }
+  __syncthreads();
+  // ---- the pad cells: the tile's rows are the cells [s0 L, (s0 + ns) L) of out; thread t takes cells t, t + EMIT_T,
+  // ... and steps its (row, column) without a division per cell
+  if (L) {
+    const uint64_t n_cells = (uint64_t)ns * L, step_r = EMIT_T / L, step_c = EMIT_T % L;
+    uint64_t r = tid / L, col = tid % L;
+    int32_t *out = p.out + s0 * L;
+    for (uint64_t x = tid; x < n_cells; x += EMIT_T) {
+      if (col >= s_len[r]) {
+        out[x] = p.pad_id;
+        if constexpr (SPANS) {
+          const unsigned long long hi = a.offs[s0 + r + 1];
+          so.spans[s0 * L + x] = Span64{hi, hi};
+        }
+      }
+      r += step_r;
+      col += step_c;
+      if (col >= L) { col -= L; r++; }
+    }
+  }
+  // ---- the words' kept ids, EMIT_T words at a time in order: a block scan gives each word its first content index
+  unsigned long long carry = 0;  // content ids of the tile's words before the chunk
+  for (uint32_t j0 = 0; j0 < n_tw; j0 += EMIT_T) {  // block-uniform
+    const uint32_t j = j0 + tid;
+    uint32_t k = 0, w = 0, r = 0;
+    uint4 rc = make_uint4(0u, 0u, 0u, 0u);
+    if (j < n_tw) {
+      w = word(j, &k);
+      r = rep ? rep[w] : w;
+      rc = a.rec[r];
+    }
+    unsigned long long chunk;
+    const unsigned long long x = emit_block_scan(rc.x, s_red, &chunk);
+    const uint32_t n = rc.x;
+    const unsigned long long c0 = carry + x - (n ? s_cofs[k] : 0ull);  // the word's first content index in its row
+    if (n && c0 < K) {
+      const uint32_t m = (uint32_t)min((unsigned long long)n, K - c0);  // ids of the word that are kept
+      const uint64_t row = (s0 + k) * L, last = s_len[k] - 1, c1 = c0 + (a.bos ? 1 : 0);
+      auto at = [&](uint32_t q) { return row + (a.reverse ? last - (c1 + q) : c1 + q); };
+      uint64_t slot = 0;
+      if (SPANS || n > 3) slot = (uint64_t)a.word_pos[r] + 3ull * a.word_sent[r] + 1;
+      if (n <= 3) {
+        p.out[at(0)] = (int32_t)rc.y;
+        if (m > 1) p.out[at(1)] = (int32_t)rc.z;
+        if (m > 2) p.out[at(2)] = (int32_t)rc.w;
+      } else {
+        const int32_t *src = a.slots + slot;
+        for (uint32_t q = 0; q < m; q++) p.out[at(q)] = src[q];
+      }
+      if constexpr (SPANS) {
+        const unsigned long long wp = a.offs[0] + a.word_pos[w];  // this occurrence's first byte
+        for (uint32_t q = 0; q < m; q++) {
+          const uint2 rs = so.rel[slot + q];
+          so.spans[at(q)] = Span64{wp + rs.x, wp + rs.y};
+        }
+      }
+    }
+    carry += chunk;
+  }
+}
+
 // ---- subwords ---------------------------------------------------------------------------------------------------
 // One piece per output id: the model's piece of an ordinary id (recipe UTF-8, leading U+2581 kept) or of <BOS> / <EOS>,
 // and for <UNK> the characters of its run: the valid units of its span, copied from the source bytes.
@@ -1009,11 +1159,18 @@ int build_sub_table(yttm_enc *e) {
   return 0;
 }
 
+// The padded form of an encode call: rows of `width` ids (0 = the longest row of the batch, set by enc_device).
+struct PadReq {
+  uint64_t width;
+  int32_t pad_id;
+};
+
 // Encodes one batch on the device.  mode >= ENC_SPANS also writes e->out_spans; ENC_SUBWORDS also the pieces
-// (e->sub_off: out_n + 1 byte offsets, e->sub_out: *out_bytes bytes).
+// (e->sub_off: out_n + 1 byte offsets, e->sub_out: *out_bytes bytes).  With pad (ENC_IDS / ENC_SPANS) the ids and
+// spans are the n_sent x pad->width rows of emit_padded_kernel and e->out_off holds the row lengths.
 int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const uint64_t *d_offs, uint64_t n_bytes,
                uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence,
-               uint64_t *out_n, int mode = ENC_IDS, uint64_t *out_bytes = nullptr) {
+               uint64_t *out_n, int mode = ENC_IDS, uint64_t *out_bytes = nullptr, PadReq *pad = nullptr) {
   yttm_ctx *c = enc->ctx;
   if (n_bytes >= 0xfffffff0ull || n_sent >= 0xfffffff0ull)
     YT_FAIL(c, "encode batch too large: at most 2^32 bytes / sentences per call (split the batch)");
@@ -1133,6 +1290,40 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
     }
     ytc::timer_end(c, "enc_words");
   }
+  if (pad) {  // rows of width L: n_sent x L ids (and spans) are reserved, not the packed bound
+    PadArgs pa;
+    pa.rep = d_rep; pa.lengths = e->out_off.as<unsigned long long>(); pa.max_len = d_total; pa.pad_id = pad->pad_id;
+    pa.out = nullptr; pa.width = 0;
+    const unsigned n_tiles_pad = (unsigned)n_tiles;
+    ytc::timer_begin(c, "enc_gather");
+    if (pad->width == 0) {  // the longest row: one counting pass and one 8-byte read-back (d_total was zeroed above)
+      emit_padded_kernel<false, true><<<n_tiles_pad, EMIT_T, 0, c->stream>>>(a, pa, so);
+      c->launches++;
+      unsigned long long longest = 0;
+      YT_CUDA(c, cudaMemcpyAsync(&longest, d_total, 8, cudaMemcpyDeviceToHost, c->stream));
+      YT_CUDA(c, cudaStreamSynchronize(c->stream));
+      if (longest > 0x7fffffffull) YT_FAIL(c, "encode padded: the longest row has more than 2^31 - 1 ids (pass a width)");
+      pad->width = longest;
+    }
+    const uint64_t cells = n_sent * pad->width;  // < 2^32 * 2^31
+    const uint64_t span_bytes = mode != ENC_IDS ? cells * 16 : 0;
+    if (cells > (1ull << 40) || e->out_ids.reserve(cells * 4 + 16) != cudaSuccess ||
+        (span_bytes && e->out_spans.reserve(span_bytes + 16) != cudaSuccess)) {
+      cudaGetLastError();  // the failed allocation is reported here, not by the next call
+      YT_FAIL(c, "encode padded: " + std::to_string(n_sent) + " x " + std::to_string(pad->width) +
+                     " rows do not fit in device memory (split the batch or lower the width)");
+    }
+    pa.out = e->out_ids.as<int32_t>(); pa.width = pad->width;
+    if (mode != ENC_IDS) so.spans = e->out_spans.as<Span64>();
+    if (mode == ENC_IDS) emit_padded_kernel<false, false><<<n_tiles_pad, EMIT_T, 0, c->stream>>>(a, pa, so);
+    else emit_padded_kernel<true, false><<<n_tiles_pad, EMIT_T, 0, c->stream>>>(a, pa, so);
+    c->launches++;
+    ytc::timer_end(c, "enc_gather");
+    ytc::timer_end(c, "encode");
+    YT_CUDA(c, cudaGetLastError());
+    *out_n = cells;
+    return 0;
+  }
   // The output is reserved at a bound, so that the emit needs no count from the host first: a sentence of len bytes
   // has at most len + 1 + bos + eos ids (a word of k bytes has at most k + 1 ids, and its words are separated by at least
   // one byte each).
@@ -1198,6 +1389,8 @@ struct HostOut {
   uint8_t *pieces;
   uint64_t bytes_cap;
   uint64_t *piece_offsets;      // n_pieces + 1
+  const PadReq *pad = nullptr;  // padded rows: ids / spans hold n_sent x pad->width cells
+  uint64_t *lengths = nullptr;  // padded rows: n_sent
 };
 
 // The host-buffer form of enc_device: the batch is cut into chunks at sentence boundaries, chunk i runs in slot i & 1
@@ -1260,9 +1453,23 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
     YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_in[i & 1], 0));
     if (i >= 2) YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_out[i & 1], 0));  // results of chunk i-2 have left
     uint64_t total = 0, tbytes = 0;
+    PadReq pr{0, 0};
+    if (o.pad) pr = *o.pad;
     if (enc_device(e, &sl, sl.d_bytes.as<uint8_t>(), sl.d_offs.as<uint64_t>(), nb, hi - lo, bos, eos, reverse, dropout,
-                   seed, first_sentence_index + lo, &total, o.mode, &tbytes))
+                   seed, first_sentence_index + lo, &total, o.mode, &tbytes, o.pad ? &pr : nullptr))
       return 1;
+    if (o.pad) {  // rows [lo, hi) land at row lo: nothing to rebase
+      const uint64_t W = pr.width;
+      YT_CUDA(c, cudaEventRecord(e->ev_done[i & 1], c->stream));
+      YT_CUDA(c, cudaStreamWaitEvent(e->s_out, e->ev_done[i & 1], 0));
+      YT_CUDA(c, cudaMemcpyAsync(o.ids + lo * W, sl.out_ids.p, (hi - lo) * W * 4, cudaMemcpyDeviceToHost, e->s_out));
+      if (o.spans)
+        YT_CUDA(c, cudaMemcpyAsync(o.spans + 2 * lo * W, sl.out_spans.p, (hi - lo) * W * 16, cudaMemcpyDeviceToHost, e->s_out));
+      YT_CUDA(c, cudaMemcpyAsync(o.lengths + lo, sl.out_off.p, (hi - lo) * 8, cudaMemcpyDeviceToHost, e->s_out));
+      YT_CUDA(c, cudaEventRecord(e->ev_out[i & 1], e->s_out));
+      base += total;
+      continue;
+    }
     if (base && hi > lo) {  // chunk-local offsets -> batch offsets
       add_base_kernel<<<(unsigned)std::min<uint64_t>((hi - lo + 255) / 256, (uint64_t)c->n_sm * 4), 256, 0, c->stream>>>(
           sl.out_off.as<unsigned long long>(), hi - lo, (unsigned long long)base);
@@ -1297,7 +1504,7 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
   *out_n = base;
   if (out_bytes) *out_bytes = bbase;
   if (rc_small) { c->err = std::string(who) + ": output buffer too small"; return 2; }
-  o.id_offsets[n_sent] = base;
+  if (o.id_offsets) o.id_offsets[n_sent] = base;
   if (o.piece_offsets) o.piece_offsets[base] = bbase;
   (void)total_bytes;
   return 0;
@@ -1438,6 +1645,44 @@ int yttm_enc_run_spans(yttm_enc *e, const char *bytes, const uint64_t *offsets, 
   const HostOut o{ENC_SPANS, out_ids, out_spans, out_cap, out_offsets, nullptr, ~0ull, nullptr};
   return enc_run_host(e, "yttm_enc_run_spans", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
                       first_sentence_index, o, out_n, nullptr);
+}
+
+int yttm_enc_run_padded(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
+                        int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, uint64_t width,
+                        int32_t pad_id, int32_t *out_ids, uint64_t *out_lengths, uint64_t *out_spans) {
+  YT_ENC_ENTRY(e, "yttm_enc_run_padded")
+  if (width == 0 || width < (uint64_t)(bos ? 1 : 0) + (eos ? 1 : 0) || width > 0x7fffffffull)
+    YT_FAIL(c, "yttm_enc_run_padded: width must be at least 1 and bos + eos, and below 2^31");
+  PadReq pr{width, pad_id};
+  HostOut o{out_spans ? ENC_SPANS : ENC_IDS, out_ids, out_spans, ~0ull, nullptr, nullptr, ~0ull, nullptr, &pr, out_lengths};
+  uint64_t n = 0;
+  return enc_run_host(e, "yttm_enc_run_padded", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
+                      first_sentence_index, o, &n, nullptr);
+}
+
+int yttm_enc_run_padded_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                               uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                               uint64_t first_sentence_index, uint64_t width, int32_t pad_id, int with_spans,
+                               const int32_t **d_ids, const uint64_t **d_lengths, const uint64_t **d_spans,
+                               uint32_t *out_width) {
+  YT_ENC_ENTRY(e, "yttm_enc_run_padded_device")
+  if (width && (width < (uint64_t)(bos ? 1 : 0) + (eos ? 1 : 0) || width > 0x7fffffffull))
+    YT_FAIL(c, "yttm_enc_run_padded_device: width must be 0 (the longest row) or at least bos + eos, and below 2^31");
+  yttm_enc::Slot &sl = e->slot[0];
+  PadReq pr{width, pad_id};
+  uint64_t n = 0;
+  if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
+                 first_sentence_index, &n, with_spans ? ENC_SPANS : ENC_IDS, nullptr, &pr))
+    return 1;
+  YT_CUDA(c, sl.out_off.reserve(16));
+  YT_CUDA(c, sl.out_ids.reserve(16));
+  if (with_spans) YT_CUDA(c, sl.out_spans.reserve(16));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));  // the results are complete for readers on any stream
+  if (d_ids) *d_ids = sl.out_ids.as<int32_t>();
+  if (d_lengths) *d_lengths = sl.out_off.as<uint64_t>();
+  if (d_spans) *d_spans = with_spans ? sl.out_spans.as<uint64_t>() : nullptr;
+  if (out_width) *out_width = (uint32_t)pr.width;
+  return 0;
 }
 
 int yttm_enc_run_subwords_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,

@@ -2,7 +2,8 @@
 youtokentome/cpp/yttm.pyx:52-181) over the CUDA library: same class, method names, argument
 meaning, return types and exceptions (ValueError(status.message), TypeError for bad argument
 types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path, optionally with the source byte
-span of every id), `encode_subwords_packed` (the subword pieces on the GPU), `decode_packed` (the inverse of
+span of every id), `encode_padded` (the same ids as padded, truncated [N, L] rows with their lengths),
+`encode_subwords_packed` (the subword pieces on the GPU), `decode_packed` (the inverse of
 `encode_packed`, on the GPU) and `dropout_seed`."""
 import ctypes as C
 import threading
@@ -158,6 +159,124 @@ class BPE:
         if out == "torch":
             return ids.cpu(), oo.cpu()
         return ids.cpu().numpy(), oo.cpu().numpy().astype(np.uint64)
+
+    def encode_padded(self, data, offsets, max_length=None, pad_id=None, bos=False, eos=False, reverse=False,
+                      dropout_prob=0.0, out="numpy", with_spans=False):
+        """encode_packed as model input, on the GPU: sentence i becomes row i of an [N, L] matrix.  With c_i = the ids
+        encode_packed gives sentence i without bos / eos / reverse and K = L - bos - eos, row i is
+        [<BOS>]? + c_i[:K] + [<EOS>]? (truncated at the end of the content, <BOS> / <EOS> kept), reversed as a whole
+        with reverse, and its cells from len(row i) on hold the pad id.  L = max_length, or the longest row of the
+        batch when max_length is None.  pad_id defaults to the model's <PAD> id.  Inputs as for encode_packed; dropout
+        draws and the dropout_seed counter advance as in encode_packed.  Returns (ids int32 [N, L], lengths int64 [N])
+        and with with_spans also spans [N, L, 2] (encode_packed's span of every kept id, [offsets[i+1], offsets[i+1])
+        for pads) as numpy arrays (spans uint64), CPU torch tensors (out="torch") or CUDA tensors (out="cuda")."""
+        if out not in ("numpy", "torch", "cuda"):
+            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+        _check_dropout(dropout_prob)
+        if max_length is not None:
+            if isinstance(max_length, bool) or not isinstance(max_length, (int, np.integer)):
+                raise TypeError("max_length must be an int or None, not %s" % type(max_length).__name__)
+            max_length = int(max_length)
+            if max_length < 1 or max_length < int(bos) + int(eos) or max_length >= 2**31:
+                raise ValueError("max_length must be at least 1 and at least bos + eos, and below 2^31. Current value "
+                                 "of max_length = %d" % max_length)
+        if pad_id is None:
+            pad = -2**63   # YTTM_PAD_FROM_MODEL
+        else:
+            if isinstance(pad_id, bool) or not isinstance(pad_id, (int, np.integer)):
+                raise TypeError("pad_id must be an int or None, not %s" % type(pad_id).__name__)
+            pad = int(pad_id)
+            if not -2**31 <= pad < 2**31:
+                raise ValueError("pad_id must fit in int32. Current value of pad_id = %d" % pad)
+        is_torch = type(data).__module__.startswith("torch")
+        if out == "cuda" or (is_torch and data.is_cuda) or max_length is None:
+            return self._encode_padded_device(data, offsets, max_length or 0, pad, bos, eos, reverse, dropout_prob, out,
+                                              with_spans)
+        L = _lib.lib()
+        if is_torch:
+            keep = data = data.contiguous()
+            ptr = data.data_ptr()
+        elif isinstance(data, np.ndarray):
+            keep = data = np.ascontiguousarray(data)
+            ptr = data.ctypes.data
+        else:
+            keep = data = bytes(data) if not isinstance(data, bytes) else data
+            ptr = C.cast(C.c_char_p(data), C.c_void_p)
+        if type(offsets).__module__.startswith("torch"):
+            offsets = offsets.cpu().numpy()
+        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
+        n = len(offsets) - 1
+        if n < 0:
+            raise ValueError("offsets must hold at least one value")
+        W = max_length
+        if out == "torch":
+            import torch
+            pin = is_torch and data.is_pinned()
+            ids = torch.empty((n, W), dtype=torch.int32, pin_memory=pin)
+            lengths = torch.empty(n, dtype=torch.int64, pin_memory=pin)
+            spans = torch.empty((n, W, 2), dtype=torch.int64, pin_memory=pin) if with_spans else None
+            ptrs = ids.data_ptr(), lengths.data_ptr(), spans.data_ptr() if with_spans else None
+        else:
+            ids, lengths = np.empty((n, W), dtype=np.int32), np.empty(n, dtype=np.int64)
+            spans = np.empty((n, W, 2), dtype=np.uint64) if with_spans else None
+            ptrs = ids.ctypes.data, lengths.ctypes.data, spans.ctypes.data if with_spans else None
+        rc = L.yttm_api_encode_padded_into(self._h, ptr, offsets.ctypes.data, n, int(bos), int(eos), int(reverse),
+                                           float(dropout_prob), W, pad, *ptrs)
+        del keep
+        if rc != 0:
+            raise self._err()
+        return (ids, lengths, spans) if with_spans else (ids, lengths)
+
+    def _encode_padded_device(self, data, offsets, width, pad, bos, eos, reverse, dropout_prob, out, with_spans):
+        import torch
+        from .distributed import _DevView
+        L = _lib.lib()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if type(data).__module__.startswith("torch"):
+            d_bytes = data.to(dev, non_blocking=True).contiguous()
+        else:
+            raw = data if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).tobytes()
+            d_bytes = (torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev) if raw
+                       else torch.empty(0, dtype=torch.uint8, device=dev))
+        if type(offsets).__module__.startswith("torch"):
+            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
+        else:
+            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
+        n = d_offs.numel() - 1
+        if n < 0:
+            raise ValueError("offsets must hold at least one value")
+        first, last = (int(v) for v in d_offs[[0, n]].cpu())
+        p = [C.c_void_p() for _ in range(3)]
+        w = C.c_uint32(0)
+
+        def view(ptr, shape, ts):
+            k = int(np.prod(shape))
+            if k == 0:
+                return torch.empty(shape, dtype={"<i4": torch.int32, "<i8": torch.int64}[ts], device=dev)
+            return torch.as_tensor(_DevView(ptr.value, k, ts), device=dev).view(shape).clone()
+
+        torch.cuda.synchronize()   # the library runs on its own stream
+        with self._dev_lock:       # the result pointers are valid until the next encode on this handle: copy under the lock
+            # the library reads sentence 0 at the byte pointer it gets: the byte at offsets[0]
+            rc = L.yttm_api_encode_padded_device(self._h, d_bytes.data_ptr() + first, d_offs.data_ptr(), last - first, n,
+                                                 int(bos), int(eos), int(reverse), float(dropout_prob), width, pad,
+                                                 int(with_spans), C.byref(p[0]), C.byref(p[1]), C.byref(p[2]),
+                                                 C.byref(w))
+            if rc != 0:
+                raise self._err()
+            W = w.value
+            res = [view(p[0], (n, W), "<i4"), view(p[1], (n,), "<i8")]
+            if with_spans:
+                res.append(view(p[2], (n, W, 2), "<i8"))
+            torch.cuda.synchronize()
+        if out == "cuda":
+            return tuple(res)
+        if out == "torch":
+            return tuple(t.cpu() for t in res)
+        res = [t.cpu().numpy() for t in res]
+        if with_spans:
+            res[2] = res[2].astype(np.uint64)
+        return tuple(res)
 
     def encode_subwords_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy"):
         """encode(output_type=SUBWORD) of a packed batch on the GPU (inputs as for encode_packed).  Returns
