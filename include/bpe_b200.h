@@ -8,6 +8,7 @@
 // instead of the reference's bpe.h compiles unchanged.
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <iostream>
 #include <string>
 #include <unordered_map>
@@ -240,6 +241,12 @@ class BaseEncoder {
  private:
   Status init_device();
   Status resolve_pad(int64_t pad_id, int32_t *out) const;  // encode_padded_*: kModelPad -> the model's pad id
+  // The frame of every encode_*_into / _device and decode_packed_* call: the <BOS> / <EOS> check, `checked` (an argument
+  // error the caller found), the device status, then call() (a yttm_enc_run* / yttm_dec_run* call): its return code 2 is
+  // Status 2 ("<name>: output buffer too small"), any other error the context's message.  With dropout, a call that
+  // succeeds advances the sentence counter by n_sent.
+  Status run_device(const char *name, bool bos, bool eos, double dropout_prob, uint64_t n_sent,
+                    const std::function<int()> &call, const Status &checked = Status()) const;
   mutable yttm_ctx *ctx_ = nullptr;
   mutable yttm_enc *enc_ = nullptr;
   mutable uint64_t dropout_seed_ = 5489;  // std::mt19937's default seed, for flavour

@@ -521,23 +521,32 @@ int BaseEncoder::vocab_size() const {
   return (int)(bpe_state.rules.size() + bpe_state.char2id.size() + bpe_state.special_tokens.n_special_tokens());
 }
 
-Status BaseEncoder::encode_packed(const char *bytes, const uint64_t *offsets, uint64_t n_sent,
-                                  std::vector<int32_t> *ids, std::vector<uint64_t> *id_offsets, bool bos, bool eos,
-                                  bool reverse, double dropout_prob) const {
+Status BaseEncoder::run_device(const char *name, bool bos, bool eos, double dropout_prob, uint64_t n_sent,
+                               const std::function<int()> &call, const Status &checked) const {
   if (bos && bpe_state.special_tokens.bos_id == -1)  // bpe.cpp:1702-1707
     return Status(1, "Can't add <BOS> token. Model was trained without it.");
   if (eos && bpe_state.special_tokens.eos_id == -1)
     return Status(1, "Can't add <EOS> token. Model was trained without it.");
+  if (!checked.ok()) return checked;
   if (!device_status_.ok()) return device_status_;
+  int rc = call();
+  if (rc == 2) return Status(2, std::string(name) + ": output buffer too small");
+  if (rc) return Status(1, ctx_err(ctx_));
+  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  return Status();
+}
+
+Status BaseEncoder::encode_packed(const char *bytes, const uint64_t *offsets, uint64_t n_sent,
+                                  std::vector<int32_t> *ids, std::vector<uint64_t> *id_offsets, bool bos, bool eos,
+                                  bool reverse, double dropout_prob) const {
   uint64_t total_bytes = n_sent ? offsets[n_sent] - offsets[0] : 0;
   uint64_t cap = total_bytes + 3 * n_sent + 16;  // a sentence of L bytes yields at most L + 1 (+bos +eos) ids
   ids->resize(cap);
   id_offsets->resize(n_sent + 1);
   uint64_t n_out = 0;
-  int rc = yttm_enc_run(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
-                        sentence_counter_, ids->data(), cap, id_offsets->data(), &n_out);
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
+  Status st = encode_packed_into(bytes, offsets, n_sent, ids->data(), cap, id_offsets->data(), &n_out, bos, eos, reverse,
+                                 dropout_prob);
+  if (!st.ok()) return st;
   ids->resize(n_out);
   return Status();
 }
@@ -545,53 +554,37 @@ Status BaseEncoder::encode_packed(const char *bytes, const uint64_t *offsets, ui
 Status BaseEncoder::encode_packed_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, int32_t *ids,
                                        uint64_t ids_cap, uint64_t *id_offsets, uint64_t *total_ids, bool bos, bool eos,
                                        bool reverse, double dropout_prob) const {
-  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
-  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
-  if (!device_status_.ok()) return device_status_;
-  *total_ids = 0;
-  int rc = yttm_enc_run(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_, sentence_counter_, ids,
+  return run_device("encode_packed_into", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_, sentence_counter_, ids,
                         ids_cap, id_offsets, total_ids);
-  if (rc == 2) return Status(2, "encode_packed_into: output buffer too small");
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  });
 }
 
 Status BaseEncoder::encode_packed_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
                                          const int32_t **d_ids, const uint64_t **d_id_offsets, uint64_t *total_ids, bool bos,
                                          bool eos, bool reverse, double dropout_prob) const {
-  if (!device_status_.ok()) return device_status_;
-  int rc = yttm_enc_run_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+  return run_device("encode_packed_device", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
                                sentence_counter_, d_ids, d_id_offsets, total_ids);
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  });
 }
 
 Status BaseEncoder::encode_spans_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, int32_t *ids,
                                       uint64_t ids_cap, uint64_t *id_offsets, uint64_t *spans, uint64_t *total_ids, bool bos,
                                       bool eos, bool reverse, double dropout_prob) const {
-  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
-  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
-  if (!device_status_.ok()) return device_status_;
-  *total_ids = 0;
-  int rc = yttm_enc_run_spans(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+  return run_device("encode_spans_into", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_spans(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
                               sentence_counter_, ids, ids_cap, id_offsets, spans, total_ids);
-  if (rc == 2) return Status(2, "encode_spans_into: output buffer too small");
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  });
 }
 
 Status BaseEncoder::encode_spans_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
                                         const int32_t **d_ids, const uint64_t **d_id_offsets, const uint64_t **d_spans,
                                         uint64_t *total_ids, bool bos, bool eos, bool reverse, double dropout_prob) const {
-  if (!device_status_.ok()) return device_status_;
-  int rc = yttm_enc_run_spans_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+  return run_device("encode_spans_device", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_spans_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
                                      dropout_seed_, sentence_counter_, d_ids, d_id_offsets, d_spans, total_ids);
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  });
 }
 
 Status BaseEncoder::resolve_pad(int64_t pad_id, int32_t *out) const {
@@ -610,17 +603,11 @@ Status BaseEncoder::resolve_pad(int64_t pad_id, int32_t *out) const {
 Status BaseEncoder::encode_padded_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, uint64_t width,
                                        int32_t *ids, uint64_t *lengths, uint64_t *spans, bool bos, bool eos, bool reverse,
                                        double dropout_prob, int64_t pad_id) const {
-  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
-  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
   int32_t pad = 0;
-  Status ps = resolve_pad(pad_id, &pad);
-  if (!ps.ok()) return ps;
-  if (!device_status_.ok()) return device_status_;
-  int rc = yttm_enc_run_padded(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+  return run_device("encode_padded_into", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_padded(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
                                sentence_counter_, width, pad, ids, lengths, spans);
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  }, resolve_pad(pad_id, &pad));
 }
 
 Status BaseEncoder::encode_padded_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
@@ -628,67 +615,50 @@ Status BaseEncoder::encode_padded_device(const char *d_bytes, const uint64_t *d_
                                          const uint64_t **d_spans, uint32_t *out_width, bool bos, bool eos, bool reverse,
                                          double dropout_prob, int64_t pad_id) const {
   int32_t pad = 0;
-  Status ps = resolve_pad(pad_id, &pad);
-  if (!ps.ok()) return ps;
-  if (!device_status_.ok()) return device_status_;
-  int rc = yttm_enc_run_padded_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+  return run_device("encode_padded_device", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_padded_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
                                       dropout_seed_, sentence_counter_, width, pad, with_spans, d_ids, d_lengths, d_spans,
                                       out_width);
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  }, resolve_pad(pad_id, &pad));
 }
 
 Status BaseEncoder::encode_subwords_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, uint8_t *pieces,
                                          uint64_t bytes_cap, uint64_t *piece_offsets, uint64_t pieces_cap,
                                          uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes, bool bos, bool eos,
                                          bool reverse, double dropout_prob) const {
-  if (bos && bpe_state.special_tokens.bos_id == -1) return Status(1, "Can't add <BOS> token. Model was trained without it.");
-  if (eos && bpe_state.special_tokens.eos_id == -1) return Status(1, "Can't add <EOS> token. Model was trained without it.");
-  if (!device_status_.ok()) return device_status_;
-  *n_pieces = 0;
-  *n_bytes = 0;
-  int rc = yttm_enc_run_subwords(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
+  return run_device("encode_subwords_into", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_subwords(enc_, bytes, offsets, n_sent, bos, eos, reverse, dropout_prob, dropout_seed_,
                                  sentence_counter_, pieces, bytes_cap, piece_offsets, pieces_cap, sent_offsets, n_pieces,
                                  n_bytes);
-  if (rc == 2) return Status(2, "encode_subwords_into: output buffer too small");
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  });
 }
 
 Status BaseEncoder::encode_subwords_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
                                            const uint8_t **d_pieces, const uint64_t **d_piece_offsets,
                                            const uint64_t **d_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes,
                                            bool bos, bool eos, bool reverse, double dropout_prob) const {
-  if (!device_status_.ok()) return device_status_;
-  int rc = yttm_enc_run_subwords_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+  return run_device("encode_subwords_device", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_subwords_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
                                         dropout_seed_, sentence_counter_, d_pieces, d_piece_offsets, d_sent_offsets,
                                         n_pieces, n_piece_bytes);
-  if (rc) return Status(1, ctx_err(ctx_));
-  if (dropout_prob > 0) sentence_counter_ += n_sent;
-  return Status();
+  });
 }
 
 Status BaseEncoder::decode_packed_into(const int32_t *ids, const uint64_t *offsets, uint64_t n_sent, const int32_t *ignore_ids,
                                        uint64_t n_ignore, uint8_t *text, uint64_t text_cap, uint64_t *text_offsets,
                                        uint64_t *total_bytes) const {
-  if (!device_status_.ok()) return device_status_;
-  *total_bytes = 0;
-  int rc = yttm_dec_run(enc_, ids, offsets, n_sent, ignore_ids, n_ignore, text, text_cap, text_offsets, total_bytes);
-  if (rc == 2) return Status(2, "decode_packed_into: output buffer too small");
-  if (rc) return Status(1, ctx_err(ctx_));
-  return Status();
+  return run_device("decode_packed_into", false, false, 0, n_sent, [&] {
+    return yttm_dec_run(enc_, ids, offsets, n_sent, ignore_ids, n_ignore, text, text_cap, text_offsets, total_bytes);
+  });
 }
 
 Status BaseEncoder::decode_packed_device(const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
                                          const int32_t *ignore_ids, uint64_t n_ignore, const uint8_t **d_text,
                                          const uint64_t **d_text_offsets, uint64_t *total_bytes) const {
-  if (!device_status_.ok()) return device_status_;
-  int rc = yttm_dec_run_device(enc_, d_ids, n_ids, d_offsets, n_sent, ignore_ids, n_ignore, d_text, d_text_offsets,
+  return run_device("decode_packed_device", false, false, 0, n_sent, [&] {
+    return yttm_dec_run_device(enc_, d_ids, n_ids, d_offsets, n_sent, ignore_ids, n_ignore, d_text, d_text_offsets,
                                total_bytes);
-  if (rc) return Status(1, ctx_err(ctx_));
-  return Status();
+  });
 }
 
 Status BaseEncoder::encode_as_ids(const std::vector<std::string> &sentences, std::vector<std::vector<int>> *ids,

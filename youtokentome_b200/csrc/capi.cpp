@@ -36,6 +36,9 @@ struct Handle {
   std::mutex mu;
 };
 int fail(Handle *h, const std::string &m) { (h ? h->err : g_err) = m; return 1; }
+// the return code of a call that reports a Status: 0, 1 (error, message in the handle) or 2 (a caller buffer too small:
+// the counts hold the sizes needed, nothing written)
+int ret(Handle *h, const Status &st) { return st.code == 2 ? 2 : st.ok() ? 0 : fail(h, st.message); }
 }  // namespace
 
 extern "C" {
@@ -123,11 +126,8 @@ int yttm_api_encode_ids_into(void *hv, const char *bytes, const uint64_t *offset
                              uint64_t *total_ids) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_packed_into(bytes, offsets, n_sent, ids_out, ids_cap, offsets_out, total_ids, bos != 0, eos != 0,
-                                         reverse != 0, dropout);
-  if (st.code == 2) return 2;
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_packed_into(bytes, offsets, n_sent, ids_out, ids_cap, offsets_out, total_ids, bos != 0, eos != 0,
+                                           reverse != 0, dropout));
 }
 
 // Device-resident input and output (torch / CuPy callers): pointers into library-owned device memory, valid until the
@@ -137,10 +137,8 @@ int yttm_api_encode_device(void *hv, const char *d_bytes, const uint64_t *d_offs
                            uint64_t *total_ids) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_packed_device(d_bytes, d_offsets, n_bytes, n_sent, d_ids, d_id_offsets, total_ids, bos != 0,
-                                           eos != 0, reverse != 0, dropout);
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_packed_device(d_bytes, d_offsets, n_bytes, n_sent, d_ids, d_id_offsets, total_ids, bos != 0,
+                                             eos != 0, reverse != 0, dropout));
 }
 
 // Pieces come back length-framed (no in-band separator: a piece may hold any character, U+0001 included):
@@ -172,11 +170,8 @@ int yttm_api_encode_spans_into(void *hv, const char *bytes, const uint64_t *offs
                                uint64_t *spans_out, uint64_t *total_ids) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_spans_into(bytes, offsets, n_sent, ids_out, ids_cap, offsets_out, spans_out, total_ids,
-                                        bos != 0, eos != 0, reverse != 0, dropout);
-  if (st.code == 2) return 2;
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_spans_into(bytes, offsets, n_sent, ids_out, ids_cap, offsets_out, spans_out, total_ids,
+                                          bos != 0, eos != 0, reverse != 0, dropout));
 }
 
 int yttm_api_encode_spans_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
@@ -184,10 +179,8 @@ int yttm_api_encode_spans_device(void *hv, const char *d_bytes, const uint64_t *
                                  const uint64_t **d_id_offsets, const uint64_t **d_spans, uint64_t *total_ids) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_spans_device(d_bytes, d_offsets, n_bytes, n_sent, d_ids, d_id_offsets, d_spans, total_ids,
-                                          bos != 0, eos != 0, reverse != 0, dropout);
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_spans_device(d_bytes, d_offsets, n_bytes, n_sent, d_ids, d_id_offsets, d_spans, total_ids,
+                                            bos != 0, eos != 0, reverse != 0, dropout));
 }
 
 // Padded rows (yttm_enc_run_padded*): pad_id = YTTM_PAD_FROM_MODEL takes the model's pad id
@@ -196,10 +189,8 @@ int yttm_api_encode_padded_into(void *hv, const char *bytes, const uint64_t *off
                                 uint64_t *lengths_out, uint64_t *spans_out) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_padded_into(bytes, offsets, n_sent, width, ids_out, lengths_out, spans_out, bos != 0, eos != 0,
-                                         reverse != 0, dropout, pad_id);
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_padded_into(bytes, offsets, n_sent, width, ids_out, lengths_out, spans_out, bos != 0, eos != 0,
+                                           reverse != 0, dropout, pad_id));
 }
 
 int yttm_api_encode_padded_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
@@ -208,10 +199,8 @@ int yttm_api_encode_padded_device(void *hv, const char *d_bytes, const uint64_t 
                                   uint32_t *out_width) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_padded_device(d_bytes, d_offsets, n_bytes, n_sent, width, with_spans != 0, d_ids, d_lengths,
-                                           d_spans, out_width, bos != 0, eos != 0, reverse != 0, dropout, pad_id);
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_padded_device(d_bytes, d_offsets, n_bytes, n_sent, width, with_spans != 0, d_ids, d_lengths,
+                                             d_spans, out_width, bos != 0, eos != 0, reverse != 0, dropout, pad_id));
 }
 
 int yttm_api_encode_subwords_into(void *hv, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
@@ -219,11 +208,8 @@ int yttm_api_encode_subwords_into(void *hv, const char *bytes, const uint64_t *o
                                   uint64_t pieces_cap, uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_subwords_into(bytes, offsets, n_sent, pieces, bytes_cap, piece_offsets, pieces_cap, sent_offsets,
-                                           n_pieces, n_bytes, bos != 0, eos != 0, reverse != 0, dropout);
-  if (st.code == 2) return 2;
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_subwords_into(bytes, offsets, n_sent, pieces, bytes_cap, piece_offsets, pieces_cap, sent_offsets,
+                                             n_pieces, n_bytes, bos != 0, eos != 0, reverse != 0, dropout));
 }
 
 int yttm_api_encode_subwords_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
@@ -232,10 +218,8 @@ int yttm_api_encode_subwords_device(void *hv, const char *d_bytes, const uint64_
                                     uint64_t *n_piece_bytes) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->encode_subwords_device(d_bytes, d_offsets, n_bytes, n_sent, d_pieces, d_piece_offsets, d_sent_offsets,
-                                             n_pieces, n_piece_bytes, bos != 0, eos != 0, reverse != 0, dropout);
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->encode_subwords_device(d_bytes, d_offsets, n_bytes, n_sent, d_pieces, d_piece_offsets, d_sent_offsets,
+                                               n_pieces, n_piece_bytes, bos != 0, eos != 0, reverse != 0, dropout));
 }
 
 void yttm_api_result_counts(void *, uint64_t *n_pieces, uint64_t *n_sentences) {
@@ -270,10 +254,7 @@ int yttm_api_decode_into(void *hv, const int32_t *ids, const uint64_t *offsets, 
                          uint64_t n_ignore, uint8_t *text, uint64_t text_cap, uint64_t *text_offsets, uint64_t *total_bytes) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->decode_packed_into(ids, offsets, n_sent, ignore, n_ignore, text, text_cap, text_offsets, total_bytes);
-  if (st.code == 2) return 2;
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->decode_packed_into(ids, offsets, n_sent, ignore, n_ignore, text, text_cap, text_offsets, total_bytes));
 }
 
 // decode of device-resident ids: pointers into library-owned device memory, valid until the next decode_device call on
@@ -283,10 +264,8 @@ int yttm_api_decode_device(void *hv, const int32_t *d_ids, uint64_t n_ids, const
                            uint64_t *total_bytes) {
   auto *h = static_cast<Handle *>(hv);
   std::lock_guard<std::mutex> lock(h->mu);
-  Status st = h->enc->decode_packed_device(d_ids, n_ids, d_offsets, n_sent, ignore, n_ignore, d_text, d_text_offsets,
-                                           total_bytes);
-  if (!st.ok()) return fail(h, st.message);
-  return 0;
+  return ret(h, h->enc->decode_packed_device(d_ids, n_ids, d_offsets, n_sent, ignore, n_ignore, d_text, d_text_offsets,
+                                             total_bytes));
 }
 
 int64_t yttm_api_id_to_subword(void *hv, int id) {

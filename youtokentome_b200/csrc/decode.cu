@@ -383,9 +383,8 @@ extern "C" {
 int yttm_dec_run_device(yttm_enc *e, const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
                         const int32_t *ignore, uint64_t n_ignore, const uint8_t **d_out, const uint64_t **d_out_offsets,
                         uint64_t *out_n) {
-  if (!e) { g_yttm_create_error = "yttm_dec_run_device: null encoder handle (no CUDA device, or yttm_enc_create failed)"; return 1; }
+  if (yttm_enc_check(e, "yttm_dec_run_device", 0, 0)) return 1;
   yttm_ctx *c = e->ctx;
-  YT_CUDA(c, cudaSetDevice(c->device));
   if (!e->dec) e->dec = new yttm_dec();
   yttm_dec *d = e->dec;
   if (dec_device(e, d_ids, 0, n_ids, d_offsets, n_sent, ignore, n_ignore, &d->out, &d->out_off, ~0ull, out_n)) return 1;
@@ -397,9 +396,8 @@ int yttm_dec_run_device(yttm_enc *e, const int32_t *d_ids, uint64_t n_ids, const
 
 int yttm_dec_run(yttm_enc *e, const int32_t *ids, const uint64_t *offsets, uint64_t n_sent, const int32_t *ignore,
                  uint64_t n_ignore, uint8_t *out, uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_n) {
-  if (!e) { g_yttm_create_error = "yttm_dec_run: null encoder handle (no CUDA device, or yttm_enc_create failed)"; return 1; }
+  if (yttm_enc_check(e, "yttm_dec_run", 0, 0)) return 1;
   yttm_ctx *c = e->ctx;
-  YT_CUDA(c, cudaSetDevice(c->device));
   *out_n = 0;
   const uint64_t base = offsets[0], lim = offsets[n_sent];
   if (lim < base) YT_FAIL(c, offsets_error(lim));

@@ -11,6 +11,10 @@ struct yttm_enc;
 // The piece of every id in [0, vocab) as id_to_subword gives it (recipe UTF-8 with a leading U+2581 kept, special ids
 // their token); special[i] = 1 for the special ids.  Checks the model tables; error texts start with `who`.
 int yttm_model_pieces(yttm_enc *e, const char *who, std::vector<std::string> *raw, std::vector<uint8_t> *special);
+// The checks every encode and decode entry point makes before it runs (encode.cu): a handle, its device made current,
+// and a model with <BOS> / <EOS> when they are asked for.  Returns 1 with the error recorded (a null handle's text
+// starts with `who`).
+int yttm_enc_check(yttm_enc *e, const char *who, int bos, int eos);
 
 struct yttm_enc {
   yttm_ctx *ctx = nullptr;

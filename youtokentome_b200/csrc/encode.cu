@@ -1510,7 +1510,32 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
   return 0;
 }
 
+// The epilogue of the device entry points: every output buffer is allocated (the pointers handed out are never null),
+// the offsets of an empty batch read [0], and the stream is idle, so that readers on any stream see complete results.
+int publish_device(yttm_ctx *c, uint64_t n_sent, std::initializer_list<ytc::DevBuf *> outs,
+                   std::initializer_list<ytc::DevBuf *> offsets) {
+  for (ytc::DevBuf *b : outs) YT_CUDA(c, b->reserve(16));
+  for (ytc::DevBuf *b : offsets) {
+    YT_CUDA(c, b->reserve(16));
+    if (n_sent == 0) YT_CUDA(c, cudaMemsetAsync(b->p, 0, 8, c->stream));
+  }
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
 }  // namespace
+
+int yttm_enc_check(yttm_enc *e, const char *who, int bos, int eos) {
+  if (!e) {
+    g_yttm_create_error = std::string(who) + ": null encoder handle (no CUDA device, or yttm_enc_create failed)";
+    return 1;
+  }
+  yttm_ctx *c = e->ctx;
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
+  if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
+  return 0;
+}
 
 extern "C" {
 
@@ -1584,54 +1609,36 @@ void yttm_enc_destroy(yttm_enc *e) {
 int yttm_enc_run_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
                         int bos, int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index,
                         const int32_t **d_out_ids, const uint64_t **d_out_offsets, uint64_t *out_n) {
-  if (!e) { g_yttm_create_error = "yttm_enc_run_device: null encoder handle (no CUDA device, or yttm_enc_create failed)"; return 1; }
-  yttm_ctx *c = e->ctx;
-  YT_CUDA(c, cudaSetDevice(c->device));
-  if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
-  if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
-  if (enc_device(e, &e->slot[0], (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout,
-                 seed, first_sentence_index, out_n))
+  if (yttm_enc_check(e, "yttm_enc_run_device", bos, eos)) return 1;
+  yttm_enc::Slot &sl = e->slot[0];
+  if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
+                 first_sentence_index, out_n) ||
+      publish_device(e->ctx, n_sent, {&sl.out_ids}, {&sl.out_off}))
     return 1;
-  if (d_out_ids) *d_out_ids = e->slot[0].out_ids.as<int32_t>();
-  if (d_out_offsets) *d_out_offsets = e->slot[0].out_off.as<uint64_t>();
+  if (d_out_ids) *d_out_ids = sl.out_ids.as<int32_t>();
+  if (d_out_offsets) *d_out_offsets = sl.out_off.as<uint64_t>();
   return 0;
 }
 
 int yttm_enc_run(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos, int reverse,
                  double dropout, uint64_t seed, uint64_t first_sentence_index, int32_t *out_ids, uint64_t out_cap,
                  uint64_t *out_offsets, uint64_t *out_n) {
-  if (!e) { g_yttm_create_error = "yttm_enc_run: null encoder handle (no CUDA device, or yttm_enc_create failed)"; return 1; }
-  yttm_ctx *c = e->ctx;
-  YT_CUDA(c, cudaSetDevice(c->device));
-  if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
-  if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
+  if (yttm_enc_check(e, "yttm_enc_run", bos, eos)) return 1;
   const HostOut o{ENC_IDS, out_ids, nullptr, out_cap, out_offsets, nullptr, ~0ull, nullptr};
   return enc_run_host(e, "yttm_enc_run", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed, first_sentence_index, o,
                       out_n, nullptr);
 }
 
-// the checks every encode entry point makes before it runs
-#define YT_ENC_ENTRY(e, name)                                                                                         \
-  if (!e) { g_yttm_create_error = name ": null encoder handle (no CUDA device, or yttm_enc_create failed)"; return 1; } \
-  yttm_ctx *c = e->ctx;                                                                                                \
-  YT_CUDA(c, cudaSetDevice(c->device));                                                                                \
-  if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");                         \
-  if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
-
 int yttm_enc_run_spans_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
                               int bos, int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index,
                               const int32_t **d_out_ids, const uint64_t **d_out_offsets, const uint64_t **d_out_spans,
                               uint64_t *out_n) {
-  YT_ENC_ENTRY(e, "yttm_enc_run_spans_device")
+  if (yttm_enc_check(e, "yttm_enc_run_spans_device", bos, eos)) return 1;
   yttm_enc::Slot &sl = e->slot[0];
   if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
-                 first_sentence_index, out_n, ENC_SPANS))
+                 first_sentence_index, out_n, ENC_SPANS) ||
+      publish_device(e->ctx, n_sent, {&sl.out_ids, &sl.out_spans}, {&sl.out_off}))
     return 1;
-  YT_CUDA(c, sl.out_off.reserve(16));
-  YT_CUDA(c, sl.out_ids.reserve(16));
-  YT_CUDA(c, sl.out_spans.reserve(16));
-  if (n_sent == 0) YT_CUDA(c, cudaMemsetAsync(sl.out_off.p, 0, 8, c->stream));
-  YT_CUDA(c, cudaStreamSynchronize(c->stream));  // the results are complete for readers on any stream
   if (d_out_ids) *d_out_ids = sl.out_ids.as<int32_t>();
   if (d_out_offsets) *d_out_offsets = sl.out_off.as<uint64_t>();
   if (d_out_spans) *d_out_spans = sl.out_spans.as<uint64_t>();
@@ -1641,7 +1648,7 @@ int yttm_enc_run_spans_device(yttm_enc *e, const char *d_bytes, const uint64_t *
 int yttm_enc_run_spans(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
                        int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, int32_t *out_ids,
                        uint64_t out_cap, uint64_t *out_offsets, uint64_t *out_spans, uint64_t *out_n) {
-  YT_ENC_ENTRY(e, "yttm_enc_run_spans")
+  if (yttm_enc_check(e, "yttm_enc_run_spans", bos, eos)) return 1;
   const HostOut o{ENC_SPANS, out_ids, out_spans, out_cap, out_offsets, nullptr, ~0ull, nullptr};
   return enc_run_host(e, "yttm_enc_run_spans", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
                       first_sentence_index, o, out_n, nullptr);
@@ -1650,9 +1657,9 @@ int yttm_enc_run_spans(yttm_enc *e, const char *bytes, const uint64_t *offsets, 
 int yttm_enc_run_padded(yttm_enc *e, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
                         int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, uint64_t width,
                         int32_t pad_id, int32_t *out_ids, uint64_t *out_lengths, uint64_t *out_spans) {
-  YT_ENC_ENTRY(e, "yttm_enc_run_padded")
+  if (yttm_enc_check(e, "yttm_enc_run_padded", bos, eos)) return 1;
   if (width == 0 || width < (uint64_t)(bos ? 1 : 0) + (eos ? 1 : 0) || width > 0x7fffffffull)
-    YT_FAIL(c, "yttm_enc_run_padded: width must be at least 1 and bos + eos, and below 2^31");
+    YT_FAIL(e->ctx, "yttm_enc_run_padded: width must be at least 1 and bos + eos, and below 2^31");
   PadReq pr{width, pad_id};
   HostOut o{out_spans ? ENC_SPANS : ENC_IDS, out_ids, out_spans, ~0ull, nullptr, nullptr, ~0ull, nullptr, &pr, out_lengths};
   uint64_t n = 0;
@@ -1665,19 +1672,16 @@ int yttm_enc_run_padded_device(yttm_enc *e, const char *d_bytes, const uint64_t 
                                uint64_t first_sentence_index, uint64_t width, int32_t pad_id, int with_spans,
                                const int32_t **d_ids, const uint64_t **d_lengths, const uint64_t **d_spans,
                                uint32_t *out_width) {
-  YT_ENC_ENTRY(e, "yttm_enc_run_padded_device")
+  if (yttm_enc_check(e, "yttm_enc_run_padded_device", bos, eos)) return 1;
   if (width && (width < (uint64_t)(bos ? 1 : 0) + (eos ? 1 : 0) || width > 0x7fffffffull))
-    YT_FAIL(c, "yttm_enc_run_padded_device: width must be 0 (the longest row) or at least bos + eos, and below 2^31");
+    YT_FAIL(e->ctx, "yttm_enc_run_padded_device: width must be 0 (the longest row) or at least bos + eos, and below 2^31");
   yttm_enc::Slot &sl = e->slot[0];
   PadReq pr{width, pad_id};
   uint64_t n = 0;
   if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
-                 first_sentence_index, &n, with_spans ? ENC_SPANS : ENC_IDS, nullptr, &pr))
+                 first_sentence_index, &n, with_spans ? ENC_SPANS : ENC_IDS, nullptr, &pr) ||
+      publish_device(e->ctx, n_sent, {&sl.out_ids, &sl.out_spans}, {&sl.out_off}))
     return 1;
-  YT_CUDA(c, sl.out_off.reserve(16));
-  YT_CUDA(c, sl.out_ids.reserve(16));
-  if (with_spans) YT_CUDA(c, sl.out_spans.reserve(16));
-  YT_CUDA(c, cudaStreamSynchronize(c->stream));  // the results are complete for readers on any stream
   if (d_ids) *d_ids = sl.out_ids.as<int32_t>();
   if (d_lengths) *d_lengths = sl.out_off.as<uint64_t>();
   if (d_spans) *d_spans = with_spans ? sl.out_spans.as<uint64_t>() : nullptr;
@@ -1689,19 +1693,12 @@ int yttm_enc_run_subwords_device(yttm_enc *e, const char *d_bytes, const uint64_
                                  uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                                  uint64_t first_sentence_index, const uint8_t **d_pieces, const uint64_t **d_piece_offsets,
                                  const uint64_t **d_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes) {
-  YT_ENC_ENTRY(e, "yttm_enc_run_subwords_device")
+  if (yttm_enc_check(e, "yttm_enc_run_subwords_device", bos, eos)) return 1;
   yttm_enc::Slot &sl = e->slot[0];
   if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout, seed,
-                 first_sentence_index, n_pieces, ENC_SUBWORDS, n_piece_bytes))
+                 first_sentence_index, n_pieces, ENC_SUBWORDS, n_piece_bytes) ||
+      publish_device(e->ctx, n_sent, {&sl.sub_out}, {&sl.out_off, &sl.sub_off}))
     return 1;
-  YT_CUDA(c, sl.out_off.reserve(16));
-  YT_CUDA(c, sl.sub_off.reserve(16));
-  YT_CUDA(c, sl.sub_out.reserve(16));
-  if (n_sent == 0) {
-    YT_CUDA(c, cudaMemsetAsync(sl.out_off.p, 0, 8, c->stream));
-    YT_CUDA(c, cudaMemsetAsync(sl.sub_off.p, 0, 8, c->stream));
-  }
-  YT_CUDA(c, cudaStreamSynchronize(c->stream));
   if (d_pieces) *d_pieces = sl.sub_out.as<uint8_t>();
   if (d_piece_offsets) *d_piece_offsets = sl.sub_off.as<uint64_t>();
   if (d_sent_offsets) *d_sent_offsets = sl.out_off.as<uint64_t>();
@@ -1712,7 +1709,7 @@ int yttm_enc_run_subwords(yttm_enc *e, const char *bytes, const uint64_t *offset
                           int reverse, double dropout, uint64_t seed, uint64_t first_sentence_index, uint8_t *out_pieces,
                           uint64_t bytes_cap, uint64_t *out_piece_offsets, uint64_t pieces_cap, uint64_t *out_sent_offsets,
                           uint64_t *n_pieces, uint64_t *n_piece_bytes) {
-  YT_ENC_ENTRY(e, "yttm_enc_run_subwords")
+  if (yttm_enc_check(e, "yttm_enc_run_subwords", bos, eos)) return 1;
   const HostOut o{ENC_SUBWORDS, nullptr, nullptr, pieces_cap, out_sent_offsets, out_pieces, bytes_cap, out_piece_offsets};
   return enc_run_host(e, "yttm_enc_run_subwords", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
                       first_sentence_index, o, n_pieces, n_piece_bytes);

@@ -39,6 +39,92 @@ def _offsets_error(n_ids):  # the library's text for the same error
     return "decode: offsets must be non-decreasing and lie within the ids (n_ids = %d)" % n_ids
 
 
+def _is_torch(x):
+    return type(x).__module__.startswith("torch")
+
+
+def _check_out(out):
+    if out not in ("numpy", "torch", "cuda"):
+        raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+
+
+def _host_offsets(offsets):
+    """offsets as contiguous numpy uint64, and n = len - 1."""
+    if _is_torch(offsets):
+        offsets = offsets.cpu().numpy()
+    offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
+    if len(offsets) < 1:
+        raise ValueError("offsets must hold at least one value")
+    return offsets, len(offsets) - 1
+
+
+def _stage_host(data, offsets):
+    """A host batch as the library reads it: (keep-alive, byte pointer, byte count, uint64 offsets, n, pinned).  `data`:
+    bytes-like, numpy array or CPU torch tensor."""
+    pinned = False
+    if _is_torch(data):
+        data = data.contiguous()
+        ptr, n_bytes, pinned = data.data_ptr(), data.numel(), data.is_pinned()
+    elif isinstance(data, np.ndarray):
+        data = np.ascontiguousarray(data)
+        ptr, n_bytes = data.ctypes.data, data.nbytes
+    else:
+        data = data if isinstance(data, bytes) else bytes(data)
+        ptr, n_bytes = C.cast(C.c_char_p(data), C.c_void_p), len(data)
+    return (data, ptr, n_bytes) + _host_offsets(offsets) + (pinned,)
+
+
+def _stage_device(data, offsets):
+    """A batch on the current CUDA device, uploaded if needed: (device, data tensor, int64 offsets tensor, n)."""
+    import torch
+    dev = torch.device("cuda", torch.cuda.current_device())
+    if _is_torch(data):
+        d = data.to(dev, non_blocking=True).contiguous()
+    elif isinstance(data, (bytes, bytearray, memoryview)):
+        raw = bytearray(data)   # a writable copy: torch warns on read-only buffers
+        d = (torch.frombuffer(raw, dtype=torch.uint8) if raw else torch.empty(0, dtype=torch.uint8)).to(dev)
+    else:
+        d = torch.from_numpy(np.require(data, requirements=["C", "W"])).to(dev)
+    if _is_torch(offsets):
+        d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
+    else:
+        d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
+    if d_offs.numel() < 1:
+        raise ValueError("offsets must hold at least one value")
+    return dev, d, d_offs, d_offs.numel() - 1
+
+
+def _stage_bytes(data, offsets):
+    """_stage_device for encode: the library reads sentence 0 at the byte pointer it gets, so that pointer is the byte at
+    offsets[0] and the byte count is offsets[n] - offsets[0].  Returns (device, keep-alive, pointer, byte count, int64
+    offsets tensor, n)."""
+    dev, d, d_offs, n = _stage_device(data, offsets)
+    first, last = (int(v) for v in d_offs[[0, n]].cpu())
+    return dev, d, d.data_ptr() + first, last - first, d_offs, n
+
+
+def _outputs(res, out, unsigned):
+    """Device results (CUDA tensors) as `out` asks: CUDA tensors, CPU tensors, or numpy arrays where the results at the
+    indices `unsigned` (offsets and spans) become uint64."""
+    if out == "cuda":
+        return tuple(res)
+    if out == "torch":
+        return tuple(t.cpu() for t in res)
+    return tuple(t.cpu().numpy().astype(np.uint64) if i in unsigned else t.cpu().numpy() for i, t in enumerate(res))
+
+
+def _host_buffers(out, pinned, *specs):
+    """Output buffers of a host call, one per (shape, numpy dtype): numpy arrays, or for out="torch" CPU tensors, pinned
+    like the input, with uint64 as int64.  Returns (buffers, their pointers)."""
+    if out == "torch":
+        import torch
+        dt = {np.int32: torch.int32, np.int64: torch.int64, np.uint64: torch.int64}
+        bufs = [torch.empty(shape, dtype=dt[t], pin_memory=pinned) for shape, t in specs]
+        return bufs, [b.data_ptr() for b in bufs]
+    bufs = [np.empty(shape, dtype=t) for shape, t in specs]
+    return bufs, [b.ctypes.data for b in bufs]
+
+
 class BPE:
     def __init__(self, model: str, n_threads: int = -1):
         self.model = model
@@ -74,6 +160,25 @@ class BPE:
             raise ValueError(L.yttm_api_last_error(None).decode())
         return BPE(model=model, n_threads=n_threads)
 
+    def _run_device(self, dev, call, results):
+        """Runs call() (a yttm_api_*_device call) and returns clones of what it published: results() lists (pointer,
+        typestr, shape) once the call has set the counts.  The library's result buffers are reused by the next call on
+        the handle, so they are copied under the lock."""
+        import torch
+        from .distributed import _DevView
+        torch.cuda.synchronize()   # the library runs on its own stream
+        with self._dev_lock:
+            if call() != 0:
+                raise self._err()
+            res = []
+            for ptr, ts, shape in results():
+                k = int(np.prod(shape))
+                res.append(torch.as_tensor(_DevView(ptr.value, k, ts), device=dev).view(shape).clone() if k else
+                           torch.empty(shape, dtype={"|u1": torch.uint8, "<i4": torch.int32, "<i8": torch.int64}[ts],
+                                       device=dev))
+            torch.cuda.synchronize()
+        return res
+
     # -- encode ---------------------------------------------------------------------------------
     def encode_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy",
                       with_spans=False):
@@ -88,77 +193,36 @@ class BPE:
         came from, in the coordinates of `offsets` (data[start:end]); shape (n_ids, 2), dtype and device of
         id_offsets.  An id covers a run of its word's units (code points or invalid bytes) and the invalid bytes
         between them; the word-initial "▁" and <BOS> / <EOS> have empty spans (yttm_enc_run_spans in yttm_b200.h)."""
-        if with_spans:
-            return self._encode_extra("spans", data, offsets, bos, eos, reverse, dropout_prob, out)
+        _check_out(out)
+        _check_dropout(dropout_prob)
         L = _lib.lib()
-        if out not in ("numpy", "torch", "cuda"):
-            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
-        is_torch = type(data).__module__.startswith("torch")
-        if out == "cuda" or (is_torch and data.is_cuda):
-            return self._encode_device(data, offsets, bos, eos, reverse, dropout_prob, out)
-        keep = None
-        if is_torch:
-            keep = data = data.contiguous()
-            ptr, n_bytes = data.data_ptr(), data.numel()
-        elif isinstance(data, np.ndarray):
-            keep = data = np.ascontiguousarray(data)
-            ptr, n_bytes = data.ctypes.data, data.nbytes
-        else:
-            keep = data = bytes(data) if not isinstance(data, bytes) else data
-            ptr, n_bytes = C.cast(C.c_char_p(data), C.c_void_p), len(data)
-        if type(offsets).__module__.startswith("torch"):
-            offsets = offsets.cpu().numpy()
-        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
-        n = len(offsets) - 1
-        cap = int(n_bytes) + 3 * n + 16
+        flags = (int(bos), int(eos), int(reverse), float(dropout_prob))
+        if out == "cuda" or (_is_torch(data) and data.is_cuda):
+            dev, keep, ptr, n_bytes, d_offs, n = _stage_bytes(data, offsets)
+            p, total = [C.c_void_p() for _ in range(3)], C.c_uint64(0)
+            args = (self._h, ptr, d_offs.data_ptr(), n_bytes, n) + flags + (C.byref(p[0]), C.byref(p[1]))
+            if with_spans:
+                res = self._run_device(dev, lambda: L.yttm_api_encode_spans_device(*args, C.byref(p[2]), C.byref(total)),
+                                       lambda: [(p[0], "<i4", (total.value,)), (p[1], "<i8", (n + 1,)),
+                                                (p[2], "<i8", (total.value, 2))])
+            else:
+                res = self._run_device(dev, lambda: L.yttm_api_encode_device(*args, C.byref(total)),
+                                       lambda: [(p[0], "<i4", (total.value,)), (p[1], "<i8", (n + 1,))])
+            return _outputs(res, out, (1, 2))
+        keep, ptr, n_bytes, offsets, n, pinned = _stage_host(data, offsets)
+        cap = int(n_bytes) + 3 * n + 16   # ids of a sentence of L bytes: at most L + 1 (+ <BOS> + <EOS>)
+        specs = [((cap,), np.int32), ((n + 1,), np.uint64)] + ([((cap, 2), np.uint64)] if with_spans else [])
+        bufs, ptrs = _host_buffers(out, pinned, *specs)
         total = C.c_uint64(0)
-        if out == "torch":
-            import torch
-            pin = is_torch and data.is_pinned()
-            ids = torch.empty(cap, dtype=torch.int32, pin_memory=pin)
-            oo = torch.empty(n + 1, dtype=torch.int64, pin_memory=pin)
-            p_ids, p_oo = ids.data_ptr(), oo.data_ptr()
+        args = (self._h, ptr, offsets.ctypes.data, n) + flags + (ptrs[0], cap, ptrs[1])
+        if with_spans:
+            rc = L.yttm_api_encode_spans_into(*args, ptrs[2], C.byref(total))
         else:
-            ids = np.empty(cap, dtype=np.int32)
-            oo = np.empty(n + 1, dtype=np.uint64)
-            p_ids, p_oo = ids.ctypes.data, oo.ctypes.data
-        rc = L.yttm_api_encode_ids_into(self._h, ptr, offsets.ctypes.data, n, int(bos), int(eos), int(reverse),
-                                        float(dropout_prob), p_ids, cap, p_oo, C.byref(total))
+            rc = L.yttm_api_encode_ids_into(*args, C.byref(total))
         del keep
         if rc != 0:
             raise self._err()
-        return ids[:total.value], oo
-
-    def _encode_device(self, data, offsets, bos, eos, reverse, dropout_prob, out):
-        import torch
-        from .distributed import _DevView
-        L = _lib.lib()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if type(data).__module__.startswith("torch"):
-            d_bytes = data.to(dev, non_blocking=True).contiguous()
-        else:
-            raw = data if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).tobytes()
-            d_bytes = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
-        if type(offsets).__module__.startswith("torch"):
-            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
-        else:
-            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
-        n = d_offs.numel() - 1
-        p_ids, p_off, total = C.c_void_p(), C.c_void_p(), C.c_uint64(0)
-        torch.cuda.synchronize()   # the library runs on its own stream
-        with self._dev_lock:       # the result pointers are valid until the next encode on this handle: copy under the lock
-            rc = L.yttm_api_encode_device(self._h, d_bytes.data_ptr(), d_offs.data_ptr(), d_bytes.numel(), n, int(bos), int(eos),
-                                          int(reverse), float(dropout_prob), C.byref(p_ids), C.byref(p_off), C.byref(total))
-            if rc != 0:
-                raise self._err()
-            ids = torch.as_tensor(_DevView(p_ids.value, max(total.value, 1), "<i4"), device=dev)[:total.value].clone()
-            oo = torch.as_tensor(_DevView(p_off.value, n + 1, "<i8"), device=dev).clone()
-            torch.cuda.synchronize()
-        if out == "cuda":
-            return ids, oo
-        if out == "torch":
-            return ids.cpu(), oo.cpu()
-        return ids.cpu().numpy(), oo.cpu().numpy().astype(np.uint64)
+        return (bufs[0][:total.value], bufs[1]) + ((bufs[2][:total.value],) if with_spans else ())
 
     def encode_padded(self, data, offsets, max_length=None, pad_id=None, bos=False, eos=False, reverse=False,
                       dropout_prob=0.0, out="numpy", with_spans=False):
@@ -170,8 +234,7 @@ class BPE:
         draws and the dropout_seed counter advance as in encode_packed.  Returns (ids int32 [N, L], lengths int64 [N])
         and with with_spans also spans [N, L, 2] (encode_packed's span of every kept id, [offsets[i+1], offsets[i+1])
         for pads) as numpy arrays (spans uint64), CPU torch tensors (out="torch") or CUDA tensors (out="cuda")."""
-        if out not in ("numpy", "torch", "cuda"):
-            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+        _check_out(out)
         _check_dropout(dropout_prob)
         if max_length is not None:
             if isinstance(max_length, bool) or not isinstance(max_length, (int, np.integer)):
@@ -188,155 +251,57 @@ class BPE:
             pad = int(pad_id)
             if not -2**31 <= pad < 2**31:
                 raise ValueError("pad_id must fit in int32. Current value of pad_id = %d" % pad)
-        is_torch = type(data).__module__.startswith("torch")
-        if out == "cuda" or (is_torch and data.is_cuda) or max_length is None:
-            return self._encode_padded_device(data, offsets, max_length or 0, pad, bos, eos, reverse, dropout_prob, out,
-                                              with_spans)
         L = _lib.lib()
-        if is_torch:
-            keep = data = data.contiguous()
-            ptr = data.data_ptr()
-        elif isinstance(data, np.ndarray):
-            keep = data = np.ascontiguousarray(data)
-            ptr = data.ctypes.data
-        else:
-            keep = data = bytes(data) if not isinstance(data, bytes) else data
-            ptr = C.cast(C.c_char_p(data), C.c_void_p)
-        if type(offsets).__module__.startswith("torch"):
-            offsets = offsets.cpu().numpy()
-        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
-        n = len(offsets) - 1
-        if n < 0:
-            raise ValueError("offsets must hold at least one value")
+        flags = (int(bos), int(eos), int(reverse), float(dropout_prob))
+        if out == "cuda" or (_is_torch(data) and data.is_cuda) or max_length is None:
+            dev, keep, ptr, n_bytes, d_offs, n = _stage_bytes(data, offsets)
+            p, w = [C.c_void_p() for _ in range(3)], C.c_uint32(0)
+            res = self._run_device(
+                dev, lambda: L.yttm_api_encode_padded_device(self._h, ptr, d_offs.data_ptr(), n_bytes, n, *flags,
+                                                             max_length or 0, pad, int(with_spans), C.byref(p[0]),
+                                                             C.byref(p[1]), C.byref(p[2]), C.byref(w)),
+                lambda: [(p[0], "<i4", (n, w.value)), (p[1], "<i8", (n,))] +
+                        ([(p[2], "<i8", (n, w.value, 2))] if with_spans else []))
+            return _outputs(res, out, (2,))
+        keep, ptr, _, offsets, n, pinned = _stage_host(data, offsets)
         W = max_length
-        if out == "torch":
-            import torch
-            pin = is_torch and data.is_pinned()
-            ids = torch.empty((n, W), dtype=torch.int32, pin_memory=pin)
-            lengths = torch.empty(n, dtype=torch.int64, pin_memory=pin)
-            spans = torch.empty((n, W, 2), dtype=torch.int64, pin_memory=pin) if with_spans else None
-            ptrs = ids.data_ptr(), lengths.data_ptr(), spans.data_ptr() if with_spans else None
-        else:
-            ids, lengths = np.empty((n, W), dtype=np.int32), np.empty(n, dtype=np.int64)
-            spans = np.empty((n, W, 2), dtype=np.uint64) if with_spans else None
-            ptrs = ids.ctypes.data, lengths.ctypes.data, spans.ctypes.data if with_spans else None
-        rc = L.yttm_api_encode_padded_into(self._h, ptr, offsets.ctypes.data, n, int(bos), int(eos), int(reverse),
-                                           float(dropout_prob), W, pad, *ptrs)
+        specs = [((n, W), np.int32), ((n,), np.int64)] + ([((n, W, 2), np.uint64)] if with_spans else [])
+        bufs, ptrs = _host_buffers(out, pinned, *specs)
+        rc = L.yttm_api_encode_padded_into(self._h, ptr, offsets.ctypes.data, n, *flags, W, pad, ptrs[0], ptrs[1],
+                                           ptrs[2] if with_spans else None)
         del keep
         if rc != 0:
             raise self._err()
-        return (ids, lengths, spans) if with_spans else (ids, lengths)
-
-    def _encode_padded_device(self, data, offsets, width, pad, bos, eos, reverse, dropout_prob, out, with_spans):
-        import torch
-        from .distributed import _DevView
-        L = _lib.lib()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if type(data).__module__.startswith("torch"):
-            d_bytes = data.to(dev, non_blocking=True).contiguous()
-        else:
-            raw = data if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).tobytes()
-            d_bytes = (torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev) if raw
-                       else torch.empty(0, dtype=torch.uint8, device=dev))
-        if type(offsets).__module__.startswith("torch"):
-            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
-        else:
-            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
-        n = d_offs.numel() - 1
-        if n < 0:
-            raise ValueError("offsets must hold at least one value")
-        first, last = (int(v) for v in d_offs[[0, n]].cpu())
-        p = [C.c_void_p() for _ in range(3)]
-        w = C.c_uint32(0)
-
-        def view(ptr, shape, ts):
-            k = int(np.prod(shape))
-            if k == 0:
-                return torch.empty(shape, dtype={"<i4": torch.int32, "<i8": torch.int64}[ts], device=dev)
-            return torch.as_tensor(_DevView(ptr.value, k, ts), device=dev).view(shape).clone()
-
-        torch.cuda.synchronize()   # the library runs on its own stream
-        with self._dev_lock:       # the result pointers are valid until the next encode on this handle: copy under the lock
-            # the library reads sentence 0 at the byte pointer it gets: the byte at offsets[0]
-            rc = L.yttm_api_encode_padded_device(self._h, d_bytes.data_ptr() + first, d_offs.data_ptr(), last - first, n,
-                                                 int(bos), int(eos), int(reverse), float(dropout_prob), width, pad,
-                                                 int(with_spans), C.byref(p[0]), C.byref(p[1]), C.byref(p[2]),
-                                                 C.byref(w))
-            if rc != 0:
-                raise self._err()
-            W = w.value
-            res = [view(p[0], (n, W), "<i4"), view(p[1], (n,), "<i8")]
-            if with_spans:
-                res.append(view(p[2], (n, W, 2), "<i8"))
-            torch.cuda.synchronize()
-        if out == "cuda":
-            return tuple(res)
-        if out == "torch":
-            return tuple(t.cpu() for t in res)
-        res = [t.cpu().numpy() for t in res]
-        if with_spans:
-            res[2] = res[2].astype(np.uint64)
-        return tuple(res)
+        return tuple(bufs)
 
     def encode_subwords_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy"):
         """encode(output_type=SUBWORD) of a packed batch on the GPU (inputs as for encode_packed).  Returns
         (piece_bytes uint8, piece_offsets, sentence_offsets): piece k = piece_bytes[piece_offsets[k]:piece_offsets[k+1]]
         as UTF-8, the pieces of sentence i = [sentence_offsets[i], sentence_offsets[i+1]); offsets are uint64 numpy
         arrays for out="numpy", int64 tensors for "torch" / "cuda"."""
-        return self._encode_extra("subwords", data, offsets, bos, eos, reverse, dropout_prob, out)
-
-    def _encode_extra(self, kind, data, offsets, bos, eos, reverse, dropout_prob, out):
-        """encode_packed(with_spans=True) / encode_subwords_packed."""
-        if out not in ("numpy", "torch", "cuda"):
-            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+        _check_out(out)
         _check_dropout(dropout_prob)
-        is_torch = type(data).__module__.startswith("torch")
-        if out == "cuda" or (is_torch and data.is_cuda):
-            return self._encode_extra_device(kind, data, offsets, bos, eos, reverse, dropout_prob, out)
         L = _lib.lib()
-        if is_torch:
-            keep = data = data.contiguous()
-            ptr, n_bytes = data.data_ptr(), data.numel()
-        elif isinstance(data, np.ndarray):
-            keep = data = np.ascontiguousarray(data)
-            ptr, n_bytes = data.ctypes.data, data.nbytes
-        else:
-            keep = data = bytes(data) if not isinstance(data, bytes) else data
-            ptr, n_bytes = C.cast(C.c_char_p(data), C.c_void_p), len(data)
-        if type(offsets).__module__.startswith("torch"):
-            offsets = offsets.cpu().numpy()
-        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
-        n = len(offsets) - 1
-        if n < 0:
-            raise ValueError("offsets must hold at least one value")
-        cap = int(n_bytes) + 3 * n + 16   # ids of a sentence of L bytes: at most L + 1 (+ <BOS> + <EOS>)
-        args = (self._h, ptr, offsets.ctypes.data, n, int(bos), int(eos), int(reverse), float(dropout_prob))
-        if kind == "spans":
-            total = C.c_uint64(0)
-            if out == "torch":
-                import torch
-                pin = is_torch and data.is_pinned()
-                ids = torch.empty(cap, dtype=torch.int32, pin_memory=pin)
-                oo = torch.empty(n + 1, dtype=torch.int64, pin_memory=pin)
-                spans = torch.empty((cap, 2), dtype=torch.int64, pin_memory=pin)
-                ptrs = ids.data_ptr(), oo.data_ptr(), spans.data_ptr()
-            else:
-                ids, oo = np.empty(cap, dtype=np.int32), np.empty(n + 1, dtype=np.uint64)
-                spans = np.empty((cap, 2), dtype=np.uint64)
-                ptrs = ids.ctypes.data, oo.ctypes.data, spans.ctypes.data
-            rc = L.yttm_api_encode_spans_into(*args, ptrs[0], cap, ptrs[1], ptrs[2], C.byref(total))
-            del keep
-            if rc != 0:
-                raise self._err()
-            return ids[:total.value], oo, spans[:total.value]
+        flags = (int(bos), int(eos), int(reverse), float(dropout_prob))
+        if out == "cuda" or (_is_torch(data) and data.is_cuda):
+            dev, keep, ptr, n_bytes, d_offs, n = _stage_bytes(data, offsets)
+            p, n_p, n_b = [C.c_void_p() for _ in range(3)], C.c_uint64(0), C.c_uint64(0)
+            res = self._run_device(
+                dev, lambda: L.yttm_api_encode_subwords_device(self._h, ptr, d_offs.data_ptr(), n_bytes, n, *flags,
+                                                               C.byref(p[0]), C.byref(p[1]), C.byref(p[2]),
+                                                               C.byref(n_p), C.byref(n_b)),
+                lambda: [(p[0], "|u1", (n_b.value,)), (p[1], "<i8", (n_p.value + 1,)), (p[2], "<i8", (n + 1,))])
+            return _outputs(res, out, (1, 2))
+        keep, ptr, n_bytes, offsets, n, _ = _stage_host(data, offsets)
+        cap = int(n_bytes) + 3 * n + 16   # one piece per id
         # a piece is its units' bytes plus a leading U+2581 (3 bytes, at most one per word) or "<BOS>" / "<EOS>"
         bytes_cap = 4 * int(n_bytes) + 10 * n + 16
         text = np.empty(bytes_cap, dtype=np.uint8)
         po = np.empty(cap + 1, dtype=np.uint64)
         so = np.empty(n + 1, dtype=np.uint64)
         n_p, n_b = C.c_uint64(0), C.c_uint64(0)
-        rc = L.yttm_api_encode_subwords_into(*args, text.ctypes.data, bytes_cap, po.ctypes.data, cap, so.ctypes.data,
-                                             C.byref(n_p), C.byref(n_b))
+        rc = L.yttm_api_encode_subwords_into(self._h, ptr, offsets.ctypes.data, n, *flags, text.ctypes.data, bytes_cap,
+                                             po.ctypes.data, cap, so.ctypes.data, C.byref(n_p), C.byref(n_b))
         del keep
         if rc != 0:
             raise self._err()
@@ -345,57 +310,6 @@ class BPE:
             import torch
             return torch.from_numpy(text), torch.from_numpy(po.astype(np.int64)), torch.from_numpy(so.astype(np.int64))
         return text, po, so
-
-    def _encode_extra_device(self, kind, data, offsets, bos, eos, reverse, dropout_prob, out):
-        import torch
-        from .distributed import _DevView
-        L = _lib.lib()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if type(data).__module__.startswith("torch"):
-            d_bytes = data.to(dev, non_blocking=True).contiguous()
-        else:
-            raw = data if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).tobytes()
-            d_bytes = (torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev) if raw
-                       else torch.empty(0, dtype=torch.uint8, device=dev))
-        if type(offsets).__module__.startswith("torch"):
-            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
-        else:
-            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
-        n = d_offs.numel() - 1
-        if n < 0:
-            raise ValueError("offsets must hold at least one value")
-        first, last = (int(v) for v in d_offs[[0, n]].cpu())
-        # the library reads sentence 0 at the byte pointer it gets: the byte at offsets[0]
-        args = (self._h, d_bytes.data_ptr() + first, d_offs.data_ptr(), last - first, n, int(bos), int(eos), int(reverse),
-                float(dropout_prob))
-        p = [C.c_void_p() for _ in range(3)]
-        n_a, n_b = C.c_uint64(0), C.c_uint64(0)
-
-        def view(ptr, k, ts):
-            if k == 0:
-                return torch.empty(0, dtype={"|u1": torch.uint8, "<i4": torch.int32, "<i8": torch.int64}[ts], device=dev)
-            return torch.as_tensor(_DevView(ptr.value, k, ts), device=dev).clone()
-
-        torch.cuda.synchronize()   # the library runs on its own stream
-        with self._dev_lock:       # the result pointers are valid until the next encode on this handle: copy under the lock
-            if kind == "spans":
-                rc = L.yttm_api_encode_spans_device(*args, C.byref(p[0]), C.byref(p[1]), C.byref(p[2]), C.byref(n_a))
-                if rc != 0:
-                    raise self._err()
-                res = (view(p[0], n_a.value, "<i4"), view(p[1], n + 1, "<i8"),
-                       view(p[2], 2 * n_a.value, "<i8").view(n_a.value, 2))
-            else:
-                rc = L.yttm_api_encode_subwords_device(*args, C.byref(p[0]), C.byref(p[1]), C.byref(p[2]), C.byref(n_a),
-                                                       C.byref(n_b))
-                if rc != 0:
-                    raise self._err()
-                res = (view(p[0], n_b.value, "|u1"), view(p[1], n_a.value + 1, "<i8"), view(p[2], n + 1, "<i8"))
-            torch.cuda.synchronize()
-        if out == "cuda":
-            return res
-        if out == "torch":
-            return tuple(t.cpu() for t in res)
-        return tuple(t.cpu().numpy() if t.dtype == torch.uint8 else t.cpu().numpy().astype(np.uint64) for t in res)
 
     def _pieces(self, need):
         """The calling thread's last length-framed piece list -> list of sentences, each a list of str."""
@@ -477,26 +391,29 @@ class BPE:
           out="numpy"  numpy uint8 + uint64 arrays,
           out="torch"  CPU torch tensors (uint8 + int64),
           out="cuda"   CUDA torch tensors: ids uploaded if needed, results stay on the device."""
-        if out not in ("numpy", "torch", "cuda"):
-            raise ValueError("out must be 'numpy', 'torch' or 'cuda'")
+        _check_out(out)
         if not isinstance(ignore_ids, Collection) and ignore_ids is not None:
             raise TypeError("{} is not a Collection instance".format(type(ignore_ids)))
         ignore = sorted({int(i) for i in ignore_ids}) if ignore_ids else []
-        is_torch = type(ids).__module__.startswith("torch")
-        if out == "cuda" or (is_torch and ids.is_cuda):
-            return self._decode_device(ids, offsets, ignore, out)
-        ids = ids.numpy() if is_torch else np.asarray(ids)
-        if type(offsets).__module__.startswith("torch"):
-            offsets = offsets.cpu().numpy()
-        offsets = np.ascontiguousarray(offsets).astype(np.uint64, copy=False)
-        n = len(offsets) - 1
-        if n < 0:
-            raise ValueError("offsets must hold at least one value")
+        L = _lib.lib()
+        if out == "cuda" or (_is_torch(ids) and ids.is_cuda):
+            import torch
+            dev, d_ids, d_offs, n = _stage_device(ids, offsets)
+            d_ids, extra = self._ids_int32(d_ids, lambda: d_offs.cpu().numpy().astype(np.uint64), ignore, torch)
+            ign = np.asarray([i for i in ignore if -2**31 <= i < 2**31] + extra, dtype=np.int32)
+            p_text, p_off, total = C.c_void_p(), C.c_void_p(), C.c_uint64(0)
+            res = self._run_device(
+                dev, lambda: L.yttm_api_decode_device(self._h, d_ids.data_ptr(), d_ids.numel(), d_offs.data_ptr(), n,
+                                                      ign.ctypes.data, len(ign), C.byref(p_text), C.byref(p_off),
+                                                      C.byref(total)),
+                lambda: [(p_text, "|u1", (total.value,)), (p_off, "<i8", (n + 1,))])
+            return _outputs(res, out, (1,))
+        ids = ids.numpy() if _is_torch(ids) else np.asarray(ids)
+        offsets, n = _host_offsets(offsets)
         if int(offsets[-1]) > len(ids):
             raise ValueError(_offsets_error(len(ids)))
         ids, extra = self._ids_int32(ids, lambda: offsets, ignore, np)
         ign = np.asarray([i for i in ignore if -2**31 <= i < 2**31] + extra, dtype=np.int32)
-        L = _lib.lib()
         total = C.c_uint64(0)
         cap = 8 * (int(offsets[-1]) - int(offsets[0])) + 64   # a first guess; the exact size on return code 2
         for _ in range(2):
@@ -553,43 +470,6 @@ class BPE:
         if xp is np:
             return np.ascontiguousarray(np.where(big, -1, ids).astype(np.int32)), [-1]
         return torch.where(big, torch.full_like(ids, -1), ids).to(torch.int32).contiguous(), [-1]
-
-    def _decode_device(self, ids, offsets, ignore, out):
-        import torch
-        from .distributed import _DevView
-        L = _lib.lib()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if type(ids).__module__.startswith("torch"):
-            d_ids = ids.to(dev)
-        else:
-            d_ids = torch.from_numpy(np.ascontiguousarray(ids)).to(dev)
-        if type(offsets).__module__.startswith("torch"):
-            d_offs = offsets.to(dev, dtype=torch.int64).contiguous()
-        else:
-            d_offs = torch.from_numpy(np.ascontiguousarray(offsets).astype(np.int64)).to(dev)
-        n = d_offs.numel() - 1
-        if n < 0:
-            raise ValueError("offsets must hold at least one value")
-        d_ids, extra = self._ids_int32(d_ids, lambda: d_offs.cpu().numpy().astype(np.uint64), ignore, torch)
-        ign = np.asarray([i for i in ignore if -2**31 <= i < 2**31] + extra, dtype=np.int32)
-        p_text, p_off, total = C.c_void_p(), C.c_void_p(), C.c_uint64(0)
-        torch.cuda.synchronize()   # the library runs on its own stream
-        with self._dev_lock:       # the result pointers are valid until the next decode on this handle: copy under the lock
-            rc = L.yttm_api_decode_device(self._h, d_ids.data_ptr(), d_ids.numel(), d_offs.data_ptr(), n, ign.ctypes.data,
-                                          len(ign), C.byref(p_text), C.byref(p_off), C.byref(total))
-            if rc != 0:
-                raise self._err()
-            if total.value:
-                text = torch.as_tensor(_DevView(p_text.value, total.value, "|u1"), device=dev).clone()
-            else:
-                text = torch.empty(0, dtype=torch.uint8, device=dev)
-            oo = torch.as_tensor(_DevView(p_off.value, n + 1, "<i8"), device=dev).clone()
-            torch.cuda.synchronize()
-        if out == "cuda":
-            return text, oo
-        if out == "torch":
-            return text.cpu(), oo.cpu()
-        return text.cpu().numpy(), oo.cpu().numpy().astype(np.uint64)
 
     # -- BPE-dropout stream ---------------------------------------------------------------------
     def dropout_seed(self, seed: int):
