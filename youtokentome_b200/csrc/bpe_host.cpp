@@ -16,6 +16,7 @@
 
 #include "../../include/bpe_b200.h"
 #include "../../include/yttm_b200.h"
+#include "common.cuh"
 
 namespace vkcom {
 
@@ -335,8 +336,8 @@ static Status train_on_buffer(const char *text, uint64_t n, int n_tokens, const 
   // a context fixes its launch geometry when it first trains: the knobs that shape it are part of the cache key, so a
   // changed setting takes effect in a running process (the A/B tools and the tests vary them between calls)
   std::string geometry;
-  for (const char *k : {"YTTM_STAGES", "YTTM_LOOP_THREADS", "YT_EMU_SMS"}) {
-    const char *v = std::getenv(k);
+  for (const char *const *k = yttm_geometry_knobs; *k; k++) {
+    const char *v = std::getenv(*k);
     geometry += v ? v : "";
     geometry += '|';
   }

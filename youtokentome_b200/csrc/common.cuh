@@ -3,6 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <climits>
+#include <cstdlib>
 #include <map>
 #include <string>
 #include <vector>
@@ -114,6 +117,10 @@ struct yttm_ctx {
 
 extern thread_local std::string g_yttm_create_error;
 
+// The environment knobs that fix a context's launch geometry when it first trains (train.cu; NULL-terminated): a cache
+// of contexts must key on their values.  YT_EMU_SMS is the SM count of the CPU emulation used by the tests.
+extern const char *const yttm_geometry_knobs[];
+
 // exclusive scan of uint64 on the context stream (train.cu); *d_total receives the sum
 int yttm_device_scan_u64(yttm_ctx *c, const unsigned long long *in, uint64_t n, unsigned long long *out,
                          unsigned long long *d_total);
@@ -157,4 +164,12 @@ inline double timer_ms(yttm_ctx *c, const char *name) {
   return (double)t.ms;
 }
 inline uint64_t pow2ceil(uint64_t x) { uint64_t p = 1; while (p < x) p <<= 1; return p; }
+// The library's environment knobs (DESIGN §7.5).  env_int: `dflt` when `name` is unset, else its integer value clamped
+// to [lo, hi].  A knob is read where it takes effect: the geometry knobs (yttm_geometry_knobs) once per context, the
+// others on every call.
+inline bool env_set(const char *name) { return std::getenv(name) != nullptr; }
+inline int env_int(const char *name, int dflt, int lo, int hi) {
+  const char *e = std::getenv(name);
+  return e ? std::min(hi, std::max(lo, std::atoi(e))) : dflt;
+}
 }  // namespace ytc

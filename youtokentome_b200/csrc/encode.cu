@@ -1250,7 +1250,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
       YT_CUDA(c, cudaMemsetAsync(ll.n, 0, 8, c->stream));
       // table: 2 slots per occurrence up to 2^21 slots (16 MB, L2-resident); beyond that it works as a cache
       uint64_t tslots = std::max<uint64_t>(ytc::pow2ceil(std::min<uint64_t>(n_words, 1ull << 20) * 2), 1024);
-      if (const char *env = std::getenv("YTTM_ENC_DEDUP_SLOTS")) tslots = ytc::pow2ceil((uint64_t)std::max(1, std::atoi(env)));  // tests: tiny tables
+      if (const int v = ytc::env_int("YTTM_ENC_DEDUP_SLOTS", 0, 1, INT_MAX)) tslots = ytc::pow2ceil((uint64_t)v);  // tests: tiny tables
       YT_CUDA(c, e->dd_tab.reserve(tslots * 8));
       YT_CUDA(c, e->dd_rep.reserve(n_words * 4 + 16));
       YT_CUDA(c, e->dd_list.reserve(n_words * 4 + 16));
@@ -1258,7 +1258,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
       d.tab = e->dd_tab.as<unsigned long long>(); d.mask = (uint32_t)(tslots - 1);
       d.rep = e->dd_rep.as<uint32_t>(); d.list = e->dd_list.as<uint32_t>();
       d.n_list = e->counter.as<unsigned long long>() + 2;  // zeroed with the other counters above
-      d.weak_tag = std::getenv("YTTM_ENC_DEDUP_WEAKTAG") != nullptr;  // tests: tag collisions everywhere
+      d.weak_tag = ytc::env_set("YTTM_ENC_DEDUP_WEAKTAG");  // tests: tag collisions everywhere
       d_rep = d.rep;
       YT_CUDA(c, cudaMemsetAsync(d.tab, 0xff, tslots * 8, c->stream));
       ytc::timer_begin(c, "enc_dedup");
@@ -1418,8 +1418,7 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
   }
   // chunks of about CHUNK bytes, cut at sentence boundaries; chunk i lives in slot i & 1
   const uint64_t total_bytes = offsets[n_sent] - offsets[0];
-  uint64_t chunk_bytes = 32ull << 20;
-  if (const char *env = std::getenv("YTTM_ENC_CHUNK_MB")) chunk_bytes = (uint64_t)std::max(1, std::atoi(env)) << 20;
+  const uint64_t chunk_bytes = (uint64_t)ytc::env_int("YTTM_ENC_CHUNK_MB", 32, 1, INT_MAX) << 20;
   std::vector<uint64_t> cut(1, 0);  // sentence indices
   while (cut.back() < n_sent) {
     const uint64_t lo = cut.back();

@@ -55,6 +55,15 @@ constexpr uint32_t XQ_CNT_COMPACT = 0x20000000u;  // count word: > 25 % of the b
 constexpr uint32_t XQ_CNT_PLIMIT = 0x10000000u;   // count word: the block's partition is over the load limit
 constexpr uint32_t XQ_CNT_PFULL = 0x08000000u;    // count word: the block's partition ran full (an update was lost)
 constexpr uint32_t XQ_CNT_MASK = 0x07ffffffu;
+// ORs the XQF_* flags of count word c into `flags`.  XQ_CNT_MORE is only set by the out-of-loop table rounds: `more`
+// says whether to map it.
+__device__ __forceinline__ void cnt_flags(uint32_t &flags, uint32_t c, bool more) {
+  if (c & XQ_CNT_OVF) flags |= XQF_OVERFLOW;
+  if (more && (c & XQ_CNT_MORE)) flags |= XQF_MORE;
+  if (c & XQ_CNT_COMPACT) flags |= XQF_COMPACT;
+  if (c & XQ_CNT_PLIMIT) flags |= XQF_PLIMIT;
+  if (c & XQ_CNT_PFULL) flags |= XQF_PFULL;
+}
 // What bounds the exchange is the SM's load/store unit, not L2: a warp-wide load or store costs ~2 cycles per
 // 128-byte line it touches, so 32 lanes on 32 lines are 64 cycles, and a POLL LOOP that does this from 16 warps keeps
 // the unit busy for a microsecond per sweep.  Hence the layout:
@@ -240,6 +249,17 @@ inline unsigned long long gtimer() {
 }
 inline void loop_trap() { fprintf(stderr, "emu: merge loop gave up waiting for a peer\n"); abort(); }
 #endif
+// One trip of a wait on a peer: a peer that stays silent for limit_ns traps the kernel (never hang the box).  The clock
+// is read every 4096 trips only; t0 = 0 before the first reading.  The emulator yields to the other fibers.
+__device__ __forceinline__ void spin_step(uint32_t spin, unsigned long long &t0, unsigned long long limit_ns) {
+#ifdef YT_SIMT_EMU
+  emu::yield();
+#endif
+  if ((spin & 4095u) == 4095u) {
+    if (!t0) t0 = gtimer();
+    else if (gtimer() - t0 > limit_ns) loop_trap();
+  }
+}
 __device__ __forceinline__ Best warp_best(Best v) {
   for (int o = 16; o > 0; o >>= 1) {
     Best w;
@@ -281,6 +301,17 @@ __device__ __forceinline__ void xq_store(const LoopArgs &a, const XqOut &o, uint
 __device__ __forceinline__ void xq_push1(const LoopArgs &a, const XqOut &o, unsigned long long key, long long delta) {
   xq_store(a, o, atomicAdd(o.s_n, 1u), key, delta);
 }
+// One thread rewrites word t (`cap` token slots) that holds (x,y): -old pairs, rewrite, +new pairs.  The merges are
+// added to `merges` (a 32- or 64-bit counter).
+template <class N>
+__device__ __forceinline__ void apply_word_scalar(uint32_t *t, uint32_t cap, long long f, const MergeOp &op,
+                                                  const LoopArgs &a, const XqOut &xo, N &merges) {
+  for_each_pair(t, cap, [&](uint64_t key, uint64_t mult) {
+    if (key != op.key) xq_push1(a, xo, key, -(long long)mult * f);
+  });
+  merges += rewrite_word(t, cap, op.x, op.y, op.z);
+  for_each_pair(t, cap, [&](uint64_t key, uint64_t mult) { xq_push1(a, xo, key, (long long)mult * f); });
+}
 
 // Run structure of <= 32 live tokens held one per lane (t == DEAD beyond the n live ones): every
 // run start owns floor(L/2) self pairs and one cross pair to the next run (for_each_pair()).
@@ -307,13 +338,7 @@ __device__ __forceinline__ uint32_t warp_apply_word(uint32_t *st, uint32_t cap, 
                                                     const XqOut &xo) {
   if (cap > 32) {  // long word: scalar path on lane 0 (exact, slow)
     uint32_t merges = 0;
-    if (lane == 0) {
-      for_each_pair(st, cap, [&](uint64_t key, uint64_t mult) {
-        if (key != op.key) xq_push1(a, xo, key, -(long long)mult * f);
-      });
-      merges = rewrite_word(st, cap, op.x, op.y, op.z);
-      for_each_pair(st, cap, [&](uint64_t key, uint64_t mult) { xq_push1(a, xo, key, (long long)mult * f); });
-    }
+    if (lane == 0) apply_word_scalar(st, cap, f, op, a, xo, merges);
     __syncwarp();
     if (gt)
       for (uint32_t i = lane; i < cap; i += 32) gt[i] = st[i];
@@ -375,6 +400,23 @@ __device__ __forceinline__ uint32_t warp_apply_word(uint32_t *st, uint32_t cap, 
   return n - n2;
 }
 
+// Bit k: token k and token k+1 of the eight tokens v, u, nxt are (x,y).
+__device__ __forceinline__ uint32_t match8(const uint4 &v, const uint4 &u, uint32_t nxt, const MergeOp &op) {
+  return (v.x == op.x && v.y == op.y ? 1u : 0u) | (v.y == op.x && v.z == op.y ? 2u : 0u) |
+         (v.z == op.x && v.w == op.y ? 4u : 0u) | (v.w == op.x && u.x == op.y ? 8u : 0u) |
+         (u.x == op.x && u.y == op.y ? 16u : 0u) | (u.y == op.x && u.z == op.y ? 32u : 0u) |
+         (u.z == op.x && u.w == op.y ? 64u : 0u) | (u.w == op.x && nxt == op.y ? 128u : 0u);
+}
+// The word that holds token i: the largest w < nw with off[w] - base <= i.
+__device__ __forceinline__ uint32_t word_at(const uint32_t *off, uint32_t nw, uint32_t i, uint32_t base) {
+  uint32_t lo = 0, hi = nw;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (off[mid] - base <= i) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // One RESIDENT tile: its token slots sit in shared memory (`span` slots at stok, word w at
 // [soff[w], soff[w+1])).  The scan is TOKEN-parallel: a lane compares four consecutive slots and
 // the one after them with (x, y) — consecutive lanes read consecutive 16-byte pieces of shared
@@ -398,10 +440,7 @@ __device__ __forceinline__ unsigned long long process_tile(uint32_t *stok, const
     if (p + 4 < span) u = *reinterpret_cast<const uint4 *>(stok + p + 4);
     uint32_t nxt = __shfl_down_sync(0xffffffffu, v.x, 1);
     if (lane == 31) nxt = p + 8 < span ? stok[p + 8] : DEAD;
-    uint32_t m = (v.x == op.x && v.y == op.y ? 1u : 0u) | (v.y == op.x && v.z == op.y ? 2u : 0u) |
-                 (v.z == op.x && v.w == op.y ? 4u : 0u) | (v.w == op.x && u.x == op.y ? 8u : 0u) |
-                 (u.x == op.x && u.y == op.y ? 16u : 0u) | (u.y == op.x && u.z == op.y ? 32u : 0u) |
-                 (u.z == op.x && u.w == op.y ? 64u : 0u) | (u.w == op.x && nxt == op.y ? 128u : 0u);
+    uint32_t m = match8(v, u, nxt, op);
     if (p + 8 >= span) m &= span > p + 1 ? (1u << (span - p - 1)) - 1u : 0u;  // occurrence i needs i + 1 < span
     while (__ballot_sync(0xffffffffu, m != 0)) {  // one round per hit of the busiest lane (almost always one)
       uint32_t w = 0, o = 0, cap = 0;
@@ -411,12 +450,7 @@ __device__ __forceinline__ unsigned long long process_tile(uint32_t *stok, const
         m &= m - 1u;
         // re-read: an earlier round (or another warp) may already have rewritten this word
         if (stok[i] == op.x && stok[i + 1] == op.y) {
-          uint32_t lo = 0, hi = nw;  // largest w with soff[w] <= i
-          while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (soff[mid] <= i) lo = mid; else hi = mid;
-          }
-          w = lo;
+          w = word_at(soff, nw, i, 0);
           o = soff[w];
           cap = soff[w + 1] - o;
           own = !((atomicOr(&claim[w >> 5], 1u << (w & 31)) >> (w & 31)) & 1u);
@@ -447,12 +481,7 @@ __device__ __forceinline__ unsigned long long process_tile_direct(uint32_t *tok,
     uint32_t o = off[w], wcap = off[w + 1] - o;
     uint32_t *t = tok + o;
     if (!has_pair(t, wcap, op.x, op.y)) continue;
-    long long f = (long long)freq[w];
-    for_each_pair(t, wcap, [&](uint64_t key, uint64_t mult) {
-      if (key != op.key) xq_push1(a, xo, key, -(long long)mult * f);
-    });
-    dead += rewrite_word(t, wcap, op.x, op.y, op.z);
-    for_each_pair(t, wcap, [&](uint64_t key, uint64_t mult) { xq_push1(a, xo, key, (long long)mult * f); });
+    apply_word_scalar(t, wcap, (long long)freq[w], op, a, xo, dead);
   }
   return dead;
 }
@@ -524,6 +553,12 @@ inline void mbar_wait(unsigned long long *bar, uint32_t parity) {  // returns on
   }
 }
 #endif
+// Tile descriptors travel in lane-distributed batches: lane j of a warp holds tile_desc[base + j], and tile base + j
+// (j < 31) takes its first and last descriptor (d0, d1) from lanes j and j + 1.
+__device__ __forceinline__ void tile_pair(uint2 batch, uint32_t j, uint2 &d0, uint2 &d1) {
+  d0.x = __shfl_sync(0xffffffffu, batch.x, j);     d0.y = __shfl_sync(0xffffffffu, batch.y, j);
+  d1.x = __shfl_sync(0xffffffffu, batch.x, j + 1); d1.y = __shfl_sync(0xffffffffu, batch.y, j + 1);
+}
 // bytes of a 16-byte aligned window [lo & ~3, roundup(hi, 4)) over uint32 elements
 __device__ __forceinline__ uint32_t win_lo(uint32_t lo) { return lo & ~3u; }
 __device__ __forceinline__ uint32_t win_bytes(uint32_t lo, uint32_t hi) { return (((hi + 3u) & ~3u) - (lo & ~3u)) * 4u; }
@@ -561,20 +596,10 @@ __device__ __forceinline__ void xq_poll_counts(const LoopArgs &a, uint32_t round
     for (uint32_t spin = 0;; spin++) {
       v = ld_relaxed_any(w, sys);   // entries validate themselves: no acquire needed
       if ((uint32_t)(v >> 32) == round) break;
-#ifdef YT_SIMT_EMU
-      emu::yield();
-#endif
-      if ((spin & 4095u) == 4095u) {
-        if (!t0) t0 = gtimer();
-        else if (gtimer() - t0 > a.spin_limit_ns) loop_trap();
-      }
+      spin_step(spin, t0, a.spin_limit_ns);
     }
     const uint32_t c = (uint32_t)v;
-    if (c & XQ_CNT_OVF) flags |= XQF_OVERFLOW;
-    if (c & XQ_CNT_MORE) flags |= XQF_MORE;
-    if (c & XQ_CNT_COMPACT) flags |= XQF_COMPACT;
-    if (c & XQ_CNT_PLIMIT) flags |= XQF_PLIMIT;
-    if (c & XQ_CNT_PFULL) flags |= XQF_PFULL;
+    cnt_flags(flags, c, true);
     uint32_t n = c & XQ_CNT_MASK;
     if (n > a.xq.seg_cap) n = a.xq.seg_cap;
     s_pref[j] = (skip_self && s == a.xq.me) ? 0u : n;
@@ -640,15 +665,8 @@ __device__ __forceinline__ void xq_entry(const LoopArgs &a, uint32_t round, cons
       : reinterpret_cast<const unsigned long long *>(xq_base(a.xq, a.xq.me) + xq_seg_off(a.xq, round & 1u, s, b) + (size_t)idx * sizeof(uint4));
   const bool sys = a.xq.world > 1;
   unsigned long long t0 = 0;
-  for (uint32_t spin = 0; !xq_unpack(ld_relaxed_any(ep, sys), ld_relaxed_any(ep + 1, sys), round % XQ_STAMP_MOD, key, delta); spin++) {
-#ifdef YT_SIMT_EMU
-    emu::yield();
-#endif
-    if ((spin & 4095u) == 4095u) {   // the count word overtook the entry: it is on its way
-      if (!t0) t0 = gtimer();
-      else if (gtimer() - t0 > a.spin_limit_ns) loop_trap();
-    }
-  }
+  for (uint32_t spin = 0; !xq_unpack(ld_relaxed_any(ep, sys), ld_relaxed_any(ep + 1, sys), round % XQ_STAMP_MOD, key, delta); spin++)
+    spin_step(spin, t0, a.spin_limit_ns);   // the count word overtook the entry: it is on its way
 }
 __device__ __forceinline__ void xq_drain(const LoopArgs &a, uint32_t round, uint32_t *s_pref, uint32_t *s_scan /* 33 words */,
                                          uint32_t *s_occ_add) {
@@ -1038,15 +1056,8 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
     {
       unsigned long long t0 = 0;
       for (unsigned j = threadIdx.x; j < gridDim.x; j += blockDim.x)
-        for (uint32_t spin = 0; ld_acquire(a.frontbuf + (size_t)j * 16, false) != (unsigned long long)fseq; spin++) {
-#ifdef YT_SIMT_EMU
-          emu::yield();
-#endif
-          if ((spin & 4095u) == 4095u) {
-            if (!t0) t0 = gtimer();
-            else if (gtimer() - t0 > a.spin_limit_ns) loop_trap();
-          }
-        }
+        for (uint32_t spin = 0; ld_acquire(a.frontbuf + (size_t)j * 16, false) != (unsigned long long)fseq; spin++)
+          spin_step(spin, t0, a.spin_limit_ns);
     }
     __syncthreads();
     Best bd{0, 0, 0};   // the bound: the last pair of every list that is full (a shorter list holds its whole partition)
@@ -1160,8 +1171,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
           const uint32_t j = t % 31;
           if (j == 0) batch = load_batch(t);
           uint2 d0, d1;
-          d0.x = __shfl_sync(0xffffffffu, batch.x, j);     d0.y = __shfl_sync(0xffffffffu, batch.y, j);
-          d1.x = __shfl_sync(0xffffffffu, batch.x, j + 1); d1.y = __shfl_sync(0xffffffffu, batch.y, j + 1);
+          tile_pair(batch, j, d0, d1);
           if (!staged(d0, d1)) continue;
           if (lane == 0) {
             if ((used >> st) & 1u) mbar_wait(&s_empty[st], (ephase >> st) & 1u);
@@ -1185,8 +1195,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
           const uint32_t j = t % 31;
           if (j == 0) batch = load_batch(t);
           uint2 d0, d1;
-          d0.x = __shfl_sync(0xffffffffu, batch.x, j);     d0.y = __shfl_sync(0xffffffffu, batch.y, j);
-          d1.x = __shfl_sync(0xffffffffu, batch.x, j + 1); d1.y = __shfl_sync(0xffffffffu, batch.y, j + 1);
+          tile_pair(batch, j, d0, d1);
           if (d1.x <= d0.x) continue;
           if (!staged(d0, d1)) { if (cw == 0 && lane == 0) s_direct = 1; continue; }  // oversized: direct pass below
           mbar_wait(&s_full[st], (fphase >> st) & 1u);
@@ -1197,11 +1206,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
           const uint32_t *of = stg + a.stream_tok_cap + (d0.x - win_lo(d0.x));
           const uint32_t span = d1.y - d0.y, nw = d1.x - d0.x, obase = d0.y;
           auto report = [&](uint32_t i) {  // token i of the tile starts an (x,y) occurrence
-            uint32_t lo = 0, hi = nw;      // largest w with of[w] - obase <= i
-            while (hi - lo > 1) {
-              const uint32_t mid = (lo + hi) >> 1;
-              if (of[mid] - obase <= i) lo = mid; else hi = mid;
-            }
+            const uint32_t lo = word_at(of, nw, i, obase);
             const uint32_t o = of[lo] - obase, wcap = of[lo + 1] - obase - o;
             for (uint32_t q2 = o; q2 < i; q2++)  // only the first hit of a word reports it
               if (tk[q2] == op.x && tk[q2 + 1] == op.y) return;
@@ -1221,10 +1226,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
             if (p + 4 < total) u = *reinterpret_cast<const uint4 *>(stg + p + 4);
             uint32_t nxt = __shfl_down_sync(0xffffffffu, v.x, 1);
             if (lane == 31) nxt = p + 8 < total ? stg[p + 8] : ~0u;
-            uint32_t m = (v.x == op.x && v.y == op.y ? 1u : 0u) | (v.y == op.x && v.z == op.y ? 2u : 0u) |
-                         (v.z == op.x && v.w == op.y ? 4u : 0u) | (v.w == op.x && u.x == op.y ? 8u : 0u) |
-                         (u.x == op.x && u.y == op.y ? 16u : 0u) | (u.y == op.x && u.z == op.y ? 32u : 0u) |
-                         (u.z == op.x && u.w == op.y ? 64u : 0u) | (u.w == op.x && nxt == op.y ? 128u : 0u);
+            uint32_t m = match8(v, u, nxt, op);
             if (!__ballot_sync(0xffffffffu, m)) continue;
             while (m) {
               const uint32_t pk = p + (uint32_t)__ffs(m) - 1u;
@@ -1294,15 +1296,6 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
       const uint32_t nseg = a.xq.world * a.xq.nblocks, parity = round & 1u, stamp = round % XQ_STAMP_MOD;
       uint32_t flags = 0, big = 0;
       unsigned long long t0 = 0;
-      auto spin_check = [&](uint32_t spin) {   // a peer that stays silent traps the kernel (never hang the box)
-#ifdef YT_SIMT_EMU
-        emu::yield();
-#endif
-        if ((spin & 4095u) == 4095u) {
-          if (!t0) t0 = gtimer();
-          else if (gtimer() - t0 > a.spin_limit_ns) loop_trap();
-        }
-      };
       // One work item per (place e, segment j), numbered place-major: item = e * nseg + j.  The thread of an item polls
       // the count word of segment j in this block's row and loads place e of that segment from the matrix — consecutive
       // lanes touch consecutive words / slots, and the entries of a round spread over the whole block.  No barrier between
@@ -1333,7 +1326,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
             if (ie[k] == ~0u) continue;
             const uint32_t e = ie[k], j = ij[k];
             for (uint32_t spin = 0; (uint32_t)(hv[k] >> 32) != round; spin++) {
-              spin_check(spin);
+              spin_step(spin, t0, a.spin_limit_ns);
               hv[k] = ld_relaxed_any(wp[k], sys);
               if (k == 0) ld_relaxed2(ep[0], &e0, &e1, sys);
             }
@@ -1341,10 +1334,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
             uint32_t n = c & XQ_CNT_MASK;
             if (n > a.xq.seg_cap) n = a.xq.seg_cap;
             if (e == 0) {   // the place-0 thread speaks for the segment
-              if (c & XQ_CNT_OVF) flags |= XQF_OVERFLOW;
-              if (c & XQ_CNT_COMPACT) flags |= XQF_COMPACT;
-              if (c & XQ_CNT_PLIMIT) flags |= XQF_PLIMIT;
-              if (c & XQ_CNT_PFULL) flags |= XQF_PFULL;
+              cnt_flags(flags, c, false);
               const uint32_t nb = n < a.drain_places ? n : a.drain_places;
               s_pref[j] = n - nb;   // the rest: the shared walk below (place matrix up to XQ_BOX, then the sender's segment)
               if (n > nb) big = 1;
@@ -1354,7 +1344,7 @@ __global__ void __launch_bounds__(512, 1) merge_loop_kernel(LoopArgs a) {
             unsigned long long key = 0;
             long long delta = 0;
             for (uint32_t spin = 0; !xq_unpack(e0, e1, stamp, &key, &delta); spin++) {   // the count word overtook the entry
-              spin_check(spin);
+              spin_step(spin, t0, a.spin_limit_ns);
               ld_relaxed2(ep[k], &e0, &e1, sys);
             }
             front_take(fx, key, delta);

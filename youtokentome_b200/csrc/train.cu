@@ -547,18 +547,21 @@ PairTab tab_of(yttm_ctx *c) {
 // Default 50 / 25: since round 2 a block sweeps only its own partition, so a roomier table costs little and keeps the
 // probe chains of the owners' updates short.  YTTM_PAIR_MAX_LOAD_PCT = 30..90 is an A/B knob.
 static uint64_t pair_max_load_pct() {
-  if (const char *e = std::getenv("YTTM_PAIR_MAX_LOAD_PCT")) return (uint64_t)std::min(90, std::max(30, std::atoi(e)));
-  return 50;
+  return (uint64_t)ytc::env_int("YTTM_PAIR_MAX_LOAD_PCT", 50, 30, 90);
 }
 // smallest pair table; YTTM_PAIR_CAP_FLOOR lowers it so that tests reach the rebuild / overflow paths on tiny inputs
+// (pair_cap_floor_knob: its value, 0 when unset)
+static int pair_cap_floor_knob() { return ytc::env_int("YTTM_PAIR_CAP_FLOOR", 0, 16, INT_MAX); }
 static uint64_t pair_cap_floor() {
-  if (const char *e = std::getenv("YTTM_PAIR_CAP_FLOOR")) return ytc::pow2ceil((uint64_t)std::max(16, std::atoi(e)));
-  return 1u << 16;
+  const int v = pair_cap_floor_knob();
+  return v ? ytc::pow2ceil((uint64_t)v) : 1u << 16;
 }
 
 // Launch geometry of the cooperative merge loop: one block per SM, all co-resident, with (almost) all of the SM's
 // shared memory as the tile buffer.  Fixed per context before the first table is built, because the pair table has one
 // partition per block.
+// The knobs that shape that geometry, read once per context (yttm_geometry_knobs lists them)
+constexpr const char *KNOB_STAGES = "YTTM_STAGES", *KNOB_LOOP_THREADS = "YTTM_LOOP_THREADS";
 constexpr int LOOP_SMEM_HEAD = (XQ_MAX_WORLD * XQ_MAX_BLOCKS + 4) * 4 + 2 * CLAIM_WORDS * 4 + (int)LOOP_FRONT_BYTES;  // segment prefix + claim bitmaps + front
 int ensure_loop_geometry(yttm_ctx *c) {
   if (c->loop_blocks) return 0;
@@ -575,8 +578,8 @@ int ensure_loop_geometry(yttm_ctx *c) {
   // STREAMING: n_stage stages; a stage holds a window of q slots plus the overhang of its last
   // word (words of up to q/4 slots stay on the shared-memory path) and at most q/2 + 1 offsets
   {
-    int n_stage = 2;  // H100: 2, 3 and 4 stages scan within 1.5 % of each other (tools/probe_scan.py, YTTM_STAGES)
-    if (const char *e = std::getenv("YTTM_STAGES")) n_stage = std::max(2, std::min(MAX_STAGES, std::atoi(e)));
+    // H100: 2, 3 and 4 stages scan within 1.5 % of each other (tools/probe_scan.py, YTTM_STAGES)
+    const int n_stage = ytc::env_int(KNOB_STAGES, 2, 2, MAX_STAGES);
     const uint32_t per_stage = (uint32_t)(tile_bytes / n_stage / 4) & ~3u;  // uint32 per stage
     // tokens: q + q/4 + 8, offsets: q/2 + 16  ->  q * 1.75 + 24 <= per_stage
     uint32_t q = (uint32_t)((per_stage - 24) / 1.75);
@@ -587,9 +590,10 @@ int ensure_loop_geometry(yttm_ctx *c) {
     c->loop_stream_tok_cap = (per_stage - c->loop_stream_word_cap) & ~3u;
   }
   YT_CUDA(c, cudaFuncSetAttribute(merge_loop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
-  int threads = 512, per_sm = 0;   // H100, 100 MB Zipf: 8.1 us per merge with 512 threads (128 registers), 11.3 with 1024 (64, spills)
+  // H100, 100 MB Zipf: 8.1 us per merge with 512 threads (128 registers), 11.3 with 1024 (64, spills)
   // tests: smaller blocks change how the scans and the drain split their work (512 at most: the kernel's launch bounds)
-  if (const char *e = std::getenv("YTTM_LOOP_THREADS")) threads = std::max(64, std::min(512, std::atoi(e) / 32 * 32));
+  const int threads = ytc::env_int(KNOB_LOOP_THREADS, 512, 64, 512) / 32 * 32;
+  int per_sm = 0;
   YT_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, merge_loop_kernel, threads, dyn));
   if (per_sm < 1) YT_FAIL(c, "merge_loop_kernel does not fit on an SM");
   c->loop_threads = threads;
@@ -605,8 +609,7 @@ int ensure_loop_geometry(yttm_ctx *c) {
 // the table is rebuilt from them, so the capacity is a performance knob, not a limit.
 int xq_alloc(yttm_ctx *c, uint32_t me, uint32_t world) {
   if (ensure_loop_geometry(c)) return 1;
-  uint32_t seg_cap = 8192;
-  if (const char *e = std::getenv("YTTM_XQ_SEG_CAP")) seg_cap = (uint32_t)std::max(4, std::atoi(e));
+  const uint32_t seg_cap = (uint32_t)ytc::env_int("YTTM_XQ_SEG_CAP", 8192, 4, INT_MAX);
   c->xq_world = world; c->xq_me = me; c->xq_seg_cap = seg_cap; c->xq_nblocks = (uint32_t)c->loop_blocks;
   c->xq_per_sender = (sizeof(XqHdr) + (uint64_t)c->xq_nblocks * seg_cap * sizeof(uint4) + 255) / 256 * 256;
   c->xq_bytes = 2ull * world * c->xq_per_sender;
@@ -624,8 +627,7 @@ int xq_alloc(yttm_ctx *c, uint32_t me, uint32_t world) {
   return 0;
 }
 static unsigned long long xq_spin_limit_ns() {
-  if (const char *e = std::getenv("YTTM_XQ_TIMEOUT_MS")) return (unsigned long long)std::max(1, std::atoi(e)) * 1000000ull;
-  return 30ull * 1000000000ull;
+  return (unsigned long long)ytc::env_int("YTTM_XQ_TIMEOUT_MS", 30000, 1, INT_MAX) * 1000000ull;
 }
 int xq_args(yttm_ctx *c, LoopArgs *a) {
   if (!c->xq_buf.p && xq_alloc(c, 0, 1)) return 1;
@@ -787,9 +789,8 @@ int plan_tiles(yttm_ctx *c, LoopArgs *a) {
   if (c->n_words == 0 || c->n_slots == 0) return 0;
   YT_CUDA(c, c->counters.reserve(64));
   uint32_t *d_stats = reinterpret_cast<uint32_t *>(c->counters.as<unsigned long long>() + 7);
-  const bool force_stream = std::getenv("YTTM_FORCE_STREAM") != nullptr;
-  uint32_t stream_q = c->loop_stream_q;
-  if (const char *e = std::getenv("YTTM_STREAM_Q")) stream_q = (uint32_t)std::max(1, std::atoi(e));
+  const bool force_stream = ytc::env_set("YTTM_FORCE_STREAM");
+  const uint32_t stream_q = (uint32_t)ytc::env_int("YTTM_STREAM_Q", (int)c->loop_stream_q, 1, INT_MAX);
   for (int pass = force_stream ? 1 : 0; pass < 2; pass++) {
     uint64_t q = pass == 0 ? (c->n_slots + c->loop_blocks - 1) / c->loop_blocks : stream_q;
     if (q == 0) q = 1;
@@ -802,8 +803,8 @@ int plan_tiles(yttm_ctx *c, LoopArgs *a) {
     a->tile_desc = c->tiles.as<uint2>();
     a->n_tiles = (uint32_t)n_tiles;
     if (pass == 1) {
-      a->defer_cap = 8192;  // words per block and merge on the deferred path; beyond it the direct pass takes over
-      if (const char *e = std::getenv("YTTM_DEFER_CAP")) a->defer_cap = (uint32_t)std::max(1, std::atoi(e));
+      // words per block and merge on the deferred path; beyond it the direct pass takes over
+      a->defer_cap = (uint32_t)ytc::env_int("YTTM_DEFER_CAP", 8192, 1, INT_MAX);
       YT_CUDA(c, c->defer.reserve((size_t)c->loop_blocks * a->defer_cap * sizeof(uint4)));
       a->defer = c->defer.as<uint4>();
       break;
@@ -833,6 +834,8 @@ int plan_tiles(yttm_ctx *c, LoopArgs *a) {
 }
 
 }  // namespace
+
+const char *const yttm_geometry_knobs[] = {KNOB_STAGES, KNOB_LOOP_THREADS, "YT_EMU_SMS", nullptr};
 
 thread_local std::string g_yttm_create_error;
 
@@ -921,8 +924,7 @@ static int pipelined_load(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n
     YT_CUDA(c, cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
     YT_CUDA(c, cudaEventCreateWithFlags(&c->ev_pipe, cudaEventDisableTiming));
   }
-  uint64_t piece = 32ull << 20;
-  if (const char *e = std::getenv("YTTM_TRAIN_PIPELINE_PIECE_KB")) piece = (uint64_t)std::max(1, std::atoi(e)) << 10;   // tests
+  const uint64_t piece = (uint64_t)ytc::env_int("YTTM_TRAIN_PIPELINE_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;   // tests: small pieces
   YT_CUDA(c, c->hist.reserve((CP_LIMIT + 1) * 8));
   YT_CUDA(c, cudaMemsetAsync(c->hist.p, 0, (CP_LIMIT + 1) * 8, c->stream));
   YT_CUDA(c, c->counters.reserve(64));
@@ -975,8 +977,9 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
   c->text_external = false;
   c->pipe_hist = false;
   c->pipe_wtab_cap = 0;
-  uint64_t pipe_min = 64ull << 20;   // below this the passes are too short to be worth a second stream
-  if (const char *e = std::getenv("YTTM_TRAIN_PIPELINE")) pipe_min = std::atoi(e) > 0 ? (uint64_t)std::atoi(e) : ~0ull;   // bytes; 0 = off
+  // bytes; below 64 MB the passes are too short to be worth a second stream; YTTM_TRAIN_PIPELINE=0: off
+  const int pipe_knob = ytc::env_int("YTTM_TRAIN_PIPELINE", 64 << 20, 0, INT_MAX);
+  const uint64_t pipe_min = pipe_knob > 0 ? (uint64_t)pipe_knob : ~0ull;
   if (n >= pipe_min) { if (pipelined_load(c, base + 16, bytes, n)) return 1; }
   else if (n) YT_CUDA(c, cudaMemcpyAsync(base + 16, bytes, n, cudaMemcpyHostToDevice, c->stream));
   ytc::timer_end(c, "h2d");
@@ -1057,7 +1060,7 @@ static int finish_build(yttm_ctx *c, yttm_train_stats *stats) {
   // the table is accepted at load <= 1/4).  Starting at the floor and doubling cost five histogram passes on the
   // multilingual corpus (60 ms per GB); a partition is only swept by the rare refreshes of the front, so a roomy table
   // costs nothing per merge.  (YTTM_PAIR_CAP_FLOOR still forces small tables in the tests.)
-  const uint64_t guess = std::getenv("YTTM_PAIR_CAP_FLOOR") ? 0 : c->n_slots / 2;
+  const uint64_t guess = pair_cap_floor_knob() ? 0 : c->n_slots / 2;
   int rc = rebuild_pair_table(c, std::max<uint64_t>(pair_cap_floor(), guess));
   ytc::timer_end(c, "pair_hist");
   if (rc) return rc;
@@ -1487,15 +1490,13 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
     a.max_total = max_merges;
     a.max_iters = max_merges;
     a.part_limit = (uint32_t)(((uint64_t)c->p_rmask + 1) * pair_max_load_pct() / 100);  // rebuild above this partition load (default 1/2)
-    a.front_top = 4;   // smaller front: shorter probes and scans, but more refreshes (A/B: YTTM_FRONT_TOP)
-    if (const char *e = std::getenv("YTTM_FRONT_TOP")) a.front_top = (uint32_t)std::max(1, std::min((int)FRONT_TOP, std::atoi(e)));
+    a.front_top = (uint32_t)ytc::env_int("YTTM_FRONT_TOP", 4, 1, FRONT_TOP);   // smaller front: shorter probes and scans, but more refreshes
     {  // as many places per segment as ONE trip of the drain's items holds (1 GPU: all 7; 8 GPUs: 1)
       const uint32_t nseg = c->xq_world * c->xq_nblocks;
-      a.drain_places = std::max<uint32_t>(1, std::min<uint32_t>(XQ_BOX, (uint32_t)DRAIN_ITEMS * (uint32_t)c->loop_threads / std::max<uint32_t>(nseg, 1)));
-      if (const char *e = std::getenv("YTTM_DRAIN_PLACES")) a.drain_places = (uint32_t)std::max(1, std::min((int)XQ_BOX, std::atoi(e)));
+      const uint32_t places = std::max<uint32_t>(1, std::min<uint32_t>(XQ_BOX, (uint32_t)DRAIN_ITEMS * (uint32_t)c->loop_threads / std::max<uint32_t>(nseg, 1)));
+      a.drain_places = (uint32_t)ytc::env_int("YTTM_DRAIN_PLACES", (int)places, 1, XQ_BOX);
     }
-    a.newp_limit = NEWP_LIMIT;
-    if (const char *e = std::getenv("YTTM_NEWP_LIMIT")) a.newp_limit = (uint32_t)std::max(1, std::min((int)NEWP_LIMIT, std::atoi(e)));
+    a.newp_limit = (uint32_t)ytc::env_int("YTTM_NEWP_LIMIT", (int)NEWP_LIMIT, 1, (int)NEWP_LIMIT);
     a.dead_min_slots = 4096;
     YT_CUDA(c, cudaMemsetAsync(c->frontbuf.p, 0, front_buf_words((uint32_t)c->loop_blocks) * 8, c->stream));  // refresh numbers restart at 1
 #ifndef YT_SIMT_EMU
