@@ -100,11 +100,14 @@ struct TrainReport {
   double read_s = 0, h2d_ms = 0, char_hist_ms = 0, word_count_ms = 0, tokenise_ms = 0, pair_hist_ms = 0,
          merge_loop_ms = 0, total_s = 0;
   uint64_t launches = 0;
+  uint64_t loop_launches = 0;   // launches of the merge loop (more than one: a compaction or a table rebuild ran)
 };
 const TrainReport &last_train_report();
 // train_bpe keeps one training context (device buffers of the corpus, word table, packed words, pair table) per host
 // thread between calls; this frees the calling thread's.
 void release_training_cache();
+// Training contexts currently cached by all host threads of the process (0 unless YTTM_TRAIN_KEEP_CACHE is set).
+int training_cache_held();
 
 // bpe.h:19 — reads input_path, trains on the GPU, writes the model file.
 Status train_bpe(const std::string &input_path, const std::string &model_path, int vocab_size, BpeConfig config);

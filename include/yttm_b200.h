@@ -30,7 +30,10 @@ int yttm_device_count(void);
 
 /* cudaEvent milliseconds of the last call of the named stage ("char_hist", "word_count",
  * "tokenise", "pair_hist", "merge_loop", "encode", "h2d", "d2h", "enc_spans", "enc_subwords", "decode", "dec_count",
- * "dec_scan", "dec_emit", "dec_e2e"); < 0 if unknown. */
+ * "dec_scan", "dec_emit", "dec_e2e"); < 0 if unknown or if the stage did not run in the current training (since the last
+ * yttm_train_load_corpus) or the last encode / decode call.  Counters of the last yttm_train_run under the same name:
+ * "loop_iters", "loop_refreshes", "loop_launches", "loop_resident", "table_capacity", and "xq_round" (exchange rounds
+ * of the merge loop since the context was created or joined a job; they run on across trainings). */
 double yttm_stage_ms(const yttm_ctx *ctx, const char *stage);
 /* number of kernel launches issued by this context so far (bench.py: gpu_launches) */
 uint64_t yttm_launch_count(const yttm_ctx *ctx);
@@ -42,7 +45,9 @@ uint64_t yttm_launch_count(const yttm_ctx *ctx);
  * Replaces fast_read_file_utf8's buffer (bpe.cpp:67-84) as the input of the passes below.
  * Host corpora of >= 64 MB are copied in pieces that end behind an ASCII space / newline; phase 1
  * and the word table of phase 2 run per piece on a second stream behind the copy of the next piece
- * (the calls below then only collect the results; YTTM_TRAIN_PIPELINE=0 turns this off). */
+ * (the calls below then only collect the results; YTTM_TRAIN_PIPELINE=0 turns this off).
+ * A context may train again: this call drops whatever an earlier corpus built (words, pair table), so that export_words,
+ * dump_pairs, scan_once and run fail until yttm_train_build has run on the new corpus. */
 int yttm_train_load_corpus(yttm_ctx *ctx, const char *bytes, uint64_t n, int on_device);
 
 /* Phase 1 — compute_char_count (bpe.cpp:839-857): *data_len = number of decode units (spaces

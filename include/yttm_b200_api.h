@@ -23,6 +23,8 @@ int yttm_api_train_memory(const char *text, uint64_t n, const char *model_path, 
 int yttm_api_train_report(double *out, int n);
 /* frees the device buffers train_bpe keeps cached for the calling thread (vkcom::release_training_cache) */
 void yttm_api_release_training_cache(void);
+/* training contexts currently cached by all threads of the process (vkcom::training_cache_held) */
+int yttm_api_training_cache_held(void);
 
 /* yttm.pyx:58-62 BPE.__init__ -> BaseEncoder(model_path, n_threads, &status) */
 void *yttm_api_open(const char *model_path, int n_threads);

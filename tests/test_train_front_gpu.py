@@ -156,11 +156,14 @@ def _device_buffer(text, off, dev):
     return raw.ctypes.data + off, raw
 
 
-def device_front(L, text, cp2id, off=None, dev=False):
+def device_front(L, text, cp2id, off=None, dev=False, ctx=None):
     """load_corpus (host bytes, or device-resident at base offset `off`), char_hist, set_alphabet, build,
-    export_words, dump_pairs -> the fields of _front_ref.expected_front."""
-    ctx = C.c_void_p()
-    assert L.yttm_ctx_create(0, C.byref(ctx)) == 0
+    export_words, dump_pairs -> the fields of _front_ref.expected_front.  ctx: run on this context (it stays open)
+    instead of a new one."""
+    own = ctx is None
+    if own:
+        ctx = C.c_void_p()
+        assert L.yttm_ctx_create(0, C.byref(ctx)) == 0
     keep = None
     try:
         if off is None:
@@ -197,7 +200,8 @@ def device_front(L, text, cp2id, off=None, dev=False):
                     n_unique=st.n_unique, n_tokens=st.n_tokens, words=words, pairs=pairs, n_pairs=st.n_pairs,
                     table_capacity=st.table_capacity)
     finally:
-        L.yttm_ctx_destroy(ctx)
+        if own:
+            L.yttm_ctx_destroy(ctx)
         del keep
 
 

@@ -15,8 +15,10 @@ def functions(path):
     out = {}
     for p in parts[1:]:
         name, body = p.split("\n", 1)
-        # the anonymous-namespace suffix (_cu_<hash>) depends on the source text, not only on its path
-        out[re.sub(r"_cu_[0-9a-f]{8}", "_cu_", name.strip())] = "\n".join(re.sub(r"\s+", " ", ln).strip() for ln in body.splitlines())
+        # the anonymous-namespace hash (_cu_<hash>, or _GLOBAL__N__<hash>_ in CUDA 12.9) depends on the source text,
+        # not only on its path; "identifier = <source path>" lines name the file, not code
+        name = re.sub(r"_GLOBAL__N__[0-9a-f]{8}_", "_GLOBAL__N__", re.sub(r"_cu_[0-9a-f]{8}", "_cu_", name.strip()))
+        out[name] = "\n".join(re.sub(r"\s+", " ", ln).strip() for ln in body.splitlines() if not ln.strip().startswith("identifier ="))
     return out
 
 

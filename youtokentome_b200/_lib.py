@@ -42,6 +42,7 @@ def bind(L):
         "yttm_api_train_memory": (i32, [cp, u64, cp, i32, dbl, i32, i32, i32, i32]),
         "yttm_api_train_report": (i32, [vp, i32]),
         "yttm_api_release_training_cache": (None, []),
+        "yttm_api_training_cache_held": (i32, []),
         "yttm_api_open": (vp, [cp, i32]),
         "yttm_api_close": (None, [vp]),
         "yttm_api_vocab_size": (i32, [vp]),

@@ -4,6 +4,7 @@
 // config validation, the coverage cut (the only floating point of training), id renaming,
 // model I/O, id <-> subword tables, decode.
 #include <algorithm>
+#include <atomic>
 #include <cassert>
 #include <chrono>
 #include <cmath>
@@ -319,17 +320,33 @@ struct TrainCache {  // deliberately not destroyed at thread / process exit (no 
   std::string geometry;
 };
 static thread_local TrainCache g_train_cache;
+static std::atomic<int> g_train_contexts_held{0};   // cached training contexts of all threads
+
+static void drop_cached_context(TrainCache &cache) {
+  if (!cache.ctx) return;
+  yttm_ctx_destroy(cache.ctx);
+  cache.ctx = nullptr;
+  g_train_contexts_held--;
+}
 
 // Gives the device memory of this thread's cached training context back (the next train_bpe builds a new one).
 void release_training_cache() {
-  if (g_train_cache.ctx) yttm_ctx_destroy(g_train_cache.ctx);
-  g_train_cache.ctx = nullptr;
+  drop_cached_context(g_train_cache);
   g_train_cache.device = -1;
 }
+
+int training_cache_held() { return g_train_contexts_held.load(); }
 
 static Status train_on_buffer(const char *text, uint64_t n, int n_tokens, const std::string &output_file,
                               BpeConfig cfg, BPEState *out_state) {
   double t_start = now_s();
+  // The context holds the corpus, the word table, the packed words and the pair table (more than the corpus itself).
+  // The reference's train_bpe is stateless, so the device memory goes back on every return, errors included;
+  // YTTM_TRAIN_KEEP_CACHE=1 keeps the context for the next training of this thread (benchmarks, test loops),
+  // release_training_cache() frees it.
+  struct ReleaseUnlessKept {
+    ~ReleaseUnlessKept() { if (!std::getenv("YTTM_TRAIN_KEEP_CACHE")) release_training_cache(); }
+  } release_on_return;
   // one training context per host thread and device; with YTTM_TRAIN_KEEP_CACHE=1 it survives the call and its device
   // buffers (corpus, word table, packed words, pair table) are reused by the next training of this thread
   TrainCache &cache = g_train_cache;
@@ -341,12 +358,10 @@ static Status train_on_buffer(const char *text, uint64_t n, int n_tokens, const 
     geometry += v ? v : "";
     geometry += '|';
   }
-  if (cache.ctx && (cache.device != default_device() || cache.geometry != geometry)) {
-    yttm_ctx_destroy(cache.ctx);
-    cache.ctx = nullptr;
-  }
+  if (cache.ctx && (cache.device != default_device() || cache.geometry != geometry)) drop_cached_context(cache);
   if (!cache.ctx) {
     if (yttm_ctx_create(default_device(), &cache.ctx)) { cache.ctx = nullptr; return Status(1, yttm_last_error(nullptr)); }
+    g_train_contexts_held++;
     cache.device = default_device();
     cache.geometry = geometry;
   }
@@ -409,11 +424,8 @@ static Status train_on_buffer(const char *text, uint64_t n, int n_tokens, const 
   r.word_count_ms = yttm_stage_ms(ctx, "word_count"); r.tokenise_ms = yttm_stage_ms(ctx, "tokenise");
   r.pair_hist_ms = yttm_stage_ms(ctx, "pair_hist"); r.merge_loop_ms = yttm_stage_ms(ctx, "merge_loop");
   r.launches = yttm_launch_count(ctx) - launches0;
+  r.loop_launches = (uint64_t)yttm_stage_ms(ctx, "loop_launches");
   r.total_s = now_s() - t_start;
-  // The context holds the corpus, the word table, the packed words and the pair table (more than the corpus itself).
-  // The reference's train_bpe is stateless, so the device memory goes back by default; YTTM_TRAIN_KEEP_CACHE=1 keeps
-  // the context for the next training of this thread (benchmarks, test loops), release_training_cache() frees it.
-  if (!std::getenv("YTTM_TRAIN_KEEP_CACHE")) release_training_cache();
   return Status();
 }
 

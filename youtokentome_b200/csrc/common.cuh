@@ -111,14 +111,17 @@ struct yttm_ctx {
   int loop_blocks = 0, loop_threads = 0;
   double loop_phase_ms[4] = {0, 0, 0, 0};   // YtLoopCtl::t_phase of the last yttm_train_run
   uint64_t loop_iters = 0, loop_relaunches = 0, loop_sweeps = 0;
+  uint32_t loop_xq_round = 0;   // YtLoopCtl::xq_round after the last yttm_train_run
+  double enc_chunks = -1;       // chunks the last host-buffer encode call was cut into (encode.cu)
 
   yttm_train_stats stats{};
 };
 
 extern thread_local std::string g_yttm_create_error;
 
-// The environment knobs that fix a context's launch geometry when it first trains (train.cu; NULL-terminated): a cache
-// of contexts must key on their values.  YT_EMU_SMS is the SM count of the CPU emulation used by the tests.
+// The environment knobs that fix a context's launch geometry and its exchange buffer when it first trains (train.cu;
+// NULL-terminated): a cache of contexts must key on their values.  YT_EMU_SMS is the SM count of the CPU emulation used
+// by the tests.
 extern const char *const yttm_geometry_knobs[];
 
 // exclusive scan of uint64 on the context stream (train.cu); *d_total receives the sum
@@ -162,6 +165,11 @@ inline double timer_ms(yttm_ctx *c, const char *name) {
     t.pending = false;
   }
   return (double)t.ms;
+}
+// Every stage reads -1 (did not run) again: called where a training or an encode / decode call starts, so that a
+// context that is used again never reports a stage time of an earlier call.
+inline void timers_reset(yttm_ctx *c) {
+  for (auto &kv : c->timers) { kv.second.ms = -1.f; kv.second.pending = false; }
 }
 inline uint64_t pow2ceil(uint64_t x) { uint64_t p = 1; while (p < x) p <<= 1; return p; }
 // The library's environment knobs (DESIGN §7.5).  env_int: `dflt` when `name` is unset, else its integer value clamped

@@ -1429,7 +1429,7 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
     cut.push_back(std::min<uint64_t>(hi, n_sent));
   }
   const size_t K = cut.size() - 1;
-  c->timers["enc_chunks"].ms = (float)K;  // yttm_stage_ms(ctx, "enc_chunks"): how many chunks the last call used
+  c->enc_chunks = (double)K;  // yttm_stage_ms(ctx, "enc_chunks"): how many chunks the last host-buffer call used
   auto h2d = [&](size_t i) -> int {  // enqueue the input copies of chunk i on the copy-in stream
     yttm_enc::Slot &sl = e->slot[i & 1];
     const uint64_t lo = cut[i], hi = cut[i + 1], nb = offsets[hi] - offsets[lo];
@@ -1531,6 +1531,7 @@ int yttm_enc_check(yttm_enc *e, const char *who, int bos, int eos) {
   }
   yttm_ctx *c = e->ctx;
   YT_CUDA(c, cudaSetDevice(c->device));
+  ytc::timers_reset(c);   // every encode and decode call starts here: the stage times describe this call alone
   if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
   if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
   return 0;

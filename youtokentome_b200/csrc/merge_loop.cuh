@@ -178,9 +178,9 @@ constexpr uint32_t BB_ID_LIMIT = 1u << 22;
 // consumer an acquire — an entry whose stamps are not the round's has simply not arrived yet (NVLink and L2 deliver an
 // aligned 8-byte word whole; nothing orders different addresses without a fence, and a system-scope fence after peer
 // stores cost microseconds per merge).  w0 = stamp20 | x22 | y22, w1 = stamp20 | value44 (signed).
-// stamp = round % 0xfffff, never 0xfffff: the buffer starts as all-ones.  (A slot left untouched for exactly k * 0xfffff
-// rounds of its parity would carry a matching stamp again; with at most 2^22 merges per job that needs one slot to be
-// idle for half a million merges and then be read in the few hundred nanoseconds before its new content lands.)
+// stamp = round % 0xfffff, never 0xfffff: the buffer starts as all-ones.  (The round counter runs on across the runs and
+// the kept trainings of a context, so stamps do repeat: a slot left untouched for exactly k * 0xfffff rounds of its parity
+// carries a matching stamp again, and is then read wrongly only in the few hundred nanoseconds before its new content lands.)
 constexpr uint32_t XQ_STAMP_MOD = 0xfffffu;
 __device__ __forceinline__ uint4 xq_pack(uint32_t stamp, unsigned long long key, long long value) {
   const unsigned long long st = (unsigned long long)stamp << 44;

@@ -560,8 +560,9 @@ static uint64_t pair_cap_floor() {
 // Launch geometry of the cooperative merge loop: one block per SM, all co-resident, with (almost) all of the SM's
 // shared memory as the tile buffer.  Fixed per context before the first table is built, because the pair table has one
 // partition per block.
-// The knobs that shape that geometry, read once per context (yttm_geometry_knobs lists them)
-constexpr const char *KNOB_STAGES = "YTTM_STAGES", *KNOB_LOOP_THREADS = "YTTM_LOOP_THREADS";
+// The knobs that shape that geometry and the exchange buffer, read once per context (yttm_geometry_knobs lists them)
+constexpr const char *KNOB_STAGES = "YTTM_STAGES", *KNOB_LOOP_THREADS = "YTTM_LOOP_THREADS",
+                     *KNOB_XQ_SEG_CAP = "YTTM_XQ_SEG_CAP";
 constexpr int LOOP_SMEM_HEAD = (XQ_MAX_WORLD * XQ_MAX_BLOCKS + 4) * 4 + 2 * CLAIM_WORDS * 4 + (int)LOOP_FRONT_BYTES;  // segment prefix + claim bitmaps + front
 int ensure_loop_geometry(yttm_ctx *c) {
   if (c->loop_blocks) return 0;
@@ -606,10 +607,11 @@ int ensure_loop_geometry(yttm_ctx *c) {
 
 // Exchange buffer of the merge loop.  Entries per (sender, block) segment: YTTM_XQ_SEG_CAP (tests use tiny values
 // to reach the overflow -> rebuild path); a merge whose count changes do not fit is still applied to the words and
-// the table is rebuilt from them, so the capacity is a performance knob, not a limit.
+// the table is rebuilt from them, so the capacity is a performance knob, not a limit.  It sizes a buffer whose address
+// the other ranks of a job hold from yttm_train_dist_connect on, so it is read once per context, like the geometry.
 int xq_alloc(yttm_ctx *c, uint32_t me, uint32_t world) {
   if (ensure_loop_geometry(c)) return 1;
-  const uint32_t seg_cap = (uint32_t)ytc::env_int("YTTM_XQ_SEG_CAP", 8192, 4, INT_MAX);
+  const uint32_t seg_cap = (uint32_t)ytc::env_int(KNOB_XQ_SEG_CAP, 8192, 4, INT_MAX);
   c->xq_world = world; c->xq_me = me; c->xq_seg_cap = seg_cap; c->xq_nblocks = (uint32_t)c->loop_blocks;
   c->xq_per_sender = (sizeof(XqHdr) + (uint64_t)c->xq_nblocks * seg_cap * sizeof(uint4) + 255) / 256 * 256;
   c->xq_bytes = 2ull * world * c->xq_per_sender;
@@ -835,7 +837,7 @@ int plan_tiles(yttm_ctx *c, LoopArgs *a) {
 
 }  // namespace
 
-const char *const yttm_geometry_knobs[] = {KNOB_STAGES, KNOB_LOOP_THREADS, "YT_EMU_SMS", nullptr};
+const char *const yttm_geometry_knobs[] = {KNOB_STAGES, KNOB_LOOP_THREADS, KNOB_XQ_SEG_CAP, "YT_EMU_SMS", nullptr};
 
 thread_local std::string g_yttm_create_error;
 
@@ -906,6 +908,8 @@ double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
   for (int i = 0; i < 4; i++)
     if (!std::strcmp(stage, ph[i])) return c->loop_phase_ms[i];
   if (!std::strcmp(stage, "loop_iters")) return (double)c->loop_iters;
+  if (!std::strcmp(stage, "xq_round")) return (double)c->loop_xq_round;   // exchange rounds of the context so far
+  if (!std::strcmp(stage, "enc_chunks")) return c->enc_chunks;
   if (!std::strcmp(stage, "loop_refreshes")) return (double)c->loop_sweeps;
   if (!std::strcmp(stage, "loop_launches")) return (double)c->loop_relaunches;
   if (!std::strcmp(stage, "table_capacity")) return (double)c->pcap;
@@ -961,8 +965,16 @@ static int pipelined_load(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n
 int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_device) {
   YT_CUDA(c, cudaSetDevice(c->device));
   if (n >= POS_MASK) YT_FAIL(c, "corpus shard too large (>= 2^40 bytes)");
+  // a new training starts: nothing built from an earlier corpus (words, pair table, a pipelined histogram or word
+  // table that no char_hist / build consumed) and no stage time of an earlier training may pass for this one's
   c->n_text = n;
   c->have_alphabet = false;
+  c->pipe_hist = false;
+  c->pipe_wtab_cap = 0;
+  c->n_words = c->n_slots = c->n_unique = c->n_word_occ = 0;
+  c->pcap = 0;
+  c->stats = yttm_train_stats{};
+  ytc::timers_reset(c);
   if (on_device) {
     c->d_text = reinterpret_cast<const uint8_t *>(bytes);
     c->text_external = true;
@@ -975,8 +987,6 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
   YT_CUDA(c, cudaMemsetAsync(base + 16 + n, ' ', 32, c->stream));
   c->d_text = base + 16;
   c->text_external = false;
-  c->pipe_hist = false;
-  c->pipe_wtab_cap = 0;
   // bytes; below 64 MB the passes are too short to be worth a second stream; YTTM_TRAIN_PIPELINE=0: off
   const int pipe_knob = ytc::env_int("YTTM_TRAIN_PIPELINE", 64 << 20, 0, INT_MAX);
   const uint64_t pipe_min = pipe_knob > 0 ? (uint64_t)pipe_knob : ~0ull;
@@ -1332,6 +1342,7 @@ int yttm_train_dist_import_words(yttm_ctx *c, const void *d_bytes, const uint64_
 int yttm_train_export_words(yttm_ctx *c, uint32_t *tokens, uint64_t tokens_cap, uint32_t *offsets, uint64_t *freq,
                             uint64_t words_cap, uint64_t *n_words, uint64_t *n_tokens) {
   YT_CUDA(c, cudaSetDevice(c->device));
+  if (!c->pcap) YT_FAIL(c, "yttm_train_export_words: yttm_train_build has not run");
   *n_words = c->n_words;
   *n_tokens = c->n_slots;
   if (!tokens) return 0;  // size query
@@ -1388,7 +1399,7 @@ int yttm_train_synth_words(yttm_ctx *c, uint64_t n_words, uint32_t len, uint32_t
 
 int yttm_train_scan_once(yttm_ctx *c, double *ms, uint64_t *algo_bytes) {
   YT_CUDA(c, cudaSetDevice(c->device));
-  if (!c->pcap) YT_FAIL(c, "scan_once: nothing built");
+  if (!c->pcap) YT_FAIL(c, "yttm_train_scan_once: yttm_train_build has not run");
   uint64_t cap = c->pcap;
   YT_CUDA(c, c->scratch_key.reserve(cap * 8));
   YT_CUDA(c, c->scratch_cnt.reserve(cap * 8));
@@ -1416,7 +1427,8 @@ int yttm_train_scan_once(yttm_ctx *c, double *ms, uint64_t *algo_bytes) {
 
 int yttm_train_dump_pairs(yttm_ctx *c, uint64_t *keys, uint64_t *counts, uint64_t cap, uint64_t *n) {
   YT_CUDA(c, cudaSetDevice(c->device));
-  if (!c->pcap) { *n = 0; return 0; }
+  *n = 0;
+  if (!c->pcap) YT_FAIL(c, "yttm_train_dump_pairs: yttm_train_build has not run");
   ytc::DevBuf dk, dc;
   YT_CUDA(c, dk.reserve((cap + 1) * 8));
   YT_CUDA(c, dc.reserve((cap + 1) * 8));
@@ -1445,6 +1457,7 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
   YT_CUDA(c, cudaSetDevice(c->device));
   if (!c->pcap) YT_FAIL(c, "yttm_train_run: yttm_train_build has not run");
   *n_done_out = 0;
+  c->loop_relaunches = 0;
   if (max_merges == 0) return 0;
   if (ensure_loop_geometry(c)) return 1;
   YT_CUDA(c, c->frontbuf.reserve(front_buf_words((uint32_t)c->loop_blocks) * 8));  // gather buffer of the front refreshes
@@ -1458,7 +1471,6 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
   h.n_done = 0; h.stop = 0; h.stop_why = 0; h.iters = 0; h.n_sweeps = 0;
   for (int i = 0; i < 4; i++) h.t_phase[i] = 0;
   YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
-  c->loop_relaunches = 0;
   // compact the words and rebuild the table from them: the counts are stale (reason & 2: lost count changes), a
   // partition ran full (reason & 4: grow) or is over the load limit (reason & 1)
   auto rebuild = [&](uint32_t reason) -> int {
@@ -1538,6 +1550,7 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
   for (int i = 0; i < 4; i++) c->loop_phase_ms[i] = (double)h.t_phase[i] * 1e-6;
   c->loop_iters = h.iters;
   c->loop_sweeps = h.n_sweeps;
+  c->loop_xq_round = h.xq_round;
   *n_done_out = h.n_done;
   if (h.n_done) {
     YT_CUDA(c, cudaMemcpyAsync(rules_xyz, c->d_rules.p, (size_t)h.n_done * 12, cudaMemcpyDeviceToHost, c->stream));
