@@ -101,6 +101,8 @@ struct TrainReport {
          merge_loop_ms = 0, total_s = 0;
   uint64_t launches = 0;
   uint64_t loop_launches = 0;   // launches of the merge loop (more than one: a compaction or a table rebuild ran)
+  uint64_t feed_pieces = 0;     // pieces of a fed corpus (0: it was loaded whole)
+  uint64_t device_peak_bytes = 0;   // largest sum of the training context's device buffers
 };
 const TrainReport &last_train_report();
 // train_bpe keeps one training context (device buffers of the corpus, word table, packed words, pair table) per host

@@ -33,7 +33,9 @@ int yttm_device_count(void);
  * "dec_scan", "dec_emit", "dec_e2e"); < 0 if unknown or if the stage did not run in the current training (since the last
  * yttm_train_load_corpus) or the last encode / decode call.  Counters of the last yttm_train_run under the same name:
  * "loop_iters", "loop_refreshes", "loop_launches", "loop_resident", "table_capacity", and "xq_round" (exchange rounds
- * of the merge loop since the context was created or joined a job; they run on across trainings). */
+ * of the merge loop since the context was created or joined a job; they run on across trainings).  Counters of the
+ * current training: "feed_pieces" (pieces of a fed corpus, 0 after load_corpus) and "dev_peak_bytes" (the largest sum
+ * of the context's device buffers, sampled after every fed piece and every phase). */
 double yttm_stage_ms(const yttm_ctx *ctx, const char *stage);
 /* number of kernel launches issued by this context so far (bench.py: gpu_launches) */
 uint64_t yttm_launch_count(const yttm_ctx *ctx);
@@ -49,6 +51,19 @@ uint64_t yttm_launch_count(const yttm_ctx *ctx);
  * A context may train again: this call drops whatever an earlier corpus built (words, pair table), so that export_words,
  * dump_pairs, scan_once and run fail until yttm_train_build has run on the new corpus. */
 int yttm_train_load_corpus(yttm_ctx *ctx, const char *bytes, uint64_t n, int on_device);
+
+/* Phase 0 for corpora larger than the device's memory: the text is FED in host blocks of any size and boundaries
+ * (mid-word and mid-UTF-8 sequence included) between feed_begin and feed_end, instead of one load_corpus.  The library
+ * cuts the text into pieces behind a whitespace byte (space, \t .. \r), runs phase 1 and the word split per piece,
+ * and merges each piece's distinct words into one device table whose bytes live in a word arena; the corpus itself is
+ * never resident.  feed_begin starts a new training like load_corpus; feed copies the caller's bytes before it
+ * returns; feed_end returns what yttm_train_char_hist returns, and the arena of unique words becomes the context's
+ * text.  char_hist, set_alphabet and build then keep their meaning (build takes the fed words as they are), and so do
+ * export_words, dump_pairs, scan_once, run and yttm_train_dist_export_words.  YTTM_TRAIN_FEED_PIECE_KB sets the piece
+ * size (read by feed_begin).  feed before feed_begin, and char_hist or build between feed_begin and feed_end, fail. */
+int yttm_train_feed_begin(yttm_ctx *ctx);
+int yttm_train_feed(yttm_ctx *ctx, const char *bytes, uint64_t n);
+int yttm_train_feed_end(yttm_ctx *ctx, uint64_t *data_len, uint64_t *n_distinct);
 
 /* Phase 1 — compute_char_count (bpe.cpp:839-857): *data_len = number of decode units (spaces
  * and invalid bytes included); histogram of valid non-space code points.  *n_distinct = number

@@ -1,5 +1,6 @@
 """Fuzz the kernels under the SIMT emulator (tests/emul/simt; TEST HARNESS ONLY): random corpora x random
-geometry (blocks, STREAMING window, ring depth, pair-table floor, deferred-list capacity) against the oracle.
+geometry (blocks, STREAMING window, ring depth, pair-table floor, deferred-list capacity, fed corpora in small pieces)
+against the oracle.
 usage: python tools/fuzz_emul.py [n_cases] [first_seed]"""
 import os
 import sys
@@ -18,7 +19,8 @@ from youtokentome_b200 import synth  # noqa: E402
 
 KNOBS = ["YT_EMU_SMS", "YT_EMU_SCHED_SEED", "YTTM_FORCE_STREAM", "YTTM_STREAM_Q", "YTTM_STAGES", "YTTM_PAIR_CAP_FLOOR", "YTTM_DEFER_CAP",
          "YTTM_ENC_CHUNK_MB", "YTTM_ENC_DEDUP_SLOTS", "YTTM_ENC_DEDUP_WEAKTAG", "YTTM_XQ_SEG_CAP",
-         "YTTM_PAIR_MAX_LOAD_PCT", "YTTM_FRONT_TOP", "YTTM_NEWP_LIMIT", "YTTM_DRAIN_PLACES", "YTTM_TRAIN_PIPELINE", "YTTM_TRAIN_PIPELINE_PIECE_KB", "YTTM_LOOP_THREADS"]
+         "YTTM_PAIR_MAX_LOAD_PCT", "YTTM_FRONT_TOP", "YTTM_NEWP_LIMIT", "YTTM_DRAIN_PLACES", "YTTM_TRAIN_PIPELINE", "YTTM_TRAIN_PIPELINE_PIECE_KB", "YTTM_LOOP_THREADS",
+         "YTTM_TRAIN_FEED_ABOVE", "YTTM_TRAIN_FEED_PIECE_KB"]
 
 
 def sentences(rng, text):
@@ -136,6 +138,9 @@ def main():
         if rng.integers(0, 3) == 0:
             env["YTTM_TRAIN_PIPELINE"] = "1"
             env["YTTM_TRAIN_PIPELINE_PIECE_KB"] = str(int(rng.choice([1, 3, 16])))
+        if rng.integers(0, 3) == 0:   # a fed corpus: pieces of 1 - 5 KB, merged into the persistent word table
+            env["YTTM_TRAIN_FEED_ABOVE"] = str(int(rng.choice([0, 1000, 10000])))
+            env["YTTM_TRAIN_FEED_PIECE_KB"] = str(int(rng.integers(1, 6)))
         if rng.integers(0, 3) == 0:
             env["YTTM_LOOP_THREADS"] = str(int(rng.choice([64, 128, 256])))
         for k in KNOBS:

@@ -86,6 +86,9 @@ def bind(L):
         "yttm_stage_ms": (dbl, [vp, cp]),
         "yttm_launch_count": (u64, [vp]),
         "yttm_train_load_corpus": (i32, [vp, vp, u64, i32]),
+        "yttm_train_feed_begin": (i32, [vp]),
+        "yttm_train_feed": (i32, [vp, vp, u64]),
+        "yttm_train_feed_end": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),
         "yttm_train_char_hist": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),
         "yttm_train_get_char_hist": (i32, [vp, vp, vp]),
         "yttm_train_char_hist_devptr": (i32, [vp, C.POINTER(vp), C.POINTER(u64)]),
@@ -136,7 +139,8 @@ def bind(L):
 
 EXPORTED_SYMBOLS_DEVICE_ABI = [
     "yttm_ctx_create", "yttm_ctx_destroy", "yttm_last_error", "yttm_device_count", "yttm_stage_ms",
-    "yttm_launch_count", "yttm_train_load_corpus", "yttm_train_char_hist", "yttm_train_get_char_hist",
+    "yttm_launch_count", "yttm_train_load_corpus", "yttm_train_feed_begin", "yttm_train_feed", "yttm_train_feed_end",
+    "yttm_train_char_hist", "yttm_train_get_char_hist",
     "yttm_train_char_hist_devptr", "yttm_train_char_hist_refresh", "yttm_train_set_alphabet", "yttm_train_build",
     "yttm_train_export_words", "yttm_train_import_words", "yttm_train_dist_init", "yttm_train_dist_connect",
     "yttm_train_dist_word_table", "yttm_train_dist_export_words", "yttm_train_dist_import_words", "yttm_train_run", "yttm_train_dump_pairs",

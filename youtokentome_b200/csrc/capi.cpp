@@ -70,7 +70,8 @@ int yttm_api_train_report(double *out, int n) {
   const TrainReport &r = last_train_report();
   double v[] = {(double)r.n_bytes, (double)r.data_len, (double)r.n_words, (double)r.n_unique, (double)r.n_tokens,
                 (double)r.n_pairs, (double)r.n_merges, r.read_s, r.h2d_ms, r.char_hist_ms, r.word_count_ms,
-                r.tokenise_ms, r.pair_hist_ms, r.merge_loop_ms, r.total_s, (double)r.launches, (double)r.loop_launches};
+                r.tokenise_ms, r.pair_hist_ms, r.merge_loop_ms, r.total_s, (double)r.launches, (double)r.loop_launches,
+                (double)r.feed_pieces, (double)r.device_peak_bytes};
   int m = (int)(sizeof(v) / sizeof(v[0]));
   for (int i = 0; i < n && i < m; i++) out[i] = v[i];
   return m;

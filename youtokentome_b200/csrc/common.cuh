@@ -85,6 +85,25 @@ struct yttm_ctx {
   ytc::DevBuf wkey, wcnt, wpos, wfreq, wlen, scan_tmp, counters;
   uint64_t n_word_occ = 0, n_unique = 0;
 
+  // ---- fed corpus (yttm_train_feed_*): pieces cut on the host from two pinned staging buffers, copied on stream2 into
+  // two device piece buffers; each piece's words (per-piece table wkey / wcnt) are merged into the persistent table
+  // fkey / fcnt, whose words' bytes live in the arena (16 pad spaces + words, each followed by one space)
+  bool feeding = false;         // between feed_begin and feed_end
+  bool fed_words = false;       // the text is the arena of a fed corpus; wpos / wfreq / n_unique hold its words
+  uint8_t *feed_stage[2] = {nullptr, nullptr};
+  uint64_t feed_stage_cap[2] = {0, 0};
+  int feed_cur = 0;             // staging buffer being filled
+  uint64_t feed_len = 0;        // its bytes
+  uint64_t feed_nows = 0;       // its first bytes known to hold no whitespace byte
+  int feed_pending = -1;        // a piece copied but not yet processed (its staging / piece buffer index)
+  uint64_t feed_pending_len = 0;
+  uint64_t feed_piece = 0;      // nominal piece size
+  ytc::DevBuf feed_dev[2], fkey, fcnt, arena;
+  cudaEvent_t ev_feed_copied[2] = {nullptr, nullptr}, ev_feed_done[2] = {nullptr, nullptr};
+  uint64_t feed_wcap = 0, feed_fcap = 0, feed_fn = 0;   // per-piece / persistent table slots, persistent words
+  uint64_t arena_len = 0, n_fed = 0, feed_pieces = 0;
+  uint64_t dev_peak = 0;        // largest sum of the DevBuf capacities of the current training
+
   // ---- packed words (double buffered for compaction)
   ytc::DevBuf tok[2], off[2], freq[2];
   int cur = 0;
@@ -127,6 +146,9 @@ extern const char *const yttm_geometry_knobs[];
 // exclusive scan of uint64 on the context stream (train.cu); *d_total receives the sum
 int yttm_device_scan_u64(yttm_ctx *c, const unsigned long long *in, uint64_t n, unsigned long long *out,
                          unsigned long long *d_total);
+
+// whether the host trainings (bpe_host.cpp) feed a corpus of n bytes (UINT64_MAX: unknown) instead of loading it (train.cu)
+bool yttm_train_feed_selected(yttm_ctx *c, uint64_t n);
 
 #define YT_CUDA(ctx, call)                                                                       \
   do {                                                                                           \

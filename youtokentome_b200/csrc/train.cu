@@ -214,15 +214,22 @@ __device__ __forceinline__ bool same_word(const uint8_t *s, uint64_t n, uint64_t
   return a + len == n || space_at(s, a + len, n, &l);
 }
 
+// The word table's hash of the word that starts at byte p: FNV-1a over its bytes, then mixed with its length.  It does
+// not depend on where the word lies, so a word hashes alike in a piece of the corpus and in the word arena.
+__device__ __forceinline__ uint64_t word_hash(const uint8_t *__restrict__ s, uint64_t n, uint64_t p, uint64_t *len_out) {
+  uint64_t h = 0xcbf29ce484222325ull, q = p;
+  uint32_t l;
+  while (q < n && !space_at(s, q, n, &l)) { h = (h ^ s[q]) * 0x100000001b3ull; q++; }
+  *len_out = q - p;
+  return mix64(h ^ ((q - p) << 1));
+}
+
 // insert the word that starts at byte p (weight = its number of occurrences) ; returns false when the table is full
 __device__ __forceinline__ bool word_table_insert(const uint8_t *__restrict__ s, uint64_t n, uint64_t p, const WordTab &wt,
                                                   unsigned long long *counters, uint64_t max_unique,
                                                   unsigned long long weight) {
-  uint64_t h = 0xcbf29ce484222325ull, q = p;
-  uint32_t l;
-  while (q < n && !space_at(s, q, n, &l)) { h = (h ^ s[q]) * 0x100000001b3ull; q++; }
-  uint64_t len = q - p;
-  h = mix64(h ^ (len << 1));
+  uint64_t len;
+  const uint64_t h = word_hash(s, n, p, &len);
   uint64_t tag = h >> 40;
   unsigned long long mine = (tag << 40) | (p + 1);
   uint64_t slot = h & wt.mask;
@@ -314,6 +321,89 @@ __global__ void word_compact_kernel(WordTab wt, unsigned long long *counters, ui
     wpos[idx] = (k & POS_MASK) - 1;
     wfreq[idx] = wt.cnts[i];
   }
+}
+
+// ---- fed corpus: the distinct words of one piece (wpos / wfreq, positions in the piece) into the persistent table,
+// whose keys point into the word arena `a` (alen bytes; every word there is followed by one ' ').  Two passes, so
+// that no thread compares against arena bytes that another thread is still writing:
+//   lookup: a word already in the table adds its count; a new word records len + 1 (its arena bytes) in mlen and is
+//           counted in counters[5];
+//   (the host scans mlen into arena offsets and grows the arena / the table)
+//   insert: a new word copies its bytes + ' ' to the arena and claims an empty slot.  No byte compare: the new words
+//           differ from each other (one per-piece table) and from every word of the table (the lookup pass).
+__global__ void __launch_bounds__(256) word_merge_lookup_kernel(const uint8_t *__restrict__ s, uint64_t n,
+                                                                const uint64_t *__restrict__ wpos,
+                                                                const uint64_t *__restrict__ wfreq, uint64_t n_words,
+                                                                WordTab ft, const uint8_t *__restrict__ a,
+                                                                unsigned long long *__restrict__ mlen,
+                                                                unsigned long long *counters) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_words; i += stride) {
+    const uint64_t p = wpos[i];
+    uint64_t len;
+    const uint64_t h = word_hash(s, n, p, &len), tag = h >> 40;
+    unsigned long long miss = len + 1;
+    for (uint64_t slot = h & ft.mask;; slot = (slot + 1) & ft.mask) {   // the table is at most half full
+      const unsigned long long k = ft.keys[slot];
+      if (k == 0) break;
+      if ((k >> 40) != tag) continue;
+      const uint64_t q = (k & POS_MASK) - 1;
+      uint64_t j = 0;
+      while (j < len && a[q + j] == s[p + j]) j++;   // an arena word is followed by ' ', which no word byte equals
+      if (j == len && a[q + len] == ' ') {
+        atomicAdd(ft.cnts + slot, (unsigned long long)wfreq[i]);
+        miss = 0;
+        break;
+      }
+    }
+    mlen[i] = miss;
+    if (miss) atomicAdd(counters + 5, 1ull);
+  }
+}
+
+__global__ void __launch_bounds__(256) word_merge_insert_kernel(const uint8_t *__restrict__ s, uint64_t n,
+                                                                const uint64_t *__restrict__ wpos,
+                                                                const uint64_t *__restrict__ wfreq, uint64_t n_words,
+                                                                const unsigned long long *__restrict__ mlen,
+                                                                const unsigned long long *__restrict__ moff,
+                                                                WordTab ft, uint8_t *__restrict__ a, uint64_t alen) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_words; i += stride) {
+    if (!mlen[i]) continue;
+    const uint64_t p = wpos[i], at = alen + moff[i];
+    uint64_t len;
+    const uint64_t h = word_hash(s, n, p, &len);
+    for (uint64_t j = 0; j < len; j++) a[at + j] = s[p + j];
+    a[at + len] = ' ';
+    const unsigned long long key = ((h >> 40) << 40) | (at + 1);
+    uint64_t slot = h & ft.mask;
+    while (atomicCAS(ft.keys + slot, 0ull, key) != 0ull) slot = (slot + 1) & ft.mask;
+    ft.cnts[slot] = wfreq[i];
+  }
+}
+
+// The persistent table moved to a larger one (old -> nt): every word is hashed again from its arena bytes.
+__global__ void __launch_bounds__(256) word_table_rehash_kernel(WordTab old, WordTab nt, const uint8_t *__restrict__ a,
+                                                                uint64_t alen) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= old.mask; i += stride) {
+    const unsigned long long k = old.keys[i];
+    if (k == 0) continue;
+    uint64_t len;
+    const uint64_t h = word_hash(a, alen, (k & POS_MASK) - 1, &len);
+    uint64_t slot = h & nt.mask;
+    while (atomicCAS(nt.keys + slot, 0ull, k) != 0ull) slot = (slot + 1) & nt.mask;
+    nt.cnts[slot] = old.cnts[i];
+  }
+}
+
+// freq x tokens of every word below 2^43 (the signed 44-bit count change of the merge loop's exchange entries, as
+// yttm_train_import_words checks): a text shard cannot exceed it, a fed corpus can.  lens: tokens per word.
+__global__ void word_count_limit_kernel(const unsigned long long *__restrict__ lens, const uint64_t *__restrict__ wfreq,
+                                        uint64_t n_words, unsigned long long *bad) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < n_words; w += stride)
+    if (lens[w] && wfreq[w] >= (1ull << 43) / lens[w]) atomicExch(bad, 1ull);
 }
 
 // tokens of one unique word: [space_id] + ids of kept chars; removed / invalid units vanish.
@@ -835,6 +925,22 @@ int plan_tiles(yttm_ctx *c, LoopArgs *a) {
   return 0;
 }
 
+// every device buffer the context owns
+std::vector<ytc::DevBuf *> ctx_bufs(yttm_ctx *c) {
+  return {&c->text_buf, &c->hist, &c->cp2id, &c->wkey, &c->wcnt, &c->wpos, &c->wfreq, &c->wlen, &c->scan_tmp,
+          &c->counters, &c->tok[0], &c->tok[1], &c->off[0], &c->off[1], &c->freq[0], &c->freq[1], &c->pkey, &c->pcnt,
+          &c->scratch_key, &c->scratch_cnt, &c->ctl, &c->frontbuf, &c->tiles, &c->defer, &c->d_rules, &c->d_rfreq,
+          &c->xq_arrive, &c->xq_buf, &c->feed_dev[0], &c->feed_dev[1], &c->fkey, &c->fcnt, &c->arena};
+}
+
+// The device memory high-water mark of the current training ("dev_peak_bytes"): sampled after every phase and every fed
+// piece, it shows whether a corpus sat on the device.
+void note_peak(yttm_ctx *c) {
+  uint64_t sum = 0;
+  for (auto *b : ctx_bufs(c)) sum += b->cap;
+  c->dev_peak = std::max(c->dev_peak, sum);
+}
+
 }  // namespace
 
 const char *const yttm_geometry_knobs[] = {KNOB_STAGES, KNOB_LOOP_THREADS, KNOB_XQ_SEG_CAP, "YT_EMU_SMS", nullptr};
@@ -844,6 +950,22 @@ thread_local std::string g_yttm_create_error;
 int yttm_device_scan_u64(yttm_ctx *c, const unsigned long long *in, uint64_t n, unsigned long long *out,
                          unsigned long long *d_total) {
   return device_scan(c, in, n, out, d_total);
+}
+
+// Whether train_bpe / learn_bpe_from_string feed a corpus of n bytes (UINT64_MAX: size unknown) rather than load it.
+// The in-memory path holds the corpus, a word table of up to two slots of 16 B per 16 corpus bytes (1 GB at most) and
+// the tokens of the unique words at once, so a corpus above a third of the device's free memory at the start of the
+// training is fed (DESIGN §3).  YTTM_TRAIN_FEED_ABOVE (bytes) replaces that threshold.
+bool yttm_train_feed_selected(yttm_ctx *c, uint64_t n) {
+  if (n == UINT64_MAX) return true;
+  if (const char *e = std::getenv("YTTM_TRAIN_FEED_ABOVE")) return n > std::strtoull(e, nullptr, 10);
+#ifndef YT_SIMT_EMU
+  size_t free_b = 0, total_b = 0;
+  if (cudaSetDevice(c->device) != cudaSuccess || cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) return false;
+  return n > free_b / 3;
+#else
+  return false;   // tests/emul/simt: no device memory to ask about; the knob selects
+#endif
 }
 
 // =============================================================================================
@@ -885,14 +1007,16 @@ void yttm_ctx_destroy(yttm_ctx *c) {
   if (!c) return;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  ytc::DevBuf *bufs[] = {&c->text_buf, &c->hist, &c->cp2id, &c->wkey, &c->wcnt, &c->wpos, &c->wfreq, &c->wlen,
-                         &c->scan_tmp, &c->counters, &c->tok[0], &c->tok[1], &c->off[0], &c->off[1], &c->freq[0],
-                         &c->freq[1], &c->pkey, &c->pcnt, &c->scratch_key, &c->scratch_cnt, &c->ctl, &c->frontbuf, &c->tiles, &c->defer,
-                         &c->d_rules, &c->d_rfreq, &c->xq_arrive, &c->xq_buf};
+  if (c->stream2) cudaStreamSynchronize(c->stream2);
   for (int d = 0; d < 8; d++)
     if (c->xq_peer_ipc[d] && c->xq_peer[d]) { cudaIpcCloseMemHandle(c->xq_peer[d]); c->xq_peer[d] = nullptr; }
-  for (auto *b : bufs) b->release();
+  for (auto *b : ctx_bufs(c)) b->release();
   for (auto &kv : c->timers) { if (kv.second.a) cudaEventDestroy(kv.second.a); if (kv.second.b) cudaEventDestroy(kv.second.b); }
+  for (int s = 0; s < 2; s++) {
+    if (c->feed_stage[s]) cudaFreeHost(c->feed_stage[s]);
+    if (c->ev_feed_copied[s]) cudaEventDestroy(c->ev_feed_copied[s]);
+    if (c->ev_feed_done[s]) cudaEventDestroy(c->ev_feed_done[s]);
+  }
   if (c->stream2) cudaStreamDestroy(c->stream2);
   if (c->ev_pipe) cudaEventDestroy(c->ev_pipe);
   cudaStreamDestroy(c->stream);
@@ -914,20 +1038,36 @@ double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
   if (!std::strcmp(stage, "loop_launches")) return (double)c->loop_relaunches;
   if (!std::strcmp(stage, "table_capacity")) return (double)c->pcap;
   if (!std::strcmp(stage, "loop_resident")) return (double)c->loop_resident;
+  if (!std::strcmp(stage, "feed_pieces")) return (double)c->feed_pieces;
+  if (!std::strcmp(stage, "dev_peak_bytes")) return (double)c->dev_peak;
   return ytc::timer_ms(const_cast<yttm_ctx *>(c), stage);
 }
 uint64_t yttm_launch_count(const yttm_ctx *c) { return c->launches; }
 
-// The corpus comes from pageable host memory at ~11 GB/s, and the two byte passes over it (code point histogram, word
-// split + dedup) need neither each other nor the alphabet: the text is copied in pieces that END WITH an ASCII space or
-// newline, and both passes run on a piece (second stream) while the next one is copied.  A piece that ends with a
-// space is self-contained for both: no UTF-8 sequence and no word crosses its end, and what precedes its start is a
-// space (the kernels' view of "outside the text").  Corpora without a space in 32 MB fall back to one piece.
-static int pipelined_load(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n) {
+// Length of the longest prefix of [p, p + n) that ends with a whitespace byte (space, \t .. \r), 0 if there is none.
+// A piece of the corpus cut there is self-contained for both byte passes: no UTF-8 sequence and no word crosses its
+// end (a whitespace byte is a whole unit), and what precedes its start is a space (the kernels' view of "outside the
+// text").
+static uint64_t piece_cut(const char *p, uint64_t n) {
+  for (uint64_t i = n; i > 0; i--)
+    if (is_space_byte((uint8_t)p[i - 1])) return i;
+  return 0;
+}
+
+static int ensure_stream2(yttm_ctx *c) {
   if (!c->stream2) {
     YT_CUDA(c, cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
     YT_CUDA(c, cudaEventCreateWithFlags(&c->ev_pipe, cudaEventDisableTiming));
   }
+  return 0;
+}
+
+// The corpus comes from pageable host memory at ~11 GB/s, and the two byte passes over it (code point histogram, word
+// split + dedup) need neither each other nor the alphabet: the text is copied in pieces (piece_cut), and both passes
+// run on a piece (second stream) while the next one is copied.  Corpora without a whitespace byte in 32 MB fall back
+// to one piece.
+static int pipelined_load(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n) {
+  if (ensure_stream2(c)) return 1;
   const uint64_t piece = (uint64_t)ytc::env_int("YTTM_TRAIN_PIPELINE_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;   // tests: small pieces
   YT_CUDA(c, c->hist.reserve((CP_LIMIT + 1) * 8));
   YT_CUDA(c, cudaMemsetAsync(c->hist.p, 0, (CP_LIMIT + 1) * 8, c->stream));
@@ -942,11 +1082,9 @@ static int pipelined_load(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n
   WordTab wt{c->wkey.as<unsigned long long>(), c->wcnt.as<unsigned long long>(), cap - 1};
   for (uint64_t lo = 0; lo < n;) {
     uint64_t hi = std::min<uint64_t>(n, lo + piece);
-    if (hi < n) {   // end the piece behind its last ASCII space / newline
-      const char *a = static_cast<const char *>(memrchr(src + lo, ' ', hi - lo));
-      const char *b = static_cast<const char *>(memrchr(src + lo, '\n', hi - lo));
-      const char *q = a > b ? a : b;   // (nullptr compares low)
-      hi = q ? (uint64_t)(q - src) + 1 : n;
+    if (hi < n) {
+      const uint64_t cut = piece_cut(src + lo, hi - lo);
+      hi = cut ? lo + cut : n;
     }
     YT_CUDA(c, cudaMemcpyAsync(dst + lo, src + lo, hi - lo, cudaMemcpyHostToDevice, c->stream));
     YT_CUDA(c, cudaEventRecord(c->ev_pipe, c->stream));
@@ -962,6 +1100,9 @@ static int pipelined_load(yttm_ctx *c, uint8_t *dst, const char *src, uint64_t n
   return 0;
 }
 
+static int feed_release(yttm_ctx *c);
+static int hist_summarise(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct);
+
 int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_device) {
   YT_CUDA(c, cudaSetDevice(c->device));
   if (n >= POS_MASK) YT_FAIL(c, "corpus shard too large (>= 2^40 bytes)");
@@ -975,9 +1116,14 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
   c->pcap = 0;
   c->stats = yttm_train_stats{};
   ytc::timers_reset(c);
+  if ((c->feeding || c->arena.p) && feed_release(c)) return 1;   // an abandoned feed
+  c->fed_words = false;
+  c->feed_pieces = 0;
+  c->dev_peak = 0;
   if (on_device) {
     c->d_text = reinterpret_cast<const uint8_t *>(bytes);
     c->text_external = true;
+    note_peak(c);
     return 0;
   }
   ytc::timer_begin(c, "h2d");
@@ -997,7 +1143,254 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
     YT_CUDA(c, cudaEventRecord(c->ev_pipe, c->stream2));
     YT_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_pipe, 0));
   }
+  note_peak(c);
   return 0;
+}
+
+// ---- fed corpus (include/yttm_b200.h: yttm_train_feed_begin / feed / feed_end) ------------------------------------
+// Host side of a piece: bytes gather in staging buffer feed_cur until it holds a nominal piece; the piece then ends
+// behind its last whitespace byte (piece_cut) and what follows moves to the other staging buffer.  A piece is copied
+// on stream2 and processed (feed_process) when the next piece has been cut, so its copy overlaps the passes of the
+// piece before it.
+
+// drops what a feed holds on the device (the feed_end that consumed it or a new training after an abandoned feed)
+static int feed_release(yttm_ctx *c) {
+  if (c->stream2) YT_CUDA(c, cudaStreamSynchronize(c->stream2));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  for (ytc::DevBuf *b : {&c->feed_dev[0], &c->feed_dev[1], &c->fkey, &c->fcnt, &c->arena}) b->release();
+  c->feeding = false;
+  c->fed_words = false;
+  c->feed_pending = -1;
+  return 0;
+}
+
+// staging buffer s holds at least `need` bytes (its first feed_len bytes kept when it is the one being filled)
+static int stage_reserve(yttm_ctx *c, int s, uint64_t need) {
+  if (need <= c->feed_stage_cap[s]) return 0;
+  const uint64_t cap = std::max<uint64_t>({need, 2 * c->feed_stage_cap[s], c->feed_piece});
+  void *p = nullptr;
+  YT_CUDA(c, cudaHostAlloc(&p, cap, cudaHostAllocDefault));
+  if (s == c->feed_cur && c->feed_len) std::memcpy(p, c->feed_stage[s], c->feed_len);
+  if (c->feed_stage[s]) YT_CUDA(c, cudaFreeHost(c->feed_stage[s]));
+  c->feed_stage[s] = static_cast<uint8_t *>(p);
+  c->feed_stage_cap[s] = cap;
+  return 0;
+}
+
+// the arena holds its 16 pad bytes + `need` text bytes + 32 pad bytes; its bytes so far move to a larger buffer
+static int arena_reserve(yttm_ctx *c, uint64_t need) {
+  if (16 + need + 32 <= c->arena.cap) return 0;
+  ytc::DevBuf bigger;
+  YT_CUDA(c, bigger.reserve(std::max<uint64_t>(16 + need + 32, 2 * c->arena.cap)));
+  YT_CUDA(c, cudaMemcpyAsync(bigger.p, c->arena.p, 16 + c->arena_len, cudaMemcpyDeviceToDevice, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->arena.release();
+  c->arena = bigger;
+  return 0;
+}
+
+// the persistent table keeps its load at most 1/2 with `more` further words; a larger table is rehashed from the arena
+static int ftab_reserve(yttm_ctx *c, uint64_t more) {
+  uint64_t cap = c->feed_fcap;
+  while ((c->feed_fn + more) * 2 > cap) cap *= 4;
+  if (cap == c->feed_fcap) return 0;
+  ytc::DevBuf nk, nc;
+  YT_CUDA(c, nk.reserve(cap * 8));
+  YT_CUDA(c, nc.reserve(cap * 8));
+  YT_CUDA(c, cudaMemsetAsync(nk.p, 0, cap * 8, c->stream));
+  YT_CUDA(c, cudaMemsetAsync(nc.p, 0, cap * 8, c->stream));
+  WordTab old{c->fkey.as<unsigned long long>(), c->fcnt.as<unsigned long long>(), c->feed_fcap - 1};
+  WordTab nt{nk.as<unsigned long long>(), nc.as<unsigned long long>(), cap - 1};
+  word_table_rehash_kernel<<<grid_for(c, c->feed_fcap, 256, 8), 256, 0, c->stream>>>(old, nt, c->arena.as<uint8_t>() + 16,
+                                                                                   c->arena_len);
+  c->launches++;
+  YT_CUDA(c, cudaGetLastError());
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->fkey.release(); c->fcnt.release();
+  c->fkey = nk; c->fcnt = nc;
+  c->feed_fcap = cap;
+  return 0;
+}
+
+// Phase 1 and the word split of piece buffer s (m bytes), then its distinct words into the persistent table.
+static int feed_process(yttm_ctx *c, int s, uint64_t m) {
+  const uint8_t *d = c->feed_dev[s].as<uint8_t>();
+  auto *counters = c->counters.as<unsigned long long>();
+  YT_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_feed_copied[s], 0));
+  char_hist_kernel<<<grid_for(c, m / 16 + 1, 512, 4), 512, 0, c->stream>>>(d, m, c->hist.as<unsigned long long>());
+  c->launches++;
+  unsigned long long h[6] = {0, 0, 0, 0, 0, 0};
+  for (int attempt = 0;; attempt++) {   // a piece that overflows the per-piece table is split again in a larger one
+    if (attempt > 10) YT_FAIL(c, "word table: too many retries");
+    const uint64_t cap = c->feed_wcap;
+    YT_CUDA(c, c->wkey.reserve(cap * 8));
+    YT_CUDA(c, c->wcnt.reserve(cap * 8));
+    YT_CUDA(c, cudaMemsetAsync(c->wkey.p, 0, cap * 8, c->stream));
+    YT_CUDA(c, cudaMemsetAsync(c->wcnt.p, 0, cap * 8, c->stream));
+    YT_CUDA(c, cudaMemsetAsync(counters, 0, 64, c->stream));
+    WordTab wt{c->wkey.as<unsigned long long>(), c->wcnt.as<unsigned long long>(), cap - 1};
+    word_insert_kernel<<<grid_for(c, m, 256, 8), 256, 0, c->stream>>>(d, m, 0, m, wt, counters, cap / 2);
+    c->launches++;
+    YT_CUDA(c, cudaGetLastError());
+    YT_CUDA(c, cudaMemcpyAsync(h, counters, 32, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (!h[2]) break;
+    c->feed_wcap *= 4;
+  }
+  c->n_word_occ += h[0];
+  const uint64_t U = h[1];
+  if (U) {
+    YT_CUDA(c, c->wpos.reserve((U + 1) * 8));
+    YT_CUDA(c, c->wfreq.reserve((U + 1) * 8));
+    YT_CUDA(c, c->wlen.reserve((U + 1) * 8));
+    YT_CUDA(c, c->scratch_key.reserve((U + 1) * 8));
+    auto *mlen = c->wlen.as<unsigned long long>(), *moff = c->scratch_key.as<unsigned long long>();
+    WordTab wt{c->wkey.as<unsigned long long>(), c->wcnt.as<unsigned long long>(), c->feed_wcap - 1};
+    const unsigned grid = (unsigned)grid_for(c, U, 256, 8);
+    word_compact_kernel<<<grid_for(c, c->feed_wcap, 256, 8), 256, 0, c->stream>>>(wt, counters, c->wpos.as<uint64_t>(),
+                                                                                  c->wfreq.as<uint64_t>());
+    WordTab ft{c->fkey.as<unsigned long long>(), c->fcnt.as<unsigned long long>(), c->feed_fcap - 1};
+    word_merge_lookup_kernel<<<grid, 256, 0, c->stream>>>(d, m, c->wpos.as<uint64_t>(), c->wfreq.as<uint64_t>(), U, ft,
+                                                          c->arena.as<uint8_t>() + 16, mlen, counters);
+    c->launches += 2;
+    if (device_scan(c, mlen, U, moff, counters + 4)) return 1;
+    YT_CUDA(c, cudaMemcpyAsync(h + 4, counters + 4, 16, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    const uint64_t bytes = h[4], fresh = h[5];
+    if (fresh) {
+      if (c->arena_len + bytes >= POS_MASK) YT_FAIL(c, "fed corpus: its unique words exceed 2^40 bytes");
+      if (arena_reserve(c, c->arena_len + bytes) || ftab_reserve(c, fresh)) return 1;
+      ft = WordTab{c->fkey.as<unsigned long long>(), c->fcnt.as<unsigned long long>(), c->feed_fcap - 1};
+      word_merge_insert_kernel<<<grid, 256, 0, c->stream>>>(d, m, c->wpos.as<uint64_t>(), c->wfreq.as<uint64_t>(), U, mlen,
+                                                            moff, ft, c->arena.as<uint8_t>() + 16, c->arena_len);
+      c->launches++;
+      c->arena_len += bytes;
+      c->feed_fn += fresh;
+    }
+  }
+  YT_CUDA(c, cudaGetLastError());
+  YT_CUDA(c, cudaEventRecord(c->ev_feed_done[s], c->stream));
+  c->feed_pieces++;
+  note_peak(c);
+  return 0;
+}
+
+// The first `cut` bytes of the staging buffer being filled become a piece: copied now, processed after the next cut.
+static int feed_submit(yttm_ctx *c, uint64_t cut) {
+  const int s = c->feed_cur, o = s ^ 1;
+  const uint64_t tail = c->feed_len - cut;
+  YT_CUDA(c, cudaEventSynchronize(c->ev_feed_copied[o]));   // the copy of the piece before read buffer o
+  if (stage_reserve(c, o, tail)) return 1;
+  if (tail) std::memcpy(c->feed_stage[o], c->feed_stage[s] + cut, tail);
+  if (cut > c->feed_dev[s].cap) {   // the piece buffer grows: its last piece's passes are done first
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    YT_CUDA(c, c->feed_dev[s].reserve(cut));
+  }
+  YT_CUDA(c, cudaStreamWaitEvent(c->stream2, c->ev_feed_done[s], 0));
+  YT_CUDA(c, cudaMemcpyAsync(c->feed_dev[s].p, c->feed_stage[s], cut, cudaMemcpyHostToDevice, c->stream2));
+  YT_CUDA(c, cudaEventRecord(c->ev_feed_copied[s], c->stream2));
+  if (c->feed_pending >= 0 && feed_process(c, c->feed_pending, c->feed_pending_len)) return 1;
+  c->feed_pending = s;
+  c->feed_pending_len = cut;
+  c->feed_cur = o;
+  c->feed_len = c->feed_nows = tail;   // what follows the last whitespace byte holds none
+  return 0;
+}
+
+int yttm_train_feed_begin(yttm_ctx *c) {
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (ensure_stream2(c)) return 1;
+  for (int s = 0; s < 2; s++) {
+    if (!c->ev_feed_copied[s]) YT_CUDA(c, cudaEventCreateWithFlags(&c->ev_feed_copied[s], cudaEventDisableTiming));
+    if (!c->ev_feed_done[s]) YT_CUDA(c, cudaEventCreateWithFlags(&c->ev_feed_done[s], cudaEventDisableTiming));
+  }
+  // a new training starts, as in yttm_train_load_corpus; the corpus of an earlier one does not stay resident
+  if (feed_release(c)) return 1;
+  c->text_buf.release();
+  c->d_text = nullptr;
+  c->n_text = 0;
+  c->text_external = false;
+  c->have_alphabet = false;
+  c->pipe_hist = false;
+  c->pipe_wtab_cap = 0;
+  c->n_words = c->n_slots = c->n_unique = c->n_word_occ = 0;
+  c->pcap = 0;
+  c->stats = yttm_train_stats{};
+  ytc::timers_reset(c);
+  c->dev_peak = 0;
+  c->feed_piece = (uint64_t)ytc::env_int("YTTM_TRAIN_FEED_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;
+  c->feed_cur = 0;
+  c->feed_len = c->feed_nows = 0;
+  c->arena_len = c->n_fed = c->feed_pieces = c->feed_fn = 0;
+  // per-piece table: one slot per 32 bytes (a piece's distinct words are far fewer than its words); the persistent
+  // table and the arena start small and grow with the unique words
+  c->feed_wcap = std::min<uint64_t>(std::max<uint64_t>(ytc::pow2ceil(c->feed_piece / 32), 1u << 10), 1ull << 26);
+  c->feed_fcap = 1u << 10;
+  YT_CUDA(c, c->hist.reserve((CP_LIMIT + 1) * 8));
+  YT_CUDA(c, cudaMemsetAsync(c->hist.p, 0, (CP_LIMIT + 1) * 8, c->stream));
+  YT_CUDA(c, c->counters.reserve(64));
+  YT_CUDA(c, c->fkey.reserve(c->feed_fcap * 8));
+  YT_CUDA(c, c->fcnt.reserve(c->feed_fcap * 8));
+  YT_CUDA(c, cudaMemsetAsync(c->fkey.p, 0, c->feed_fcap * 8, c->stream));
+  YT_CUDA(c, cudaMemsetAsync(c->fcnt.p, 0, c->feed_fcap * 8, c->stream));
+  YT_CUDA(c, c->arena.reserve(1u << 16));
+  YT_CUDA(c, cudaMemsetAsync(c->arena.p, ' ', 16, c->stream));
+  c->feeding = true;
+  note_peak(c);
+  return 0;
+}
+
+int yttm_train_feed(yttm_ctx *c, const char *bytes, uint64_t n) {
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (!c->feeding) YT_FAIL(c, "yttm_train_feed: yttm_train_feed_begin has not run");
+  c->n_fed += n;
+  while (n) {
+    const uint64_t room = c->feed_len < c->feed_piece ? c->feed_piece - c->feed_len : c->feed_piece;
+    const uint64_t take = std::min(n, room);
+    if (stage_reserve(c, c->feed_cur, c->feed_len + take)) return 1;
+    std::memcpy(c->feed_stage[c->feed_cur] + c->feed_len, bytes, take);
+    c->feed_len += take;
+    bytes += take;
+    n -= take;
+    if (c->feed_len < c->feed_piece) continue;
+    const uint64_t cut = piece_cut(reinterpret_cast<const char *>(c->feed_stage[c->feed_cur]) + c->feed_nows,
+                                   c->feed_len - c->feed_nows);
+    if (!cut) { c->feed_nows = c->feed_len; continue; }   // no whitespace byte yet: the piece grows until one comes
+    if (feed_submit(c, c->feed_nows + cut)) return 1;
+  }
+  return 0;
+}
+
+int yttm_train_feed_end(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct) {
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (!c->feeding) YT_FAIL(c, "yttm_train_feed_end: yttm_train_feed_begin has not run");
+  if (c->feed_len && feed_submit(c, c->feed_len)) return 1;   // the last piece ends with the corpus
+  if (c->feed_pending >= 0 && feed_process(c, c->feed_pending, c->feed_pending_len)) return 1;
+  c->feed_pending = -1;
+  // the persistent table -> wpos / wfreq (arena positions); the arena with its pads becomes the text
+  const uint64_t U = c->feed_fn;
+  auto *counters = c->counters.as<unsigned long long>();
+  YT_CUDA(c, c->wpos.reserve((U + 1) * 8));
+  YT_CUDA(c, c->wfreq.reserve((U + 1) * 8));
+  YT_CUDA(c, cudaMemsetAsync(counters + 3, 0, 8, c->stream));
+  if (U) {
+    WordTab ft{c->fkey.as<unsigned long long>(), c->fcnt.as<unsigned long long>(), c->feed_fcap - 1};
+    word_compact_kernel<<<grid_for(c, c->feed_fcap, 256, 8), 256, 0, c->stream>>>(ft, counters, c->wpos.as<uint64_t>(),
+                                                                                  c->wfreq.as<uint64_t>());
+    c->launches++;
+  }
+  if (arena_reserve(c, c->arena_len)) return 1;
+  YT_CUDA(c, cudaMemsetAsync(c->arena.as<uint8_t>() + 16 + c->arena_len, ' ', 32, c->stream));
+  YT_CUDA(c, cudaGetLastError());
+  note_peak(c);
+  std::swap(c->text_buf, c->arena);
+  if (feed_release(c)) return 1;   // (synchronises: the compaction has run)
+  c->wkey.release(); c->wcnt.release();   // the per-piece table
+  c->d_text = c->text_buf.as<uint8_t>() + 16;
+  c->n_text = c->arena_len;
+  c->n_unique = U;
+  c->fed_words = true;
+  return hist_summarise(c, data_len, n_distinct);
 }
 
 static int hist_summarise(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct) {
@@ -1015,6 +1408,8 @@ static int hist_summarise(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct)
 
 int yttm_train_char_hist(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct) {
   YT_CUDA(c, cudaSetDevice(c->device));
+  if (c->feeding) YT_FAIL(c, "yttm_train_char_hist: yttm_train_feed_end has not run");
+  if (c->fed_words) return hist_summarise(c, data_len, n_distinct);   // counted per piece (the text is the word arena)
   if (c->pipe_hist) {   // counted while the text was copied (yttm_train_load_corpus)
     c->pipe_hist = false;
     return hist_summarise(c, data_len, n_distinct);
@@ -1081,11 +1476,12 @@ static int finish_build(yttm_ctx *c, yttm_train_stats *stats) {
   h.n_done = 0; h.stop = 0; h.dead = 0; h.slots = c->n_slots;
   YT_CUDA(c, cudaMemcpyAsync(ctl, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
   YT_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->stats.n_bytes = c->n_text;
+  c->stats.n_bytes = c->fed_words ? c->n_fed : c->n_text;
   c->stats.n_words = c->n_word_occ;
   c->stats.n_unique = c->n_words;
   c->stats.n_tokens = c->n_slots;
   if (stats) *stats = c->stats;
+  note_peak(c);
   return 0;
 }
 
@@ -1171,9 +1567,17 @@ static int build_tokens(yttm_ctx *c, uint64_t U, yttm_train_stats *stats) {
     word_tokens_kernel<0><<<nb, 256, 0, c->stream>>>(c->d_text, n, c->wpos.as<uint64_t>(), U, c->cp2id.as<uint32_t>(),
                                                      c->space_id, lens, nullptr, nullptr, nullptr);
     c->launches++;
+    unsigned long long too_many = 0;
+    if (c->fed_words) {   // a fed corpus is not bounded by 2^40 bytes, so neither is a word's count change
+      YT_CUDA(c, cudaMemsetAsync(counters + 5, 0, 8, c->stream));
+      word_count_limit_kernel<<<nb, 256, 0, c->stream>>>(lens, c->wfreq.as<uint64_t>(), U, counters + 5);
+      c->launches++;
+      YT_CUDA(c, cudaMemcpyAsync(&too_many, counters + 5, 8, cudaMemcpyDeviceToHost, c->stream));
+    }
     if (device_scan(c, lens, U, scan, counters + 4)) return 1;
     YT_CUDA(c, cudaMemcpyAsync(&T, counters + 4, 8, cudaMemcpyDeviceToHost, c->stream));
     YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (too_many) YT_FAIL(c, "fed corpus: a word's frequency x tokens must stay below 2^43");
     if (T >= 0xfffffff0ull) YT_FAIL(c, "more than 2^32 tokens in the unique words of one shard");
     YT_CUDA(c, c->tok[0].reserve((T + 4) * 4));
     word_tokens_kernel<1><<<nb, 256, 0, c->stream>>>(c->d_text, n, c->wpos.as<uint64_t>(), U, c->cp2id.as<uint32_t>(),
@@ -1196,9 +1600,14 @@ static int build_tokens(yttm_ctx *c, uint64_t U, yttm_train_stats *stats) {
 
 int yttm_train_build(yttm_ctx *c, yttm_train_stats *stats) {
   YT_CUDA(c, cudaSetDevice(c->device));
+  if (c->feeding) YT_FAIL(c, "yttm_train_build: yttm_train_feed_end has not run");
   if (!c->have_alphabet) YT_FAIL(c, "yttm_train_build: alphabet not set");
-  uint64_t U = 0;
-  if (build_word_table(c, nullptr, &U)) return 1;
+  uint64_t U = c->n_unique;   // a fed corpus: its words are in wpos / wfreq already
+  if (c->fed_words) {
+    if (c->pcap) YT_FAIL(c, "yttm_train_build: the fed words were built already (feed the corpus again)");
+  } else if (build_word_table(c, nullptr, &U)) {
+    return 1;
+  }
   return build_tokens(c, U, stats);
 }
 
@@ -1551,6 +1960,7 @@ int yttm_train_run(yttm_ctx *c, uint32_t first_new_id, uint32_t max_merges, uint
   c->loop_iters = h.iters;
   c->loop_sweeps = h.n_sweeps;
   c->loop_xq_round = h.xq_round;
+  note_peak(c);
   *n_done_out = h.n_done;
   if (h.n_done) {
     YT_CUDA(c, cudaMemcpyAsync(rules_xyz, c->d_rules.p, (size_t)h.n_done * 12, cudaMemcpyDeviceToHost, c->stream));

@@ -509,9 +509,9 @@ def release_training_cache():
 
 def train_report():
     """Sizes / stage timings of the last BPE.train on this thread (dict)."""
-    out = (C.c_double * 17)()
-    n = _lib.lib().yttm_api_train_report(out, 17)
     names = ["n_bytes", "data_len", "n_words", "n_unique", "n_tokens", "n_pairs", "n_merges", "read_s", "h2d_ms",
              "char_hist_ms", "word_count_ms", "tokenise_ms", "pair_hist_ms", "merge_loop_ms", "total_s", "launches",
-             "loop_launches"]
+             "loop_launches", "feed_pieces", "device_peak_bytes"]
+    out = (C.c_double * len(names))()
+    n = _lib.lib().yttm_api_train_report(out, len(names))
     return dict(zip(names[:n], list(out)[:n]))
