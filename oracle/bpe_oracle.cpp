@@ -25,6 +25,7 @@
 //  * apply greedily left to right (stress_test.cpp:181-188; bpe.cpp:644-690);
 //  * rename around special ids (bpe.cpp:814-837); model file as utils.cpp:50-91.
 #include <algorithm>
+#include <cmath>
 #include <chrono>
 #include <cstdint>
 #include <cstdio>
@@ -271,7 +272,7 @@ static inline void philox(uint32_t k0, uint32_t k1, uint32_t c[4]) {
   }
 }
 // One Bernoulli(skip) draw: counter = (sentence index lo/hi, byte offset of the word in the
-// sentence, draw number); key = seed.  skip <=> r < floor(p * 2^32).
+// sentence, draw number); key = seed.  skip <=> r < ceil(p * 2^32), i.e. r / 2^32 < p.
 static inline bool drop_draw(uint64_t seed, uint64_t sent, uint32_t word_off, uint32_t draw, uint64_t thresh) {
   uint32_t c[4] = {(uint32_t)sent, (uint32_t)(sent >> 32), word_off, draw};
   philox((uint32_t)seed, (uint32_t)(seed >> 32), c);
@@ -300,7 +301,7 @@ static void encode(const Model &m, const uint8_t *s, uint64_t n, bool bos, bool 
   }
   while (!cps.empty() && is_space(cps.back())) { cps.pop_back(); offs.pop_back(); }  // bpe.cpp:1500
   const uint32_t UNK_BASE = 1000000000u;  // bpe.cpp:1503
-  uint64_t thresh = (uint64_t)(dropout * 4294967296.0);
+  uint64_t thresh = dropout <= 0 ? 0 : (uint64_t)std::ceil(std::min(dropout, 1.0) * 4294967296.0);  // r / 2^32 < p
   std::vector<uint32_t> t;
   for (size_t i = 0; i < cps.size();) {
     while (i < cps.size() && is_space(cps[i])) i++;

@@ -259,6 +259,63 @@ class OracleEncoder(_Enc):
         return _unpack(ids, oo)
 
 
+class ReferenceReplay:
+    """oracle/_ref/libyttm_ref_replay.so: the unmodified reference whose BPE-dropout draws are the product's Philox
+    draws (oracle/replay_rng.h), one word at a time (oracle/ref_replay.cpp)."""
+
+    def __init__(self, model_path=None):
+        path = os.path.join(ORACLE_DIR, "_ref", "libyttm_ref_replay.so")
+        if not os.path.exists(path):
+            raise FileNotFoundError(path)
+        self.lib = lib = C.CDLL(path)
+        lib.rpl_open.restype = C.c_void_p
+        lib.rpl_open.argtypes = [C.c_char_p, C.c_char_p, C.c_int]
+        lib.rpl_close.argtypes = [C.c_void_p]
+        lib.rpl_encode.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_double, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_char_p,
+                                   C.c_int]
+        lib.rpl_result.argtypes = [C.c_void_p] * 5
+        lib.rpl_engine.argtypes = [C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
+        self.h = None
+        if model_path is not None:
+            err = C.create_string_buffer(ERRLEN)
+            self.h = lib.rpl_open(model_path.encode(), err, ERRLEN)
+            if not self.h:
+                raise ValueError(err.value.decode())
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.lib.rpl_close(self.h)
+
+    def encode_words(self, words, seeds, sents, word_offs, p, subwords=False):
+        """Word i (bytes) under key (seeds[i], sents[i], word_offs[i]) -> {"ids": flat ids, "n": ids per word,
+        "draws": draws per word, "pieces": per word the pieces joined by "\\x01" (with subwords)}."""
+        buf, offs = _pack(words)
+        seeds = np.ascontiguousarray(seeds, dtype=np.uint64)
+        sents = np.ascontiguousarray(sents, dtype=np.uint64)
+        word_offs = np.ascontiguousarray(word_offs, dtype=np.uint32)
+        n_ids, n_text, err = C.c_uint64(0), C.c_uint64(0), C.create_string_buffer(ERRLEN)
+        if self.lib.rpl_encode(self.h, buf, offs.ctypes.data, len(words), seeds.ctypes.data, sents.ctypes.data,
+                               word_offs.ctypes.data, p, int(subwords), C.byref(n_ids), C.byref(n_text), err, ERRLEN):
+            raise ValueError(err.value.decode())
+        ids = np.zeros(n_ids.value + 1, dtype=np.int32)
+        io = np.zeros(len(words) + 1, dtype=np.uint64)
+        draws = np.zeros(len(words) + 1, dtype=np.uint32)
+        text = C.create_string_buffer(n_text.value + 1)
+        self.lib.rpl_result(self.h, ids.ctypes.data, io.ctypes.data, draws.ctypes.data, text)
+        out = {"ids": ids[:n_ids.value].tolist(), "n": np.diff(io).tolist(), "draws": draws[:len(words)].tolist()}
+        if subwords:
+            out["pieces"] = text.raw[:n_text.value].decode("utf-8").split("\n")[:-1]
+        return out
+
+    def engine(self, seed, sent, word_off, n):
+        """(2n raw engine words, n uniform_real_distribution<>(0, 1) draws) under one key."""
+        words = np.zeros(2 * n, dtype=np.uint32)
+        canon = np.zeros(n, dtype=np.float64)
+        self.lib.rpl_engine(seed, sent, word_off, n, words.ctypes.data, canon.ctypes.data)
+        return words.tolist(), canon.tolist()
+
+
 def have_reference(kind="det"):
     return os.path.exists(os.path.join(ORACLE_DIR, "_ref", "libyttm_ref_%s.so" % kind))
 
@@ -419,6 +476,19 @@ class StoredRefEncoder:
     def decode(self, ids):
         return _call(_digest("decode", self.model, np.asarray(ids, dtype=np.int64).tobytes()),
                      lambda: self._live().decode(ids))
+
+    def replay_words(self, words, seeds, sents, word_offs, p, subwords=False):
+        """ReferenceReplay.encode_words on this model (BPE-dropout with the product's draws)."""
+        keys = np.stack([np.asarray(seeds, dtype=np.uint64), np.asarray(sents, dtype=np.uint64),
+                         np.asarray(word_offs, dtype=np.uint64)]).tobytes() if len(words) else b""
+        return _call(_digest("replay", self.model, *words, len(words), keys, float(p), bool(subwords)),
+                     lambda: ReferenceReplay(self.path).encode_words(words, seeds, sents, word_offs, p, subwords))
+
+
+def replay_engine(seed, sent, word_off, n):
+    """ReferenceReplay.engine, stored like the reference's answers."""
+    return _call(_digest("replay_engine", seed, sent, word_off, n),
+                 lambda: list(ReferenceReplay().engine(seed, sent, word_off, n)), full=True)
 
 
 def tmp_model_path(tag="m"):

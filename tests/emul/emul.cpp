@@ -7,6 +7,7 @@
 // compares the result with the oracle, so logic errors in the device functions are caught in
 // the build container, which has no GPU.
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <fstream>
@@ -155,7 +156,7 @@ int emul_encode(const char *model_path, const char *bytes_c, const uint64_t *off
     return it->second.first;
   };
   const uint8_t *s = (const uint8_t *)bytes_c;
-  uint64_t thresh = dropout <= 0 ? 0 : (uint64_t)(dropout * 4294967296.0);
+  uint64_t thresh = dropout <= 0 ? 0 : (uint64_t)std::ceil(std::min(dropout, 1.0) * 4294967296.0);  // as enc_device
   uint64_t pos = 0;
   for (uint64_t si = 0; si < n_sent; si++) {
     out_offs[si] = pos;

@@ -30,6 +30,7 @@
 // The ids of a word are kept in its private slots of a scratch buffer (a word of k bytes owns k+1 slots), at a
 // position that is a pure function of its byte position, so no kernel depends on another block's progress.
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 
@@ -1205,7 +1206,10 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   a.space_id = enc->space_id;
   a.unk_id = enc->unk; a.bos_id = enc->bos; a.eos_id = enc->eos;
   a.bos = bos; a.eos = eos; a.reverse = reverse;
-  a.drop_thresh = dropout <= 0 ? 0 : (uint64_t)(dropout * 4294967296.0);
+  // The reference skips an event iff u < p, and a draw r stands for u = r / 2^32, so skip iff r < ceil(p * 2^32)
+  // (p * 2^32 is exact in double).  Any p > 0 gives a threshold of at least 1 and so takes the dropout path, as the
+  // reference's `dropout_prob == 0` test does (bpe.cpp:1542); p >= 1 skips every event.
+  a.drop_thresh = dropout <= 0 ? 0 : (uint64_t)std::ceil(std::min(dropout, 1.0) * 4294967296.0);
   a.seed = seed; a.first_sentence = first_sentence;
   *out_n = 0;
   auto *d_total = e->counter.as<unsigned long long>() + 1;
