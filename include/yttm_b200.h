@@ -138,7 +138,10 @@ int yttm_train_dist_word_table(yttm_ctx *ctx, uint64_t *n_unique);
  * *d_freq (uint64 per word): its count.  Device memory owned by the context, valid until the next call on it. */
 int yttm_train_dist_export_words(yttm_ctx *ctx, uint64_t *bytes_per_dst, uint64_t *words_per_dst, void **d_bytes,
                                  void **d_pos, void **d_freq);
-/* the same three buffers after the all-to-all (DEVICE pointers, sources back to back) + the per-source sizes */
+/* the same three buffers after the all-to-all (DEVICE pointers, sources back to back) + the per-source sizes.
+ * The preconditions of yttm_train_import_words hold for the imported set; the count limit is checked on the counts
+ * summed over the sources: it fails ("yttm_train_dist_import_words: a word's frequency x tokens must stay below 2^43")
+ * when a word's total count x its tokens (U+2581 included) reaches 2^43. */
 int yttm_train_dist_import_words(yttm_ctx *ctx, const void *d_bytes, const uint64_t *bytes_per_src, const void *d_pos,
                                  const void *d_freq, const uint64_t *words_per_src, yttm_train_stats *stats);
 

@@ -132,8 +132,11 @@ def run_pairs(tokens, freq, out):
 def expected_front(data, cp2id, space_id):
     """Everything the byte passes and the initial pair table give, for an alphabet cp2id ({code point: id})."""
     data_len, hist = char_hist(data)
-    occ = byte_words(data)
-    uniq = collections.Counter(occ)
+    return dict(expected_words(collections.Counter(byte_words(data)), cp2id, space_id), data_len=data_len, hist=hist)
+
+
+def expected_words(uniq, cp2id, space_id):
+    """The word fields of expected_front for a set of byte-words with counts ({byte-word: count})."""
     words = []
     for w, f in uniq.items():
         t = word_tokens(w, cp2id, space_id)
@@ -143,5 +146,5 @@ def expected_front(data, cp2id, space_id):
     pairs = collections.Counter()
     for t, f in words:
         run_pairs(t, f, pairs)
-    return dict(data_len=data_len, hist=hist, n_words=len(occ), n_unique=len(words),
-                n_tokens=sum(len(t) for t, _ in words), words=words, pairs=dict(pairs))
+    return dict(n_words=sum(uniq.values()), n_unique=len(words), n_tokens=sum(len(t) for t, _ in words), words=words,
+                pairs=dict(pairs))

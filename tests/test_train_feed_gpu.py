@@ -221,6 +221,12 @@ def _front_after_load(L, ctx, cp2id):
     assert L.yttm_train_set_alphabet(ctx, kc.ctypes.data, ki.ctypes.data, len(kc), FG.SPACE_ID) == 0
     st = _lib.TrainStats()
     assert L.yttm_train_build(ctx, C.byref(st)) == 0, L.yttm_last_error(ctx)
+    return dict(words_and_pairs(L, ctx, st), data_len=dl.value, hist=dict(zip(cps.tolist(), cnt.tolist())))
+
+
+def words_and_pairs(L, ctx, st):
+    """The word and pair fields of _front_ref.expected_front from a context that has built its words (st: the
+    statistics the build returned)."""
     nw, nt = C.c_uint64(0), C.c_uint64(0)
     assert L.yttm_train_export_words(ctx, None, 0, None, None, 0, C.byref(nw), C.byref(nt)) == 0
     tok = np.zeros(nt.value + 1, dtype=np.uint32)
@@ -234,10 +240,9 @@ def _front_after_load(L, ctx, cp2id):
     keys = np.zeros(st.n_pairs + 16, dtype=np.uint64)
     cts = np.zeros(st.n_pairs + 16, dtype=np.uint64)
     assert L.yttm_train_dump_pairs(ctx, keys.ctypes.data, cts.ctypes.data, len(keys), C.byref(n)) == 0
-    return dict(data_len=dl.value, hist=dict(zip(cps.tolist(), cnt.tolist())), n_words=st.n_words,
-                n_unique=st.n_unique, n_tokens=st.n_tokens, words=words, pairs=dict(zip(keys[:n.value].tolist(),
-                                                                                       cts[:n.value].tolist())),
-                n_pairs=st.n_pairs, n_bytes=st.n_bytes)
+    return dict(n_words=st.n_words, n_unique=st.n_unique, n_tokens=st.n_tokens, words=words,
+                pairs=dict(zip(keys[:n.value].tolist(), cts[:n.value].tolist())), n_pairs=st.n_pairs,
+                n_bytes=st.n_bytes)
 
 
 def _sizes(kind, seed=5):

@@ -398,7 +398,8 @@ __global__ void __launch_bounds__(256) word_table_rehash_kernel(WordTab old, Wor
 }
 
 // freq x tokens of every word below 2^43 (the signed 44-bit count change of the merge loop's exchange entries, as
-// yttm_train_import_words checks): a text shard cannot exceed it, a fed corpus can.  lens: tokens per word.
+// yttm_train_import_words checks): a text shard cannot exceed it, a fed corpus and a word list imported from other ranks
+// (counts summed over the ranks) can.  lens: tokens per word.
 __global__ void word_count_limit_kernel(const unsigned long long *__restrict__ lens, const uint64_t *__restrict__ wfreq,
                                         uint64_t n_words, unsigned long long *bad) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -1550,7 +1551,9 @@ static int build_word_table(yttm_ctx *c, const WordList *list, uint64_t *n_uniqu
 }
 
 // Phase 2b + 3: tokenise the U unique words (wpos / wfreq) into the packed buffer, build the pair table.
-static int build_tokens(yttm_ctx *c, uint64_t U, yttm_train_stats *stats) {
+// counts_of: the words' counts are not bounded by the text's length (a fed corpus, a list imported from other ranks),
+// so every word's freq x tokens is checked against 2^43; the name starts the error message.  nullptr: no check.
+static int build_tokens(yttm_ctx *c, uint64_t U, yttm_train_stats *stats, const char *counts_of) {
   const uint64_t n = c->n_text;
   auto *counters = c->counters.as<unsigned long long>();
   ytc::timer_begin(c, "tokenise");
@@ -1568,7 +1571,7 @@ static int build_tokens(yttm_ctx *c, uint64_t U, yttm_train_stats *stats) {
                                                      c->space_id, lens, nullptr, nullptr, nullptr);
     c->launches++;
     unsigned long long too_many = 0;
-    if (c->fed_words) {   // a fed corpus is not bounded by 2^40 bytes, so neither is a word's count change
+    if (counts_of) {
       YT_CUDA(c, cudaMemsetAsync(counters + 5, 0, 8, c->stream));
       word_count_limit_kernel<<<nb, 256, 0, c->stream>>>(lens, c->wfreq.as<uint64_t>(), U, counters + 5);
       c->launches++;
@@ -1577,7 +1580,7 @@ static int build_tokens(yttm_ctx *c, uint64_t U, yttm_train_stats *stats) {
     if (device_scan(c, lens, U, scan, counters + 4)) return 1;
     YT_CUDA(c, cudaMemcpyAsync(&T, counters + 4, 8, cudaMemcpyDeviceToHost, c->stream));
     YT_CUDA(c, cudaStreamSynchronize(c->stream));
-    if (too_many) YT_FAIL(c, "fed corpus: a word's frequency x tokens must stay below 2^43");
+    if (too_many) YT_FAIL(c, std::string(counts_of) + ": a word's frequency x tokens must stay below 2^43");
     if (T >= 0xfffffff0ull) YT_FAIL(c, "more than 2^32 tokens in the unique words of one shard");
     YT_CUDA(c, c->tok[0].reserve((T + 4) * 4));
     word_tokens_kernel<1><<<nb, 256, 0, c->stream>>>(c->d_text, n, c->wpos.as<uint64_t>(), U, c->cp2id.as<uint32_t>(),
@@ -1608,7 +1611,8 @@ int yttm_train_build(yttm_ctx *c, yttm_train_stats *stats) {
   } else if (build_word_table(c, nullptr, &U)) {
     return 1;
   }
-  return build_tokens(c, U, stats);
+  // a fed corpus is not bounded by 2^40 bytes, so neither is a word's count change
+  return build_tokens(c, U, stats, c->fed_words ? "fed corpus" : nullptr);
 }
 
 // ---- multi-GPU (one process per GPU; include/yttm_b200.h has the protocol) ---------------------------------------
@@ -1664,6 +1668,9 @@ int yttm_train_dist_connect(yttm_ctx *c, const void *handles) {
 
 int yttm_train_dist_word_table(yttm_ctx *c, uint64_t *n_unique) {
   YT_CUDA(c, cudaSetDevice(c->device));
+  if (c->feeding) YT_FAIL(c, "yttm_train_dist_word_table: yttm_train_feed_end has not run");
+  // a fed shard: feed_end built its table; splitting the word arena again would count every word once
+  if (c->fed_words) { *n_unique = c->n_unique; return 0; }
   return build_word_table(c, nullptr, n_unique);
 }
 
@@ -1743,7 +1750,8 @@ int yttm_train_dist_import_words(yttm_ctx *c, const void *d_bytes, const uint64_
   WordList wl{lp.as<uint64_t>(), lf.as<uint64_t>(), wo, bo, world};
   uint64_t U = 0;
   int rc = build_word_table(c, &wl, &U);
-  if (!rc) rc = build_tokens(c, U, stats);
+  // an imported count is a sum over ranks: nothing bounds it by the length of one shard
+  if (!rc) rc = build_tokens(c, U, stats, "yttm_train_dist_import_words");
   lp.release(); lf.release();
   return rc;
 }
