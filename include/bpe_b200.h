@@ -236,6 +236,16 @@ class BaseEncoder {
   Status decode_cli(const std::unordered_set<int> *ignore_ids) const;
   void vocab_cli(bool verbose) const;
 
+  // Encodes a file or pipe of any size on the GPU, line by line: a line ends at '\n' and nowhere else, the text after
+  // the last '\n' (if any) is a last line, and line i gets the ids encode_packed gives it without its '\n', as the next
+  // sentence of the dropout stream (a call with dropout advances the sentence counter by the number of lines).  in_fd is
+  // read in 16 MB blocks to its end.  text: `yttm encode --output_type id`'s text to out_path ("-" = stdout); else
+  // <out_path>.ids.npy (1-D uint16 when vocab_size() <= 65536, else int32) and <out_path>.offsets.npy (uint64,
+  // lines + 1 values from 0: line i = ids[offsets[i]:offsets[i+1]]).  Outputs are written under temporary names and
+  // renamed on success, so a failed call leaves nothing at the output names.  *n_bytes = input bytes.
+  Status encode_file(int in_fd, const std::string &out_path, bool text, bool bos, bool eos, bool reverse,
+                     double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const;
+
   // BPE-dropout stream: seed of the counter-based generator and the running sentence counter
   // (replaces the reference's global std::mt19937, bpe.cpp:1415).
   void set_dropout_seed(uint64_t seed) const { dropout_seed_ = seed; sentence_counter_ = 0; }

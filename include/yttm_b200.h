@@ -35,7 +35,8 @@ int yttm_device_count(void);
  * "loop_iters", "loop_refreshes", "loop_launches", "loop_resident", "table_capacity", and "xq_round" (exchange rounds
  * of the merge loop since the context was created or joined a job; they run on across trainings).  Counters of the
  * current training: "feed_pieces" (pieces of a fed corpus, 0 after load_corpus) and "dev_peak_bytes" (the largest sum
- * of the context's device buffers, sampled after every fed piece and every phase). */
+ * of the context's device buffers, sampled after every fed piece and every phase).  Counters of the last encode stream:
+ * "stream_pieces" and "stream_dev_peak_bytes" (see yttm_enc_stream_begin). */
 double yttm_stage_ms(const yttm_ctx *ctx, const char *stage);
 /* number of kernel launches issued by this context so far (bench.py: gpu_launches) */
 uint64_t yttm_launch_count(const yttm_ctx *ctx);
@@ -252,6 +253,33 @@ int yttm_enc_run_subwords_device(yttm_enc *enc, const char *d_bytes, const uint6
                                  uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
                                  uint64_t first_sentence_index, const uint8_t **d_pieces, const uint64_t **d_piece_offsets,
                                  const uint64_t **d_sent_offsets, uint64_t *n_pieces, uint64_t *n_piece_bytes);
+
+/* ---- encode stream: text of any size fed in blocks, encoded line by line ---------------------------------------
+ * A line ends at '\n' and nowhere else; the bytes after the last '\n', if any, are a last line (a stream ending in '\n'
+ * has no extra empty line, an empty stream has none).  Line i gets exactly the ids yttm_enc_run gives it without its
+ * '\n', as sentence first_sentence_index + i of the dropout stream.  The library cuts the fed text into pieces that end
+ * behind a '\n' (YTTM_ENC_STREAM_PIECE_KB, default 32768, read by begin; a longer line makes its piece grow to hold it),
+ * finds the lines on the device and encodes piece i while piece i + 1 is copied in and piece i - 1 is copied out and
+ * handed to the sink, so device memory is bounded by two pieces and the longest line.
+ * Formats of the sink's data: YTTM_STREAM_IDS16 (uint16 ids; the vocabulary must not exceed 65536), YTTM_STREAM_IDS32
+ * (int32 ids), YTTM_STREAM_TEXT (`yttm encode --output_type id`'s text: every id in decimal followed by one space, then
+ * '\n' per line).  While a stream is open every other encode and decode call on the encoder fails; any failure closes
+ * the stream (the next begin works) and yttm_enc_destroy frees an open one.  yttm_stage_ms(ctx, "stream_pieces") /
+ * ("stream_dev_peak_bytes"): pieces of the last stream and the largest sum of the encoder's device buffers, sampled
+ * after every piece. */
+#define YTTM_STREAM_IDS16 0
+#define YTTM_STREAM_IDS32 1
+#define YTTM_STREAM_TEXT 2
+/* Called on the calling thread of feed / end, in line order, with library-owned host memory valid until it returns.
+ * data: the ids (2 or 4 bytes each) or the text bytes of the lines that completed; line_ends[k]: the global id count
+ * at the end of the k-th of those lines (the same in every format).  Non-zero fails the stream. */
+typedef int (*yttm_enc_sink)(void *user, const void *data, uint64_t n_bytes, const uint64_t *line_ends, uint64_t n_lines);
+int yttm_enc_stream_begin(yttm_enc *enc, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                          uint64_t first_sentence_index, int format, yttm_enc_sink sink, void *user);
+/* any size and boundary; the bytes are copied before the call returns */
+int yttm_enc_stream_feed(yttm_enc *enc, const char *bytes, uint64_t n);
+/* encodes what is left, hands it to the sink and closes the stream; each output may be NULL */
+int yttm_enc_stream_end(yttm_enc *enc, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes_in);
 
 /* ---- decoding: BaseEncoder::decode (bpe.cpp:1843-1861 + id_to_subword :1774-1807) of a batch ---- */
 

@@ -111,6 +111,11 @@ int64_t yttm_api_vocab(void *handle);
 int yttm_api_encode_cli(void *handle, const char *output_type, int stream, int bos, int eos, int reverse,
                         double dropout);
 int yttm_api_decode_cli(void *handle, const int32_t *ignore, uint64_t n_ignore);
+/* BaseEncoder::encode_file: the lines of in_fd to <out_path>.ids.npy + <out_path>.offsets.npy, or with text != 0 to
+ * out_path ("-" = stdout) as `yttm encode --output_type id` writes them; uses the handle's dropout seed and counter.
+ * stats[3] = lines, ids, input bytes.  0 ok, 1 error. */
+int yttm_api_encode_file(void *handle, int in_fd, const char *out_path, int text, int bos, int eos, int reverse,
+                         double dropout, uint64_t *stats);
 void yttm_api_vocab_cli(void *handle, int verbose);
 
 /* order of the char2id lines of a model file written by the reference (BPEState::dump, utils.cpp:57-59):

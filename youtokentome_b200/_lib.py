@@ -32,6 +32,11 @@ def lib():
     return _lib
 
 
+# yttm_enc_sink of include/yttm_b200.h: (user, data, n_bytes, line_ends, n_lines) -> 0 or a failure
+ENC_SINK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_uint64)
+STREAM_IDS16, STREAM_IDS32, STREAM_TEXT = 0, 1, 2
+
+
 def bind(L):
     """Declare the C signatures of include/yttm_b200.h and include/yttm_b200_api.h on a loaded library."""
     vp, cp, u64, i32, dbl, i64 = C.c_void_p, C.c_char_p, C.c_uint64, C.c_int, C.c_double, C.c_int64
@@ -73,6 +78,7 @@ def bind(L):
         "yttm_api_vocab": (i64, [vp]),
         "yttm_api_encode_cli": (i32, [vp, cp, i32, i32, i32, i32, dbl]),
         "yttm_api_decode_cli": (i32, [vp, vp, u64]),
+        "yttm_api_encode_file": (i32, [vp, i32, cp, i32, i32, i32, i32, dbl, vp]),
         "yttm_api_vocab_cli": (None, [vp, i32]),
         "yttm_api_dump_order": (i32, [vp, u64, vp]),
         "yttm_api_redump": (i32, [cp, cp]),
@@ -121,6 +127,9 @@ def bind(L):
                                         C.POINTER(u64), C.POINTER(u64)]),
         "yttm_enc_run_subwords_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, u64, u64, C.POINTER(vp),
                                                C.POINTER(vp), C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]),
+        "yttm_enc_stream_begin": (i32, [vp, i32, i32, i32, dbl, u64, u64, i32, ENC_SINK, vp]),
+        "yttm_enc_stream_feed": (i32, [vp, vp, u64]),
+        "yttm_enc_stream_end": (i32, [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
         "yttm_dec_run": (i32, [vp, vp, vp, u64, vp, u64, vp, u64, vp, C.POINTER(u64)]),
         "yttm_dec_run_device": (i32, [vp, vp, u64, vp, u64, vp, u64, C.POINTER(vp), C.POINTER(vp), C.POINTER(u64)]),
     }
@@ -146,8 +155,8 @@ EXPORTED_SYMBOLS_DEVICE_ABI = [
     "yttm_train_dist_word_table", "yttm_train_dist_export_words", "yttm_train_dist_import_words", "yttm_train_run", "yttm_train_dump_pairs",
     "yttm_train_scan_once", "yttm_train_synth_words", "yttm_enc_create", "yttm_enc_destroy", "yttm_enc_run",
     "yttm_enc_run_device", "yttm_enc_run_spans", "yttm_enc_run_spans_device", "yttm_enc_run_subwords",
-    "yttm_enc_run_subwords_device", "yttm_enc_run_padded", "yttm_enc_run_padded_device", "yttm_dec_run",
-    "yttm_dec_run_device",
+    "yttm_enc_run_subwords_device", "yttm_enc_run_padded", "yttm_enc_run_padded_device", "yttm_enc_stream_begin",
+    "yttm_enc_stream_feed", "yttm_enc_stream_end", "yttm_dec_run", "yttm_dec_run_device",
 ]
 
 

@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cassert>
+#include <cerrno>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -15,6 +16,9 @@
 #include <functional>
 #include <sstream>
 #include <thread>
+
+#include <fcntl.h>
+#include <unistd.h>
 
 #include "../../include/bpe_b200.h"
 #include "../../include/yttm_b200.h"
@@ -944,6 +948,136 @@ Status BaseEncoder::decode_cli(const std::unordered_set<int> *ignore_ids) const 
     std::cout << out[0] << "\n";
   }
   std::cout << std::flush;
+  return Status();
+}
+
+
+// ---------------------------------------------------------------------------------------------
+// encode_file: a file or pipe through the device's encode stream (yttm_enc_stream_* of yttm_b200.h) into .npy files or
+// the text of `yttm encode --output_type id`
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+// An output written under a temporary name in its directory and renamed on commit; "-" is stdout (no rename).
+class OutFile {
+ public:
+  ~OutFile() {
+    if (fd_ >= 0 && fd_ != 1) ::close(fd_);
+    if (!tmp_.empty()) ::unlink(tmp_.c_str());
+  }
+  Status open(const std::string &path) {
+    path_ = path;
+    if (path == "-") { fd_ = 1; return Status(); }
+    static std::atomic<uint64_t> serial{0};
+    tmp_ = path + ".part-" + std::to_string((long)::getpid()) + "-" + std::to_string(serial++);
+    fd_ = ::open(tmp_.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC, 0666);
+    if (fd_ < 0) { tmp_.clear(); return error("cannot create"); }
+    return Status();
+  }
+  Status write(const void *data, uint64_t n) {
+    const char *p = static_cast<const char *>(data);
+    while (n) {
+      const ssize_t k = ::write(fd_, p, std::min<uint64_t>(n, 1u << 30));
+      if (k < 0 && errno == EINTR) continue;
+      if (k <= 0) return error("cannot write");
+      p += k;
+      n -= (uint64_t)k;
+    }
+    return Status();
+  }
+  Status write_at(uint64_t at, const std::string &s) {
+    if (::pwrite(fd_, s.data(), s.size(), (off_t)at) != (ssize_t)s.size()) return error("cannot write");
+    return Status();
+  }
+  Status commit() {
+    if (fd_ == 1) return Status();
+    const int fd = fd_;
+    fd_ = -1;
+    if (::close(fd) != 0) return error("cannot write");
+    if (::rename(tmp_.c_str(), path_.c_str()) != 0) return error("cannot create");
+    tmp_.clear();
+    return Status();
+  }
+
+ private:
+  Status error(const char *what) const {
+    return Status(1, std::string("encode_file: ") + what + " '" + path_ + "': " + std::strerror(errno));
+  }
+  std::string path_, tmp_;
+  int fd_ = -1;
+};
+
+// NPY format 1.0 header of a 1-D little-endian array of n values, always 128 bytes, so that the final shape can be
+// written over the first one
+std::string npy_header(const char *descr, uint64_t n) {
+  std::string dict = std::string("{'descr': '") + descr + "', 'fortran_order': False, 'shape': (" + std::to_string(n) +
+                     ",), }";
+  dict.resize(117, ' ');
+  dict += '\n';
+  return std::string("\x93NUMPY\x01\x00", 8) + std::string(1, (char)dict.size()) + std::string(1, '\0') + dict;
+}
+
+struct FileSink {
+  bool text = false, stop = false;
+  OutFile *ids = nullptr, *offsets = nullptr;  // text: `ids` holds the text
+  Status st;
+};
+
+int file_sink(void *user, const void *data, uint64_t n_bytes, const uint64_t *line_ends, uint64_t n_lines) {
+  auto *f = static_cast<FileSink *>(user);
+  if (f->stop) return 1;
+  f->st = f->ids->write(data, n_bytes);
+  if (f->st.ok() && !f->text) f->st = f->offsets->write(line_ends, n_lines * 8);
+  return f->st.ok() ? 0 : 1;
+}
+
+}  // namespace
+
+Status BaseEncoder::encode_file(int in_fd, const std::string &out_path, bool text, bool bos, bool eos, bool reverse,
+                                double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const {
+  *n_lines = *n_ids = *n_bytes = 0;
+  Status st = run_device("encode_file", bos, eos, 0, 0, [] { return 0; });  // the <BOS> / <EOS> and device checks
+  if (!st.ok()) return st;
+  if (!text && out_path == "-") return Status(1, "encode_file: the .npy form needs an output prefix, not '-'");
+  const bool narrow = vocab_size() <= 65536;
+  OutFile ids_file, offsets_file;
+  FileSink fs;
+  fs.text = text;
+  fs.ids = &ids_file;
+  fs.offsets = &offsets_file;
+  const char *descr = narrow ? "<u2" : "<i4";
+  const uint64_t zero = 0;
+  if (text) {
+    if (!(st = ids_file.open(out_path)).ok()) return st;
+  } else if (!(st = ids_file.open(out_path + ".ids.npy")).ok() || !(st = offsets_file.open(out_path + ".offsets.npy")).ok() ||
+             !(st = ids_file.write(npy_header(descr, 0).data(), 128)).ok() ||
+             !(st = offsets_file.write(npy_header("<u8", 0).data(), 128)).ok() || !(st = offsets_file.write(&zero, 8)).ok()) {
+    return st;
+  }
+  const int format = text ? YTTM_STREAM_TEXT : narrow ? YTTM_STREAM_IDS16 : YTTM_STREAM_IDS32;
+  if (yttm_enc_stream_begin(enc_, bos, eos, reverse, dropout_prob, dropout_seed_, sentence_counter_, format, file_sink, &fs))
+    return Status(1, ctx_err(ctx_));
+  auto failed = [&]() { return fs.st.ok() ? Status(1, ctx_err(ctx_)) : fs.st; };
+  std::vector<char> block((size_t)16 << 20);
+  while (true) {
+    const ssize_t k = ::read(in_fd, block.data(), block.size());
+    if (k < 0 && errno == EINTR) continue;
+    if (k < 0) {
+      st = Status(1, std::string("encode_file: cannot read the input: ") + std::strerror(errno));
+      fs.stop = true;  // the stream is closed by the failure of its sink, or ends with nothing left to hand over
+      uint64_t a, b, c;
+      yttm_enc_stream_end(enc_, &a, &b, &c);
+      return st;
+    }
+    if (k == 0) break;
+    if (yttm_enc_stream_feed(enc_, block.data(), (uint64_t)k)) return failed();
+  }
+  if (yttm_enc_stream_end(enc_, n_lines, n_ids, n_bytes)) return failed();
+  if (!text && (!(st = ids_file.write_at(0, npy_header(descr, *n_ids))).ok() ||
+                !(st = offsets_file.write_at(0, npy_header("<u8", *n_lines + 1))).ok()))
+    return st;
+  if (!(st = ids_file.commit()).ok() || (!text && !(st = offsets_file.commit()).ok())) return st;
+  if (dropout_prob > 0) sentence_counter_ += *n_lines;
   return Status();
 }
 

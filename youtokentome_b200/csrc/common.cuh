@@ -132,6 +132,8 @@ struct yttm_ctx {
   uint64_t loop_iters = 0, loop_relaunches = 0, loop_sweeps = 0;
   uint32_t loop_xq_round = 0;   // YtLoopCtl::xq_round after the last yttm_train_run
   double enc_chunks = -1;       // chunks the last host-buffer encode call was cut into (encode.cu)
+  // the last encode stream of the context (encode.cu): its pieces and the largest sum of its encoder's device buffers
+  double enc_stream_pieces = -1, enc_stream_peak = -1;
 
   yttm_train_stats stats{};
 };

@@ -5,6 +5,8 @@
 
 #include "common.cuh"
 
+struct yttm_enc_stream;  // an open encode stream (encode.cu, yttm_enc_stream_*)
+void yttm_enc_stream_free(yttm_enc_stream *s);
 struct yttm_dec;  // decode state (decode.cu): piece table + per-call buffers, made by the first decode call
 void yttm_dec_free(yttm_dec *d);
 struct yttm_enc;
@@ -38,12 +40,14 @@ struct yttm_enc {
     ytc::DevBuf swb, swc, rec;             // per-sentence word ranges, per-word records (id count, first ids)
     ytc::DevBuf rel, out_spans;            // spans: per-slot span relative to the word start, (start, end) per id
     ytc::DevBuf sub_len, sub_off, sub_out; // subwords: piece length per id, piece offsets, piece bytes
-    void release() {
+    template <class F> void each(F f) {
       ytc::DevBuf *b[] = {&d_bytes, &d_offs, &slots, &ranks, &aux, &wpos, &wsent, &lookback, &out_off, &out_ids, &counter, &longw,
                           &dd_tab, &dd_rep, &dd_list, &swb, &swc, &rec, &rel, &out_spans, &sub_len, &sub_off, &sub_out};
-      for (auto *x : b) x->release();
+      for (auto *x : b) f(x);
     }
+    void release() { each([](ytc::DevBuf *x) { x->release(); }); }
   } slot[2];
   cudaStream_t s_in = nullptr, s_out = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
+  yttm_enc_stream *stream = nullptr;  // open between yttm_enc_stream_begin and _end; owns both slots meanwhile
 };

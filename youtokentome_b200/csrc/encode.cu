@@ -27,6 +27,8 @@
 //   span_words_kernel           one thread per encoded word: the span of each of its ids relative to the word start
 //   emit_ids_kernel<true>       ... and the spans at the occurrences' positions
 //   sub_count_kernel / scan / sub_emit_kernel   one thread per id: piece lengths, offsets, piece bytes
+// An encode stream (yttm_enc_stream_*, the section at the end of this file) finds the lines of each fed piece on the
+// device, runs this flow on them and narrows the ids to uint16 or formats them as text.
 // The ids of a word are kept in its private slots of a scratch buffer (a word of k bytes owns k+1 slots), at a
 // position that is a pure function of its byte position, so no kernel depends on another block's progress.
 #include <algorithm>
@@ -1382,6 +1384,20 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   return 0;
 }
 
+// The copy streams and events of the two slots (made by the first call that pipelines).
+int pipe_init(yttm_enc *e) {
+  yttm_ctx *c = e->ctx;
+  if (e->s_in) return 0;
+  YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
+  YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; i++) {
+    YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_in[i], cudaEventDisableTiming));
+    YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming));
+    YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming));
+  }
+  return 0;
+}
+
 // Caller buffers of the host-buffer entry points; nullptr = not asked for.  ids_cap bounds ids / spans / pieces (one
 // piece per id), bytes_cap the piece bytes.
 struct HostOut {
@@ -1411,15 +1427,7 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
     if (o.piece_offsets) o.piece_offsets[0] = 0;
     return 0;
   }
-  if (!e->s_in) {
-    YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
-    YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_in[i], cudaEventDisableTiming));
-      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming));
-      YT_CUDA(c, cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming));
-    }
-  }
+  if (pipe_init(e)) return 1;
   // chunks of about CHUNK bytes, cut at sentence boundaries; chunk i lives in slot i & 1
   const uint64_t total_bytes = offsets[n_sent] - offsets[0];
   const uint64_t chunk_bytes = (uint64_t)ytc::env_int("YTTM_ENC_CHUNK_MB", 32, 1, INT_MAX) << 20;
@@ -1535,6 +1543,8 @@ int yttm_enc_check(yttm_enc *e, const char *who, int bos, int eos) {
   }
   yttm_ctx *c = e->ctx;
   YT_CUDA(c, cudaSetDevice(c->device));
+  if (e->stream)  // the stream's pieces are in flight in both slots between its calls
+    YT_FAIL(c, std::string(who) + ": an encode stream is open on this encoder (yttm_enc_stream_end closes it)");
   ytc::timers_reset(c);   // every encode and decode call starts here: the stage times describe this call alone
   if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
   if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
@@ -1595,6 +1605,7 @@ int yttm_enc_create(yttm_ctx *c, const uint32_t *char_cp, const uint32_t *char_i
 void yttm_enc_destroy(yttm_enc *e) {
   if (!e) return;
   cudaSetDevice(e->ctx->device);
+  yttm_enc_stream_free(e->stream);
   e->cp2id.release();
   e->rules.release();
   e->sub_table.release();
@@ -1718,4 +1729,419 @@ int yttm_enc_run_subwords(yttm_enc *e, const char *bytes, const uint64_t *offset
   return enc_run_host(e, "yttm_enc_run_subwords", bytes, offsets, n_sent, bos, eos, reverse, dropout, seed,
                       first_sentence_index, o, n_pieces, n_piece_bytes);
 }
+}  // extern "C"
+
+// =====================================================================================================================
+// Encode stream (yttm_enc_stream_*): text fed in blocks of any size is cut on the host into pieces that end behind a
+// '\n' (memrchr over the staged bytes not yet searched), and each piece runs on the device as
+//   line_count_kernel   '\n' bytes per 4 KB tile, 16-byte loads
+//   scan                tile bases + the piece's '\n' count (one 8-byte read-back: enc_device takes the line count)
+//   line_write_kernel   the offsets enc_device takes: 0, the byte behind every '\n', the end of a last line without one
+//                       (a line keeps its '\n': a trailing space byte changes neither the ids nor the dropout draws)
+//   enc_device          the ids of the lines, the batch path of yttm_enc_run
+//   narrow_ids_kernel   YTTM_STREAM_IDS16: the ids as uint16, so that the copy out and the file halve
+//   text_count_kernel   YTTM_STREAM_TEXT, warp per line: its bytes, "<id> " per id and the '\n'
+//   scan                line byte offsets + the piece's text bytes (one 8-byte read-back: the size of the copy out)
+//   text_emit_kernel    warp per line, 32 ids per round: a warp scan places each id's decimal digits
+//   add_base_kernel     line ends as global id counts
+// Piece i lives in slot i & 1: its copy in overlaps the kernels of piece i - 1 and the copy out and sink call of piece
+// i - 2.  The sink runs on the caller's thread, in line order, from pinned host buffers of the stream.
+namespace {
+
+constexpr uint32_t LS_T = 256;                     // line split: threads per block, 16 bytes each
+constexpr uint64_t LS_TILE = (uint64_t)LS_T * 16;  // bytes per block
+
+// bit k set: byte q + k of p[0, n) is '\n'
+__device__ __forceinline__ uint32_t newline_bits(const uint8_t *__restrict__ p, uint64_t q, uint64_t n) {
+  uint32_t m = 0;
+  if (q + 16 <= n) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p + q));
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const uint32_t x = w[i] ^ 0x0a0a0a0au;                                      // a '\n' byte becomes 0
+      const uint32_t z = ~(((x & 0x7f7f7f7fu) + 0x7f7f7f7fu) | x) & 0x80808080u;  // 0x80 exactly at the zero bytes
+      m |= (((z >> 7) & 1u) | ((z >> 14) & 2u) | ((z >> 21) & 4u) | ((z >> 28) & 8u)) << (4 * i);
+    }
+    return m;
+  }
+  for (uint64_t k = 0; q + k < n; k++) m |= (uint32_t)(p[q + k] == '\n') << k;
+  return m;
+}
+
+// exclusive prefix sum of v over the LS_T threads of the block; *total = the block's sum
+__device__ __forceinline__ uint32_t block_prefix(uint32_t v, uint32_t *total) {
+  __shared__ uint32_t warp_sum[LS_T / 32];
+  const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (unsigned o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sum[w] = x;
+  __syncthreads();
+  uint32_t before = 0, all = 0;
+  for (unsigned k = 0; k < LS_T / 32; k++) {
+    const uint32_t t = warp_sum[k];
+    if (k < w) before += t;
+    all += t;
+  }
+  *total = all;
+  return before + x - v;
+}
+
+__global__ void __launch_bounds__(LS_T) line_count_kernel(const uint8_t *__restrict__ p, uint64_t n,
+                                                          unsigned long long *__restrict__ tile_nl) {
+  const uint64_t q = ((uint64_t)blockIdx.x * LS_T + threadIdx.x) * 16;
+  uint32_t total;
+  block_prefix(q < n ? (uint32_t)__popc(newline_bits(p, q, n)) : 0u, &total);
+  if (threadIdx.x == 0) tile_nl[blockIdx.x] = total;
+}
+
+// offs[0] = 0, offs[1 + k] = the byte behind the k-th '\n', offs[n_nl + 1] = n when the piece does not end with '\n'
+__global__ void __launch_bounds__(LS_T) line_write_kernel(const uint8_t *__restrict__ p, uint64_t n,
+                                                          const unsigned long long *__restrict__ tile_base,
+                                                          const unsigned long long *__restrict__ n_nl,
+                                                          unsigned long long *__restrict__ offs) {
+  const uint64_t q = ((uint64_t)blockIdx.x * LS_T + threadIdx.x) * 16;
+  uint32_t m = q < n ? newline_bits(p, q, n) : 0u, total;
+  uint64_t at = tile_base[blockIdx.x] + block_prefix((uint32_t)__popc(m), &total);
+  while (m) {
+    offs[1 + at++] = q + (uint32_t)(__ffs((int)m) - 1) + 1;
+    m &= m - 1;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    offs[0] = 0;
+    if (n && p[n - 1] != '\n') offs[*n_nl + 1] = n;
+  }
+}
+
+__global__ void __launch_bounds__(256) narrow_ids_kernel(const int32_t *__restrict__ ids, uint64_t n,
+                                                         uint16_t *__restrict__ out) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = (uint16_t)ids[i];
+}
+
+__device__ __forceinline__ uint32_t decimal_len(uint32_t v) {
+  uint32_t d = 1;
+  for (uint64_t t = 10; v >= t; t *= 10) d++;
+  return d;
+}
+
+// line_bytes[s] = bytes of line s in the text form (off: chunk-local id offsets of the lines, n_lines + 1)
+__global__ void __launch_bounds__(256) text_count_kernel(const int32_t *__restrict__ ids,
+                                                         const unsigned long long *__restrict__ off, uint64_t n_lines,
+                                                         unsigned long long *__restrict__ line_bytes) {
+  const unsigned lane = threadIdx.x & 31;
+  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t s = warp; s < n_lines; s += nwarps) {
+    unsigned long long sum = 0;
+    for (uint64_t j = off[s] + lane, hi = off[s + 1]; j < hi; j += 32) sum += decimal_len((uint32_t)ids[j]) + 1;
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (lane == 0) line_bytes[s] = sum + 1;
+  }
+}
+
+__global__ void __launch_bounds__(256) text_emit_kernel(const int32_t *__restrict__ ids,
+                                                        const unsigned long long *__restrict__ off, uint64_t n_lines,
+                                                        const unsigned long long *__restrict__ line_start,
+                                                        uint8_t *__restrict__ out) {
+  const unsigned lane = threadIdx.x & 31;
+  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t s = warp; s < n_lines; s += nwarps) {
+    uint64_t pos = line_start[s];
+    for (uint64_t j0 = off[s], hi = off[s + 1]; j0 < hi; j0 += 32) {  // warp-uniform
+      const uint64_t j = j0 + lane;
+      uint32_t v = 0, len = 0;
+      if (j < hi) {
+        v = (uint32_t)ids[j];
+        len = decimal_len(v) + 1;
+      }
+      uint32_t incl = len;
+#pragma unroll
+      for (unsigned o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+      }
+      if (len) {
+        uint8_t *dst = out + pos + incl - len;
+        dst[len - 1] = ' ';
+        for (uint32_t k = len - 1; k-- > 0; v /= 10) dst[k] = (uint8_t)('0' + v % 10);
+      }
+      pos += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (lane == 0) out[pos] = '\n';
+  }
+}
+
+unsigned warp_blocks(yttm_ctx *c, uint64_t n_warps) {  // blocks of 256 threads for one warp per item
+  return (unsigned)std::max<uint64_t>(std::min<uint64_t>((n_warps + 7) / 8, (uint64_t)c->n_sm * 8), 1);
+}
+
+}  // namespace
+
+struct yttm_enc_stream {
+  yttm_enc *e = nullptr;
+  int bos = 0, eos = 0, reverse = 0, format = YTTM_STREAM_IDS32;
+  double dropout = 0;
+  uint64_t seed = 0, first = 0;
+  yttm_enc_sink sink = nullptr;
+  void *user = nullptr;
+  uint64_t piece = 0;                       // nominal piece bytes
+  uint8_t *stage[2] = {nullptr, nullptr};   // pinned staging of the fed bytes: piece i is copied in from stage[i & 1]
+  uint64_t stage_cap[2] = {0, 0};
+  int cur = 0;                              // staging buffer being filled
+  uint64_t len = 0, nonl = 0;               // its bytes; its first bytes known to hold no '\n'
+  uint8_t *out[2] = {nullptr, nullptr};     // pinned results of the piece in slot s: data, then its line ends
+  uint64_t out_cap[2] = {0, 0};
+  struct Piece {
+    uint64_t n_bytes = 0, n_lines = 0, n_out = 0;
+    bool open_end = false;                  // the last line has no '\n' (the end of the stream)
+  } pc[2];
+  int to_encode = -1, to_deliver = -1;      // slot copied in, not yet encoded; slot copied out, not yet given to the sink
+  ytc::DevBuf tiles[2], fmt[2], lines_buf[2];  // per slot: '\n' per tile + bases; 16-bit ids or text; text per line
+  uint64_t lines = 0, ids = 0, bytes_in = 0;
+};
+
+void yttm_enc_stream_free(yttm_enc_stream *s) {
+  if (!s) return;
+  yttm_enc *e = s->e;
+  cudaStreamSynchronize(e->ctx->stream);
+  cudaStreamSynchronize(e->s_in);
+  cudaStreamSynchronize(e->s_out);
+  for (int i = 0; i < 2; i++) {
+    if (s->stage[i]) cudaFreeHost(s->stage[i]);
+    if (s->out[i]) cudaFreeHost(s->out[i]);
+    s->tiles[i].release();
+    s->fmt[i].release();
+    s->lines_buf[i].release();
+  }
+  e->stream = nullptr;
+  delete s;
+}
+
+namespace {
+
+// pinned host buffer *p of at least `need` bytes, its first `keep` bytes kept (it must not be in flight)
+int pinned_reserve(yttm_ctx *c, uint8_t **p, uint64_t *cap, uint64_t need, uint64_t keep) {
+  if (need <= *cap) return 0;
+  const uint64_t want = std::max(need + need / 8, 2 * *cap);
+  void *q = nullptr;
+  YT_CUDA(c, cudaHostAlloc(&q, want, cudaHostAllocDefault));
+  if (keep) std::memcpy(q, *p, keep);
+  if (*p) YT_CUDA(c, cudaFreeHost(*p));
+  *p = static_cast<uint8_t *>(q);
+  *cap = want;
+  return 0;
+}
+
+// "stream_dev_peak_bytes": every device buffer of the encoder, sampled after each piece
+void note_stream_peak(yttm_enc *e) {
+  uint64_t sum = e->cp2id.cap + e->rules.cap + e->sub_table.cap;
+  for (auto &sl : e->slot) sl.each([&](ytc::DevBuf *b) { sum += b->cap; });
+  for (int i = 0; i < 2; i++) sum += e->stream->tiles[i].cap + e->stream->fmt[i].cap + e->stream->lines_buf[i].cap;
+  e->ctx->enc_stream_peak = std::max(e->ctx->enc_stream_peak, (double)sum);
+}
+
+// The kernels of the piece in slot s, then its copy out (line ends after the data, 8-byte aligned).
+int stream_encode(yttm_enc *e, int s) {
+  yttm_ctx *c = e->ctx;
+  yttm_enc_stream *S = e->stream;
+  yttm_enc_stream::Piece &P = S->pc[s];
+  yttm_enc::Slot &sl = e->slot[s];
+  const uint8_t *d = sl.d_bytes.as<uint8_t>();
+  const uint64_t n = P.n_bytes, nt = (n + LS_TILE - 1) / LS_TILE;
+  YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_in[s], 0));
+  YT_CUDA(c, S->tiles[s].reserve((2 * nt + 2) * 8));
+  unsigned long long *tile_nl = S->tiles[s].as<unsigned long long>(), *tile_base = tile_nl + nt, *n_nl = tile_base + nt;
+  ytc::timer_begin(c, "stream_lines");
+  line_count_kernel<<<(unsigned)nt, LS_T, 0, c->stream>>>(d, n, tile_nl);
+  c->launches++;
+  if (yttm_device_scan_u64(c, tile_nl, nt, tile_base, n_nl)) return 1;
+  unsigned long long h_nl = 0;
+  YT_CUDA(c, cudaMemcpyAsync(&h_nl, n_nl, 8, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  P.n_lines = h_nl + (P.open_end ? 1 : 0);
+  YT_CUDA(c, sl.d_offs.reserve((P.n_lines + 2) * 8));
+  line_write_kernel<<<(unsigned)nt, LS_T, 0, c->stream>>>(d, n, tile_base, n_nl, sl.d_offs.as<unsigned long long>());
+  c->launches++;
+  ytc::timer_end(c, "stream_lines");
+  uint64_t n_ids = 0;
+  if (enc_device(e, &sl, d, sl.d_offs.as<uint64_t>(), n, P.n_lines, S->bos, S->eos, S->reverse, S->dropout, S->seed,
+                 S->first + S->lines, &n_ids))
+    return 1;
+  const int32_t *ids = sl.out_ids.as<int32_t>();
+  unsigned long long *id_off = sl.out_off.as<unsigned long long>();
+  const void *data = ids;
+  P.n_out = n_ids * 4;
+  ytc::timer_begin(c, "stream_format");
+  if (S->format == YTTM_STREAM_IDS16) {
+    YT_CUDA(c, S->fmt[s].reserve(n_ids * 2 + 16));
+    const uint64_t blocks = std::max<uint64_t>(std::min<uint64_t>((n_ids + 255) / 256, (uint64_t)c->n_sm * 8), 1);
+    narrow_ids_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(ids, n_ids, S->fmt[s].as<uint16_t>());
+    c->launches++;
+    data = S->fmt[s].p;
+    P.n_out = n_ids * 2;
+  } else if (S->format == YTTM_STREAM_TEXT) {
+    YT_CUDA(c, S->lines_buf[s].reserve((2 * P.n_lines + 2) * 8));
+    unsigned long long *lb = S->lines_buf[s].as<unsigned long long>(), *ls = lb + P.n_lines, *tot = ls + P.n_lines;
+    text_count_kernel<<<warp_blocks(c, P.n_lines), 256, 0, c->stream>>>(ids, id_off, P.n_lines, lb);
+    c->launches++;
+    if (yttm_device_scan_u64(c, lb, P.n_lines, ls, tot)) return 1;
+    unsigned long long text_bytes = 0;
+    YT_CUDA(c, cudaMemcpyAsync(&text_bytes, tot, 8, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    YT_CUDA(c, S->fmt[s].reserve(text_bytes + 16));
+    text_emit_kernel<<<warp_blocks(c, P.n_lines), 256, 0, c->stream>>>(ids, id_off, P.n_lines, ls, S->fmt[s].as<uint8_t>());
+    c->launches++;
+    data = S->fmt[s].p;
+    P.n_out = text_bytes;
+  }
+  if (S->ids)
+    add_base_kernel<<<(unsigned)std::max<uint64_t>(std::min<uint64_t>((P.n_lines + 255) / 256, (uint64_t)c->n_sm * 4), 1),
+                      256, 0, c->stream>>>(id_off + 1, P.n_lines, (unsigned long long)S->ids);
+  c->launches += S->ids ? 1 : 0;
+  ytc::timer_end(c, "stream_format");
+  YT_CUDA(c, cudaGetLastError());
+  YT_CUDA(c, cudaEventRecord(e->ev_done[s], c->stream));
+  const uint64_t ends_at = (P.n_out + 7) & ~7ull;
+  if (pinned_reserve(c, &S->out[s], &S->out_cap[s], ends_at + P.n_lines * 8, 0)) return 1;
+  YT_CUDA(c, cudaStreamWaitEvent(e->s_out, e->ev_done[s], 0));
+  if (P.n_out) YT_CUDA(c, cudaMemcpyAsync(S->out[s], data, P.n_out, cudaMemcpyDeviceToHost, e->s_out));
+  YT_CUDA(c, cudaMemcpyAsync(S->out[s] + ends_at, id_off + 1, P.n_lines * 8, cudaMemcpyDeviceToHost, e->s_out));
+  YT_CUDA(c, cudaEventRecord(e->ev_out[s], e->s_out));
+  S->lines += P.n_lines;
+  S->ids += n_ids;
+  c->enc_stream_pieces += 1;
+  note_stream_peak(e);
+  return 0;
+}
+
+// The results of the piece in slot s to the sink, once their copy out has completed.
+int stream_deliver(yttm_enc *e, int s) {
+  yttm_ctx *c = e->ctx;
+  yttm_enc_stream *S = e->stream;
+  const yttm_enc_stream::Piece &P = S->pc[s];
+  YT_CUDA(c, cudaEventSynchronize(e->ev_out[s]));
+  const int rc = S->sink(S->user, S->out[s], P.n_out, reinterpret_cast<const uint64_t *>(S->out[s] + ((P.n_out + 7) & ~7ull)),
+                         P.n_lines);
+  if (rc) YT_FAIL(c, "yttm_enc_stream: the sink failed (it returned " + std::to_string(rc) + ")");
+  return 0;
+}
+
+// Staging buffer cur holds a piece in its first `cut` bytes: copy it in (slot cur), move what follows to the other
+// staging buffer, encode the piece before it and hand the one before that to the sink.
+int stream_submit(yttm_enc *e, uint64_t cut) {
+  yttm_ctx *c = e->ctx;
+  yttm_enc_stream *S = e->stream;
+  const int s = S->cur, o = s ^ 1;
+  const uint64_t tail = S->len - cut;
+  YT_CUDA(c, cudaEventSynchronize(e->ev_in[o]));  // the piece before has been copied in from staging buffer o
+  if (pinned_reserve(c, &S->stage[o], &S->stage_cap[o], std::max(tail, S->piece), 0)) return 1;
+  if (tail) std::memcpy(S->stage[o], S->stage[s] + cut, tail);
+  yttm_enc::Slot &sl = e->slot[s];
+  if (cut + 16 > sl.d_bytes.cap) YT_CUDA(c, cudaEventSynchronize(e->ev_done[s]));  // replaced: the kernels of piece i-2 are done with it
+  YT_CUDA(c, sl.d_bytes.reserve(cut + 16));
+  YT_CUDA(c, cudaStreamWaitEvent(e->s_in, e->ev_done[s], 0));
+  YT_CUDA(c, cudaMemcpyAsync(sl.d_bytes.p, S->stage[s], cut, cudaMemcpyHostToDevice, e->s_in));
+  YT_CUDA(c, cudaEventRecord(e->ev_in[s], e->s_in));
+  S->pc[s].n_bytes = cut;
+  S->pc[s].open_end = S->stage[s][cut - 1] != '\n';
+  if (S->to_encode >= 0 && stream_encode(e, S->to_encode)) return 1;
+  if (S->to_deliver >= 0 && stream_deliver(e, S->to_deliver)) return 1;
+  S->to_deliver = S->to_encode;
+  S->to_encode = s;
+  S->cur = o;
+  S->len = S->nonl = tail;  // what follows the last '\n' holds none
+  return 0;
+}
+
+int stream_feed(yttm_enc *e, const char *bytes, uint64_t n) {
+  yttm_ctx *c = e->ctx;
+  yttm_enc_stream *S = e->stream;
+  YT_CUDA(c, cudaSetDevice(c->device));
+  while (n) {
+    const uint64_t room = S->len < S->piece ? S->piece - S->len : S->piece;
+    const uint64_t take = std::min(n, room);
+    if (pinned_reserve(c, &S->stage[S->cur], &S->stage_cap[S->cur], S->len + take, S->len)) return 1;
+    std::memcpy(S->stage[S->cur] + S->len, bytes, take);
+    S->len += take;
+    S->bytes_in += take;
+    bytes += take;
+    n -= take;
+    if (S->len < S->piece) continue;
+    const void *nl = memrchr(S->stage[S->cur] + S->nonl, '\n', S->len - S->nonl);
+    if (!nl) { S->nonl = S->len; continue; }  // no '\n' yet: the piece grows until one comes
+    if (stream_submit(e, (uint64_t)(static_cast<const uint8_t *>(nl) - S->stage[S->cur]) + 1)) return 1;
+  }
+  return 0;
+}
+
+int stream_end(yttm_enc *e) {
+  yttm_ctx *c = e->ctx;
+  yttm_enc_stream *S = e->stream;
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (S->len && stream_submit(e, S->len)) return 1;  // the last piece ends with the stream
+  const int last = S->to_encode;
+  if (last >= 0 && stream_encode(e, last)) return 1;
+  if (S->to_deliver >= 0 && stream_deliver(e, S->to_deliver)) return 1;
+  if (last >= 0 && stream_deliver(e, last)) return 1;
+  return 0;
+}
+
+// a failed stream call: the stream is closed, the error kept
+int stream_failed(yttm_enc *e) {
+  const std::string err = e->ctx->err;
+  yttm_enc_stream_free(e->stream);
+  cudaGetLastError();
+  e->ctx->err = err;
+  return 1;
+}
+
+}  // namespace
+
+extern "C" {
+
+int yttm_enc_stream_begin(yttm_enc *e, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                          uint64_t first_sentence_index, int format, yttm_enc_sink sink, void *user) {
+  if (yttm_enc_check(e, "yttm_enc_stream_begin", bos, eos)) return 1;
+  yttm_ctx *c = e->ctx;
+  if (format != YTTM_STREAM_IDS16 && format != YTTM_STREAM_IDS32 && format != YTTM_STREAM_TEXT)
+    YT_FAIL(c, "yttm_enc_stream_begin: format must be YTTM_STREAM_IDS16, YTTM_STREAM_IDS32 or YTTM_STREAM_TEXT");
+  if (!sink) YT_FAIL(c, "yttm_enc_stream_begin: no sink");
+  if (format == YTTM_STREAM_IDS16 && e->vocab > 65536)
+    YT_FAIL(c, "yttm_enc_stream_begin: 16-bit ids need a vocabulary of at most 65536 (this model has " +
+                   std::to_string(e->vocab) + ")");
+  if (pipe_init(e)) return 1;
+  yttm_enc_stream *S = new yttm_enc_stream();
+  S->e = e;
+  S->bos = bos; S->eos = eos; S->reverse = reverse; S->dropout = dropout; S->seed = seed;
+  S->first = first_sentence_index; S->format = format; S->sink = sink; S->user = user;
+  S->piece = (uint64_t)ytc::env_int("YTTM_ENC_STREAM_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;
+  e->stream = S;
+  c->enc_stream_pieces = 0;
+  c->enc_stream_peak = 0;
+  return 0;
+}
+
+int yttm_enc_stream_feed(yttm_enc *e, const char *bytes, uint64_t n) {
+  if (!e) return yttm_enc_check(e, "yttm_enc_stream_feed", 0, 0);
+  if (!e->stream) YT_FAIL(e->ctx, "yttm_enc_stream_feed: yttm_enc_stream_begin has not run");
+  return stream_feed(e, bytes, n) ? stream_failed(e) : 0;
+}
+
+int yttm_enc_stream_end(yttm_enc *e, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes_in) {
+  if (!e) return yttm_enc_check(e, "yttm_enc_stream_end", 0, 0);
+  if (!e->stream) YT_FAIL(e->ctx, "yttm_enc_stream_end: yttm_enc_stream_begin has not run");
+  if (stream_end(e)) return stream_failed(e);
+  if (n_lines) *n_lines = e->stream->lines;
+  if (n_ids) *n_ids = e->stream->ids;
+  if (n_bytes_in) *n_bytes_in = e->stream->bytes_in;
+  yttm_enc_stream_free(e->stream);
+  return 0;
+}
+
 }  // extern "C"

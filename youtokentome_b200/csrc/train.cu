@@ -1035,6 +1035,8 @@ double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
   if (!std::strcmp(stage, "loop_iters")) return (double)c->loop_iters;
   if (!std::strcmp(stage, "xq_round")) return (double)c->loop_xq_round;   // exchange rounds of the context so far
   if (!std::strcmp(stage, "enc_chunks")) return c->enc_chunks;
+  if (!std::strcmp(stage, "stream_pieces")) return c->enc_stream_pieces;
+  if (!std::strcmp(stage, "stream_dev_peak_bytes")) return c->enc_stream_peak;
   if (!std::strcmp(stage, "loop_refreshes")) return (double)c->loop_sweeps;
   if (!std::strcmp(stage, "loop_launches")) return (double)c->loop_relaunches;
   if (!std::strcmp(stage, "table_capacity")) return (double)c->pcap;

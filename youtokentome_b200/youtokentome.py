@@ -3,9 +3,11 @@ youtokentome/cpp/yttm.pyx:52-181) over the CUDA library: same class, method name
 meaning, return types and exceptions (ValueError(status.message), TypeError for bad argument
 types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path, optionally with the source byte
 span of every id), `encode_padded` (the same ids as padded, truncated [N, L] rows with their lengths),
-`encode_subwords_packed` (the subword pieces on the GPU), `decode_packed` (the inverse of
-`encode_packed`, on the GPU) and `dropout_seed`."""
+`encode_subwords_packed` (the subword pieces on the GPU), `encode_file` (a file of any size, line by line, to .npy files
+or the CLI's text), `decode_packed` (the inverse of `encode_packed`, on the GPU) and `dropout_seed`."""
 import ctypes as C
+import os
+import sys
 import threading
 from collections.abc import Collection
 from enum import Enum
@@ -470,6 +472,45 @@ class BPE:
         if xp is np:
             return np.ascontiguousarray(np.where(big, -1, ids).astype(np.int32)), [-1]
         return torch.where(big, torch.full_like(ids, -1), ids).to(torch.int32).contiguous(), [-1]
+
+    def encode_file(self, input, output, bos=False, eos=False, reverse=False, dropout_prob=0.0, text=False) -> dict:
+        """Encodes a text file of any size on the GPU, line by line: a line ends at "\\n" and nowhere else, the text
+        after the last "\\n" (if any) is a last line, and line i gets the ids encode_packed gives it without its
+        "\\n".  Lines are the next sentences of the dropout stream, as for encode_packed.  `input`: a path, an int file
+        descriptor or an object with fileno() (sys.stdin.buffer, a pipe), read to its end.  Writes
+          text=False  <output>.ids.npy (1-D uint16 when vocab_size() <= 65536, else int32) and <output>.offsets.npy
+                      (uint64, lines + 1 values from 0: line i = ids[offsets[i]:offsets[i+1]]), both loadable with
+                      np.load(..., mmap_mode="r");
+          text=True   the text of `yttm encode --output_type id` (every id and one space, "\\n" per line) to
+                      <output>, or to stdout when output is "-".
+        A failed call leaves nothing at the output names.  Returns {"lines", "ids", "bytes"} (bytes read)."""
+        _check_dropout(dropout_prob)
+        output = os.fspath(output)
+        opened = None
+        if isinstance(input, (str, bytes, os.PathLike)):
+            try:
+                fd = opened = os.open(input, os.O_RDONLY | getattr(os, "O_CLOEXEC", 0))
+            except OSError as e:
+                raise ValueError("encode_file: cannot open '%s': %s" % (os.fsdecode(input), e.strerror)) from None
+        elif isinstance(input, int) and not isinstance(input, bool):
+            fd = input
+        elif hasattr(input, "fileno"):
+            fd = input.fileno()
+        else:
+            raise TypeError("input must be a path, a file descriptor or an object with fileno(), not %s" %
+                            type(input).__name__)
+        stats = np.zeros(3, dtype=np.uint64)
+        try:
+            if text and output == "-":
+                sys.stdout.flush()
+            rc = _lib.lib().yttm_api_encode_file(self._h, fd, os.fsencode(output), int(text), int(bos), int(eos),
+                                                 int(reverse), float(dropout_prob), stats.ctypes.data)
+        finally:
+            if opened is not None:
+                os.close(opened)
+        if rc != 0:
+            raise self._err()
+        return {"lines": int(stats[0]), "ids": int(stats[1]), "bytes": int(stats[2])}
 
     # -- BPE-dropout stream ---------------------------------------------------------------------
     def dropout_seed(self, seed: int):

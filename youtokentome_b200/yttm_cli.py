@@ -1,6 +1,8 @@
-"""`yttm bpe | encode | decode | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
+"""`yttm bpe | encode | encode_file | decode | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
 same sub-commands, option names, defaults and stdin/stdout framing) over the CUDA library.
 Run as `python -m youtokentome_b200.yttm_cli ...`.  `--n_threads` is accepted and ignored."""
+import sys
+
 import click
 
 from .youtokentome import BPE
@@ -43,6 +45,24 @@ def encode(model, output_type, n_threads, bos, eos, reverse, stream, dropout_pro
     if n_threads < -1 or n_threads == 0:
         raise ValueError('Invalid value for "--n_threads": must be -1 or positive integer, not "%d"' % n_threads)
     BPE(model, n_threads).encode_cli(output_type, stream, bos, eos, reverse, dropout_prob)
+
+
+@main.command("encode_file")
+@click.option("--model", type=click.Path(exists=True), required=True, help="Path to file with learned model.")
+@click.option("--input", "input_", type=click.STRING, required=True, help="Text file to encode, '-' for stdin.")
+@click.option("--output", type=click.STRING, required=True,
+              help="Prefix of <output>.ids.npy and <output>.offsets.npy; with --text the output file, '-' for stdout.")
+@click.option("--text", is_flag=True, help="Write the ids as text, as `encode --output_type id` does.")
+@click.option("--bos", is_flag=True, help="Add tab 'begin of sentence'.")
+@click.option("--eos", is_flag=True, help="Add tab 'end of sentence'.")
+@click.option("--reverse", is_flag=True, help="Reverse output sequence of tokens.")
+@click.option("--dropout_prob", type=click.FLOAT, default=0, show_default=True,
+              help="BPE-dropout probability (the probability of a merge being dropped)")
+def encode_file(model, input_, output, text, bos, eos, reverse, dropout_prob):
+    """Encode a text file of any size on the GPU, line by line."""
+    src = sys.stdin.buffer if input_ == "-" else input_
+    r = BPE(model).encode_file(src, output, bos=bos, eos=eos, reverse=reverse, dropout_prob=dropout_prob, text=text)
+    click.echo("encode_file: %d lines, %d ids, %d bytes" % (r["lines"], r["ids"], r["bytes"]), err=True)
 
 
 def _ignore_ids(ctx, param, value):
