@@ -157,11 +157,13 @@ __device__ __forceinline__ bool find_before(const uint8_t *b, const uint32_t *sb
 
 // Stages the piece [pa, pa + FIND_TILE) of the group [gstart, gend), FIND_HALO bytes on either side (the address of
 // batch byte pa is 16-byte aligned), and the bitmap of the sentence starts among them; returns the word starts among
-// the thread's FIND_BPT bytes (bit j = batch byte pa + FIND_BPT * threadIdx.x + j).  Starts with a barrier: the
-// previous piece is done with the buffers.
+// the thread's FIND_BPT bytes (bit j = batch byte pa + FIND_BPT * threadIdx.x + j).  s_end[threadIdx.x] gets the word
+// ENDS among the same bytes: the first byte of a space unit, or a sentence start (the end of the sentence before it);
+// a word of the group ends at the first of them after its start (the group's end is a sentence start of the bitmap).
+// Starts with a barrier: the previous piece is done with the buffers.
 __device__ __forceinline__ uint64_t find_piece(const uint8_t *bytes, int64_t n_total, int64_t pa, int64_t gstart,
                                                int64_t gend, const uint32_t *s_off, uint32_t ng, uint4 *s_buf,
-                                               uint32_t *s_sb) {
+                                               uint32_t *s_sb, uint64_t *s_end) {
   constexpr int NCH = FIND_BUF / 16, PER = (NCH + FIND_T - 1) / FIND_T;
   const int64_t p0 = pa - FIND_HALO;  // batch position of staged byte 0
   const int tid = (int)threadIdx.x;
@@ -200,9 +202,11 @@ __device__ __forceinline__ uint64_t find_piece(const uint8_t *bytes, int64_t n_t
   const int64_t lo = pa + FIND_BPT * (int64_t)tid;  // batch position of the thread's first byte
   const int64_t b = gstart - lo, e = gend - lo;    // the group's bytes among the thread's: [bb, ee)
   const int bb = b < 0 ? 0 : b > FIND_BPT ? FIND_BPT : (int)b, ee = e < 0 ? 0 : e > FIND_BPT ? FIND_BPT : (int)e;
-  if (ee <= bb) return 0;
-  const uint64_t inside = (ee - bb == 64 ? ~0ull : (1ull << (ee - bb)) - 1) << bb;
   const int i0 = FIND_HALO + FIND_BPT * tid;  // staged index of the thread's first byte
+  const uint32_t *sw = s_sb + (i0 >> 5);
+  const uint64_t starts = (uint64_t)(sw[0] >> 16) | ((uint64_t)sw[1] << 16) | ((uint64_t)sw[2] << 48);  // sentences
+  if (ee <= bb) { s_end[tid] = starts; return 0; }
+  const uint64_t inside = (ee - bb == 64 ? ~0ull : (1ull << (ee - bb)) - 1) << bb;
   const uint32_t prev = reinterpret_cast<const uint32_t *>(s_buf)[i0 / 4 - 1];
   uint32_t e2 = swar_eq(prev, 0xe2e2e2e2u);
   uint64_t sp = 0;
@@ -216,24 +220,42 @@ __device__ __forceinline__ uint64_t find_piece(const uint8_t *bytes, int64_t n_t
   if (!(e2 & 0x80808080u)) {
     // no 0xE2 from four bytes before on, so no U+2581 touches these bytes: a word starts where a sentence starts or an
     // ASCII space is followed by a non-space byte
-    const uint32_t *sw = s_sb + (i0 >> 5);
-    const uint64_t starts = (uint64_t)(sw[0] >> 16) | ((uint64_t)sw[1] << 16) | ((uint64_t)sw[2] << 48);
+    s_end[tid] = starts | sp;
     return (starts | (sp << 1) | (swar_space(prev) >> 31)) & ~sp & inside;
   }
   const uint8_t *sbyte = reinterpret_cast<const uint8_t *>(s_buf);
-  uint64_t f = 0;
-  for (int j = bb; j < ee; j++)
-    if (find_before(sbyte, s_sb, i0 + j) && !find_at(sbyte, s_sb, i0 + j)) f |= 1ull << j;
+  uint64_t f = 0, ends = starts;
+  for (int j = bb; j < ee; j++) {
+    const bool at = find_at(sbyte, s_sb, i0 + j);
+    if (at) ends |= 1ull << j;
+    else if (find_before(sbyte, s_sb, i0 + j)) f |= 1ull << j;
+  }
+  s_end[tid] = ends;
   return f;
 }
 
+// Length of the word that starts at bit j of the thread's bytes in piece [pa, pa + FIND_TILE) of a group that ends at
+// gend (gend_in: the group ends in this piece), from the ends of find_piece; WORD_LEN_ESC when its end lies beyond the
+// piece or it is that long.
+constexpr uint16_t WORD_LEN_ESC = 0xffff;
+__device__ __forceinline__ uint16_t find_word_len(const uint64_t *s_end, int64_t pa, int j, bool gend_in, int64_t gend) {
+  int t = (int)threadIdx.x;
+  uint64_t m = s_end[t] & (~1ull << j);  // ends after the start (a sentence start at the word's start is its own)
+  while (!m && ++t < FIND_T) m = s_end[t];
+  const int64_t end = m ? pa + FIND_BPT * (int64_t)t + find_low64(m) : gend_in ? gend : -1;
+  const int64_t len = end - (pa + FIND_BPT * (int64_t)threadIdx.x + j);
+  return end < 0 || len >= WORD_LEN_ESC ? WORD_LEN_ESC : (uint16_t)len;
+}
+
 // (4 blocks of 256 threads per SM, the occupancy it is built for: 2 x 16 KB of staged bytes per SM in flight)
-__global__ void __launch_bounds__(FIND_T, 4) find_words_vec_kernel(EncArgs a, uint32_t G) {
+// word_len: per work item, bytes up to the word's end (find_word_len), WORD_LEN_ESC if not known
+__global__ void __launch_bounds__(FIND_T, 4) find_words_vec_kernel(EncArgs a, uint32_t G, uint16_t *word_len) {
   __shared__ uint4 s_buf[FIND_BUF / 16];
   __shared__ uint32_t s_sb[FIND_BUF / 32 + 1];
   __shared__ uint32_t s_off[FIND_GMAX + 1];  // the group's sentence starts (batch positions), s_off[ng] = its end
   __shared__ uint32_t s_wb[FIND_GMAX + 1];   // words of the group in front of them
   __shared__ uint32_t s_red[FIND_T / 32];
+  __shared__ uint64_t s_end[FIND_T];         // the word ends among each thread's bytes (find_piece)
   __shared__ unsigned long long s_base;
   constexpr int64_t FAR = (int64_t)1 << 62;
   const int tid = (int)threadIdx.x;
@@ -252,7 +274,7 @@ __global__ void __launch_bounds__(FIND_T, 4) find_words_vec_kernel(EncArgs a, ui
     if (np > 1) {  // a group longer than a piece: count, then reserve before the write pass
       uint32_t total = 0;
       for (uint32_t k = 0; k < np; k++) {
-        const uint64_t m = find_piece(a.bytes, n_total, a0 + (int64_t)k * FIND_TILE, gstart, gend, s_off, ng, s_buf, s_sb);
+        const uint64_t m = find_piece(a.bytes, n_total, a0 + (int64_t)k * FIND_TILE, gstart, gend, s_off, ng, s_buf, s_sb, s_end);
         long_block_scan_sum(find_popc64(m), s_red, &tot);
         total += tot;
       }
@@ -261,7 +283,7 @@ __global__ void __launch_bounds__(FIND_T, 4) find_words_vec_kernel(EncArgs a, ui
     uint32_t run = 0;  // words of the group in the earlier pieces
     for (uint32_t k = 0; k < np; k++) {
       const int64_t pa = a0 + (int64_t)k * FIND_TILE;
-      uint64_t m = find_piece(a.bytes, n_total, pa, gstart, gend, s_off, ng, s_buf, s_sb);
+      uint64_t m = find_piece(a.bytes, n_total, pa, gstart, gend, s_off, ng, s_buf, s_sb, s_end);
       uint32_t n = run + long_block_scan_sum(find_popc64(m), s_red, &tot);  // words of the group before mine
       if (np == 1) {
         if (tid == 0) s_base = tot ? atomicAdd(a.n_words, (unsigned long long)tot) : 0ull;
@@ -284,6 +306,7 @@ __global__ void __launch_bounds__(FIND_T, 4) find_words_vec_kernel(EncArgs a, ui
         if (!m) break;
         a.word_pos[base + n] = (uint32_t)p;
         a.word_sent[base + n] = (uint32_t)(g + i - 1);
+        word_len[base + n] = find_word_len(s_end, pa, (int)(p - lo), k + 1 == np, gend);
         n++;
         m &= m - 1;
       }
@@ -510,22 +533,39 @@ __global__ void __launch_bounds__(LONG_T) encode_long_words_kernel(EncArgs a, Lo
 // first byte of a space unit (never a continuation byte), INVALID_CP with length 1 in both cases (decode_unit), so
 // nothing outside the word enters.  Natural text repeats its words (the bench batch: 20 M occurrences of < 200 k
 // words), and the merge loop of encode_word is the expensive part of encoding a word.  Three launches:
-//   dedup_words_kernel       one thread per occurrence: end of the word + 64-bit hash of its bytes; an
-//                            open-addressed table of (32-bit tag, work item) words, small enough to stay in L2, elects
-//                            the first occurrence that claims a slot as the word's representative; later occurrences
-//                            with the same tag compare BYTES with it (exactness never rests on the hash).  A word that
-//                            finds neither itself nor a free slot within DEDUP_PROBES probes represents itself, so the
-//                            table is a bounded cache, not a limit.
+//   dedup_words_kernel       one thread per occurrence: the word's bytes (its length comes from the finder) + 64-bit
+//                            hash of them; an open-addressed table of 16-byte slots (32-bit tag, work item, position,
+//                            length), small enough to stay in L2, elects the first occurrence that claims a slot as the
+//                            word's representative; later occurrences with the same tag and length compare BYTES with
+//                            the slot's position (exactness never rests on the hash).  A word that finds neither itself
+//                            nor a free slot within DEDUP_PROBES probes represents itself, so the table is a bounded
+//                            cache, not a limit.
 //   encode_rep_words_kernel  the per-word body, over the representatives only (list length read on the device);
 //                            representatives of more than LONG_W slots go to the list of encode_long_words_kernel
 //   encode_long_words_kernel a block per long representative
 // emit_ids_kernel then copies the ids of a representative (its record, or its slots) to every occurrence.  The slot of the first token of work
 // item w is word_pos[w] + 3 word_sent[w] + 1 (sent_base(): the sentence start cancels), so a copy needs no sentence
 // offsets.
-constexpr unsigned long long DEDUP_EMPTY = ~0ull;
+// A slot is claimed with one 16-byte atomicCAS and never written again in the launch.  A plain 16-byte load may see
+// any of its four words before or after the claim, so a free slot is all ones in every word: no word of a claimed slot
+// but its tag can be all ones (item < n_words, pos + len <= n_bytes < 2^32 - 16), and a load that finds an all-ones
+// word asks the atomic (which returns the whole slot) instead of trusting the rest.
+struct alignas(16) DedupSlot { uint32_t tag, item, pos, len; };
+// Claims slot p for `mine` if it is free and returns what it held before: one 16-byte atomicCAS.  The SIMT emulator
+// (YT_SIMT_EMU) runs the blocks of a launch one after another on one host thread and switches threads only at
+// collectives, so there a plain compare and store is the same operation.
+__device__ __forceinline__ DedupSlot dd_claim(DedupSlot *p, DedupSlot mine) {
+#ifndef YT_SIMT_EMU
+  return atomicCAS(p, DedupSlot{~0u, ~0u, ~0u, ~0u}, mine);
+#else
+  const DedupSlot cur = *p;
+  if ((cur.tag & cur.item & cur.pos & cur.len) == ~0u) *p = mine;
+  return cur;
+#endif
+}
 constexpr uint32_t DEDUP_PROBES = 8;
 struct DedupArgs {
-  unsigned long long *tab;     // (tag << 32) | representative work item ; DEDUP_EMPTY = free
+  DedupSlot *tab;              // representative work item, its position and length under the tag; all ones = free
   uint32_t mask;
   uint32_t *rep;               // per work item: its representative (itself if it is one)
   uint32_t *list;              // the representatives, in arrival order
@@ -578,7 +618,9 @@ __device__ __forceinline__ uint32_t dd_eq16(Chunk16 c, uint32_t v4) {
 }
 __device__ __forceinline__ uint64_t dd_rotl(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
 
-__global__ void __launch_bounds__(128) dedup_words_kernel(EncArgs a, uint64_t n_words, DedupArgs d) {
+// (10 blocks of 128 threads per SM: latency-bound, so occupancy is what hides the chain of loads)
+__global__ void __launch_bounds__(128, 10) dedup_words_kernel(EncArgs a, uint64_t n_words, DedupArgs d,
+                                                              const uint16_t *__restrict__ word_len) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t o0 = a.offs[0];
@@ -588,29 +630,37 @@ __global__ void __launch_bounds__(128) dedup_words_kernel(EncArgs a, uint64_t n_
     const uint64_t w = w0 + lane;
     bool is_rep = false;
     if (w < n_words) {
-      const int64_t p0 = a.word_pos[w], hi = (int64_t)(a.offs[(uint64_t)a.word_sent[w] + 1] - o0);
-      uint32_t l;
-      // ---- end of the word: the first space unit at or after p0, or hi; its first 3 chunks stay in registers
+      const int64_t p0 = a.word_pos[w];
       const uint32_t o = (uint32_t)((p0 + mis) & 15);
+      // ---- the word's first 3 chunks (they stay in registers) and its length
       Chunk16 c0{0, 0}, c1{0, 0}, c2{0, 0};
-      int64_t end = hi;
-      for (int64_t q = p0 - o, k = 0; q < hi; q += 16, k++) {
-        const Chunk16 c = dd_chunk(a.bytes, q, n_total);
-        if (k == 0) c0 = c; else if (k == 1) c1 = c; else if (k == 2) c2 = c;
-        const int64_t lim = hi - q;  // bytes of the sentence in this chunk (if below 16)
-        uint32_t m = dd_space16(c);
-        const uint32_t e2 = dd_eq16(c, 0xe2e2e2e2u);
-        if (e2) {  // U+2581 = E2 96 81 inside the sentence; one starting in the last two bytes is checked byte by byte
-          const uint32_t whole = lim - 2 >= 14 ? 0x3fffu : lim - 2 <= 0 ? 0u : (1u << (lim - 2)) - 1;
-          m |= e2 & (dd_eq16(c, 0x96969696u) >> 1) & (dd_eq16(c, 0x81818181u) >> 2) & whole;
-          for (int j = 14; j < 16; j++)
-            if (((e2 >> j) & 1u) && j < lim && space_at(a.bytes, (uint64_t)(q + j), (uint64_t)hi, &l)) m |= 1u << j;
+      uint32_t len = word_len[w];
+      if (len != WORD_LEN_ESC) {  // independent loads
+        c0 = dd_chunk(a.bytes, p0 - o, n_total);
+        if (o + len > 16) c1 = dd_chunk(a.bytes, p0 - o + 16, n_total);
+        if (o + len > 32) c2 = dd_chunk(a.bytes, p0 - o + 32, n_total);
+      } else {  // the finder did not see the end: the first space unit at or after p0, or the sentence end hi
+        const int64_t hi = (int64_t)(a.offs[(uint64_t)a.word_sent[w] + 1] - o0);
+        uint32_t l;
+        int64_t end = hi;
+        for (int64_t q = p0 - o, k = 0; q < hi; q += 16, k++) {
+          const Chunk16 c = dd_chunk(a.bytes, q, n_total);
+          if (k == 0) c0 = c; else if (k == 1) c1 = c; else if (k == 2) c2 = c;
+          const int64_t lim = hi - q;  // bytes of the sentence in this chunk (if below 16)
+          uint32_t m = dd_space16(c);
+          const uint32_t e2 = dd_eq16(c, 0xe2e2e2e2u);
+          if (e2) {  // U+2581 = E2 96 81 inside the sentence; one starting in the last two bytes is checked byte by byte
+            const uint32_t whole = lim - 2 >= 14 ? 0x3fffu : lim - 2 <= 0 ? 0u : (1u << (lim - 2)) - 1;
+            m |= e2 & (dd_eq16(c, 0x96969696u) >> 1) & (dd_eq16(c, 0x81818181u) >> 2) & whole;
+            for (int j = 14; j < 16; j++)
+              if (((e2 >> j) & 1u) && j < lim && space_at(a.bytes, (uint64_t)(q + j), (uint64_t)hi, &l)) m |= 1u << j;
+          }
+          if (k == 0) m &= 0xffffu << o;
+          if (lim < 16) m &= (1u << lim) - 1;
+          if (m) { end = q + __ffs((int)m) - 1; break; }
         }
-        if (k == 0) m &= 0xffffu << o;
-        if (lim < 16) m &= (1u << lim) - 1;
-        if (m) { end = q + __ffs((int)m) - 1; break; }
+        len = (uint32_t)(end - p0);
       }
-      const uint32_t len = (uint32_t)(end - p0);
       // bytes 16 k .. of the word (n of them)
       auto own = [&](uint32_t k, uint32_t n) {
         return k == 0 ? dd_shift(c0, c1, o, n) : k == 1 ? dd_shift(c1, c2, o, n)
@@ -624,29 +674,37 @@ __global__ void __launch_bounds__(128) dedup_words_kernel(EncArgs a, uint64_t n_
       }
       h = mix64(h);
       const uint32_t tag = d.weak_tag ? 7u : (uint32_t)(h >> 32);
-      const unsigned long long mine = ((unsigned long long)tag << 32) | (uint32_t)w;
+      const DedupSlot mine{tag, (uint32_t)w, (uint32_t)p0, len};
       uint32_t idx = (uint32_t)h & d.mask, r = (uint32_t)w;
       is_rep = true;  // also the outcome of running out of probes
       for (uint32_t k = 0; k < DEDUP_PROBES; k++, idx = (idx + 1) & d.mask) {
-        unsigned long long cur = *(volatile unsigned long long *)(d.tab + idx);
-        if (cur == DEDUP_EMPTY) {
-          cur = atomicCAS(d.tab + idx, DEDUP_EMPTY, mine);
-          if (cur == DEDUP_EMPTY) break;  // slot claimed: this occurrence represents the word
+        const uint4 v = __ldcg(reinterpret_cast<const uint4 *>(d.tab + idx));
+        DedupSlot cur{v.x, v.y, v.z, v.w};
+        if (v.x == ~0u || v.y == ~0u || v.z == ~0u || v.w == ~0u) {  // free, or a claim seen in part
+          cur = dd_claim(d.tab + idx, mine);
+          if (cur.item == ~0u) break;  // slot claimed: this occurrence represents the word
         }
-        if ((uint32_t)(cur >> 32) != tag) continue;
-        const uint32_t w2 = (uint32_t)cur;  // written by find_words (the previous launch), like everything read below
-        const uint64_t p2 = a.word_pos[w2], hi2 = a.offs[(uint64_t)a.word_sent[w2] + 1] - o0;
-        // Equal iff the len bytes match AND the word at p2 ends right after them.  No space unit can start inside the
-        // matching bytes: an ASCII space or a whole E2 96 81 there would be one in this word too, and an E2 96 81 that
-        // starts inside and ends beyond leaves a continuation byte at p2 + len, which the end check rejects.
-        bool same = p2 + len <= hi2;
-        for (uint32_t k = 0; same && 16ull * k < len; k++) {
+        if (cur.tag != tag || cur.len != len) continue;
+        // Equal length and equal bytes: the same word.  The representative's bytes were written before this launch.
+        const int64_t p2 = cur.pos;
+        const uint32_t o2 = (uint32_t)((p2 + mis) & 15);
+        const Chunk16 r0 = dd_chunk(a.bytes, p2 - o2, n_total);
+        const Chunk16 r1 = o2 + len > 16 ? dd_chunk(a.bytes, p2 - o2 + 16, n_total) : Chunk16{0, 0};
+        const Chunk16 r2 = o2 + len > 32 ? dd_chunk(a.bytes, p2 - o2 + 32, n_total) : Chunk16{0, 0};
+        const uint32_t n0 = min(16u, len);
+        Chunk16 x = dd_shift(r0, r1, o2, n0), y = own(0, n0);
+        bool same = x.lo == y.lo && x.hi == y.hi;
+        if (len > 16) {
+          const uint32_t n1 = min(16u, len - 16);
+          x = dd_shift(r1, r2, o2, n1); y = own(1, n1);
+          same = same && x.lo == y.lo && x.hi == y.hi;
+        }
+        for (uint32_t k = 2; same && 16ull * k < len; k++) {
           const uint32_t n = min(16u, len - 16 * k);
-          const Chunk16 x = dd_window(a.bytes, (int64_t)p2 + 16 * (int64_t)k, n, n_total, mis), y = own(k, n);
+          x = dd_window(a.bytes, p2 + 16 * (int64_t)k, n, n_total, mis); y = own(k, n);
           same = x.lo == y.lo && x.hi == y.hi;
         }
-        if (same && p2 + len < hi2 && !space_at(a.bytes, p2 + len, hi2, &l)) same = false;  // the other word is longer
-        if (same) { r = w2; is_rep = false; break; }
+        if (same) { r = cur.item; is_rep = false; break; }
       }
       d.rep[w] = r;
     }
@@ -1192,6 +1250,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   const uint64_t max_words = n_bytes / 2 + n_sent + 8;
   YT_CUDA(c, e->wpos.reserve(max_words * 4));
   YT_CUDA(c, e->wsent.reserve(max_words * 4));
+  YT_CUDA(c, e->wlen.reserve(max_words * 2));
   const uint64_t n_tiles = (n_sent + EMIT_T - 1) / EMIT_T;
   YT_CUDA(c, e->lookback.reserve((n_tiles + 1) * 8));
   YT_CUDA(c, e->out_off.reserve((n_sent + 2) * 8));
@@ -1202,6 +1261,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   a.slots = e->slots.as<int32_t>(); a.ranks = e->ranks.as<uint32_t>();
   a.aux = dropout > 0 ? e->aux.as<uint32_t>() : nullptr;
   a.word_pos = e->wpos.as<uint32_t>(); a.word_sent = e->wsent.as<uint32_t>();
+  uint16_t *word_len = e->wlen.as<uint16_t>();
   a.n_words = e->counter.as<unsigned long long>();
   a.cp2id = enc->cp2id.as<uint32_t>();
   a.rt.slots = enc->rules.as<uint4>(); a.rt.mask = enc->rule_mask;
@@ -1229,7 +1289,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
     const uint64_t mean = std::max<uint64_t>(n_bytes / n_sent, 1);
     const uint32_t G = (uint32_t)std::min<uint64_t>(FIND_GMAX, std::max<uint64_t>(FIND_TILE * 3 / 4 / mean, 1));
     const uint64_t blocks = std::min<uint64_t>((n_sent + G - 1) / G, (uint64_t)c->n_sm * 4);
-    find_words_vec_kernel<<<(unsigned)std::max<uint64_t>(blocks, 1), FIND_T, 0, c->stream>>>(a, G);
+    find_words_vec_kernel<<<(unsigned)std::max<uint64_t>(blocks, 1), FIND_T, 0, c->stream>>>(a, G, word_len);
     ytc::timer_end(c, "enc_find");
     c->launches++;
   }
@@ -1254,21 +1314,21 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
       ll.item = ll.end + cap;
       ll.cap = cap;
       YT_CUDA(c, cudaMemsetAsync(ll.n, 0, 8, c->stream));
-      // table: 2 slots per occurrence up to 2^21 slots (16 MB, L2-resident); beyond that it works as a cache
-      uint64_t tslots = std::max<uint64_t>(ytc::pow2ceil(std::min<uint64_t>(n_words, 1ull << 20) * 2), 1024);
+      // table: 2 slots per occurrence up to 2^20 slots (16 MB, L2-resident); beyond that it works as a cache
+      uint64_t tslots = std::max<uint64_t>(ytc::pow2ceil(std::min<uint64_t>(n_words, 1ull << 19) * 2), 1024);
       if (const int v = ytc::env_int("YTTM_ENC_DEDUP_SLOTS", 0, 1, INT_MAX)) tslots = ytc::pow2ceil((uint64_t)v);  // tests: tiny tables
-      YT_CUDA(c, e->dd_tab.reserve(tslots * 8));
+      YT_CUDA(c, e->dd_tab.reserve(tslots * sizeof(DedupSlot)));
       YT_CUDA(c, e->dd_rep.reserve(n_words * 4 + 16));
       YT_CUDA(c, e->dd_list.reserve(n_words * 4 + 16));
       DedupArgs d;
-      d.tab = e->dd_tab.as<unsigned long long>(); d.mask = (uint32_t)(tslots - 1);
+      d.tab = e->dd_tab.as<DedupSlot>(); d.mask = (uint32_t)(tslots - 1);
       d.rep = e->dd_rep.as<uint32_t>(); d.list = e->dd_list.as<uint32_t>();
       d.n_list = e->counter.as<unsigned long long>() + 2;  // zeroed with the other counters above
       d.weak_tag = ytc::env_set("YTTM_ENC_DEDUP_WEAKTAG");  // tests: tag collisions everywhere
       d_rep = d.rep;
-      YT_CUDA(c, cudaMemsetAsync(d.tab, 0xff, tslots * 8, c->stream));
+      YT_CUDA(c, cudaMemsetAsync(d.tab, 0xff, tslots * sizeof(DedupSlot), c->stream));
       ytc::timer_begin(c, "enc_dedup");
-      dedup_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, n_words, d);
+      dedup_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, n_words, d, word_len);
       ytc::timer_end(c, "enc_dedup");
       c->launches++;
       ytc::timer_begin(c, "enc_rep");
