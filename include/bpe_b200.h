@@ -246,6 +246,15 @@ class BaseEncoder {
   Status encode_file(int in_fd, const std::string &out_path, bool text, bool bos, bool eos, bool reverse,
                      double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const;
 
+  // Decodes ids of any size on the GPU, line by line, to the text of `yttm decode` (every line's decode and '\n') at
+  // out_path ("-" = stdout).  text: in_fd is id text, read to its end and split as encode_file splits it, and a line's
+  // ids are what `std::stringstream >> int` reads from it; else in_prefix names <in_prefix>.ids.npy (1-D <u2 or <i4)
+  // and <in_prefix>.offsets.npy (1-D <u8, from 0, non-decreasing, the last = the number of ids): line i =
+  // ids[offsets[i]:offsets[i+1]].  Ids in `ignore` are skipped; any other id outside [0, vocab_size) fails with decode's
+  // message.  The output is written under a temporary name and renamed on success.  *n_bytes = text bytes written.
+  Status decode_file(int in_fd, const std::string &in_prefix, const std::string &out_path, bool text,
+                     const std::vector<int32_t> &ignore, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const;
+
   // BPE-dropout stream: seed of the counter-based generator and the running sentence counter
   // (replaces the reference's global std::mt19937, bpe.cpp:1415).
   void set_dropout_seed(uint64_t seed) const { dropout_seed_ = seed; sentence_counter_ = 0; }

@@ -36,7 +36,8 @@ int yttm_device_count(void);
  * of the merge loop since the context was created or joined a job; they run on across trainings).  Counters of the
  * current training: "feed_pieces" (pieces of a fed corpus, 0 after load_corpus) and "dev_peak_bytes" (the largest sum
  * of the context's device buffers, sampled after every fed piece and every phase).  Counters of the last encode stream:
- * "stream_pieces" and "stream_dev_peak_bytes" (see yttm_enc_stream_begin). */
+ * "stream_pieces" and "stream_dev_peak_bytes" (see yttm_enc_stream_begin); of the last decode stream:
+ * "dec_stream_pieces" and "dec_stream_dev_peak_bytes" (see yttm_dec_stream_begin). */
 double yttm_stage_ms(const yttm_ctx *ctx, const char *stage);
 /* number of kernel launches issued by this context so far (bench.py: gpu_launches) */
 uint64_t yttm_launch_count(const yttm_ctx *ctx);
@@ -301,6 +302,29 @@ int yttm_dec_run(yttm_enc *enc, const int32_t *ids, const uint64_t *offsets, uin
 int yttm_dec_run_device(yttm_enc *enc, const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
                         const int32_t *ignore, uint64_t n_ignore, const uint8_t **d_out, const uint64_t **d_out_offsets,
                         uint64_t *out_n);
+
+/* ---- decode stream: ids or id text of any size fed in pieces, decoded line by line ------------------------------
+ * format names the input: YTTM_STREAM_IDS16 / YTTM_STREAM_IDS32 (uint16 / int32 ids fed in whole lines with
+ * yttm_dec_stream_feed_ids) or YTTM_STREAM_TEXT (`yttm encode --output_type id`'s text, fed in blocks of any size and
+ * boundary with yttm_dec_stream_feed; lines split as yttm_enc_stream splits them, and a line's ids are what
+ * `std::stringstream >> int` reads from it before its first failure, as `yttm decode` reads them).  Line i gives its
+ * yttm_dec_run text followed by '\n'; ignore[n_ignore] (copied by begin) and the error of an id outside the vocabulary
+ * (the first in line order) are those of yttm_dec_run.  The sink receives the text bytes of the completed lines and their
+ * ends as global byte counts, in line order, on the calling thread of feed / end.  Pieces, overlap, the device memory
+ * bound and the failure rules are those of the encode stream, with YTTM_DEC_STREAM_PIECE_KB (default 32768, read by
+ * begin) as the nominal piece size; while a decode stream is open every other encode and decode call on the encoder,
+ * and an encode stream, fails (and the other way round).  yttm_stage_ms(ctx, "dec_stream_pieces") /
+ * ("dec_stream_dev_peak_bytes"): pieces of the last decode stream and the largest sum of its device buffers. */
+int yttm_dec_stream_begin(yttm_enc *enc, int format, const int32_t *ignore, uint64_t n_ignore, yttm_enc_sink sink,
+                          void *user);
+/* YTTM_STREAM_TEXT: any size and boundary; the bytes are copied before the call returns */
+int yttm_dec_stream_feed(yttm_enc *enc, const char *bytes, uint64_t n);
+/* the id forms: whole lines, ids[n_ids] (2 or 4 bytes each) and line_ends[n_lines], global id counts as the encode sink
+ * gives them (non-decreasing, from the ids fed before, the last = those + n_ids); copied before the call returns */
+int yttm_dec_stream_feed_ids(yttm_enc *enc, const void *ids, uint64_t n_ids, const uint64_t *line_ends, uint64_t n_lines);
+/* decodes what is left, hands it to the sink and closes the stream; n_ids: ids decoded (text: ids read); each output
+ * may be NULL */
+int yttm_dec_stream_end(yttm_enc *enc, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes);
 
 #ifdef __cplusplus
 }

@@ -116,6 +116,11 @@ int yttm_api_decode_cli(void *handle, const int32_t *ignore, uint64_t n_ignore);
  * stats[3] = lines, ids, input bytes.  0 ok, 1 error. */
 int yttm_api_encode_file(void *handle, int in_fd, const char *out_path, int text, int bos, int eos, int reverse,
                          double dropout, uint64_t *stats);
+/* BaseEncoder::decode_file: with text != 0 the id text of in_fd, else the pair <in_prefix>.ids.npy +
+ * <in_prefix>.offsets.npy, decoded to out_path ("-" = stdout) as `yttm decode` prints it; ignore[n_ignore] as for
+ * decode.  stats[3] = lines, ids, text bytes written.  0 ok, 1 error. */
+int yttm_api_decode_file(void *handle, int in_fd, const char *in_prefix, const char *out_path, int text,
+                         const int32_t *ignore, uint64_t n_ignore, uint64_t *stats);
 void yttm_api_vocab_cli(void *handle, int verbose);
 
 /* order of the char2id lines of a model file written by the reference (BPEState::dump, utils.cpp:57-59):

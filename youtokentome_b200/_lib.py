@@ -32,7 +32,8 @@ def lib():
     return _lib
 
 
-# yttm_enc_sink of include/yttm_b200.h: (user, data, n_bytes, line_ends, n_lines) -> 0 or a failure
+# yttm_enc_sink of include/yttm_b200.h (the sink of both streams): (user, data, n_bytes, line_ends, n_lines) -> 0 or a
+# failure
 ENC_SINK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_uint64)
 STREAM_IDS16, STREAM_IDS32, STREAM_TEXT = 0, 1, 2
 
@@ -79,6 +80,7 @@ def bind(L):
         "yttm_api_encode_cli": (i32, [vp, cp, i32, i32, i32, i32, dbl]),
         "yttm_api_decode_cli": (i32, [vp, vp, u64]),
         "yttm_api_encode_file": (i32, [vp, i32, cp, i32, i32, i32, i32, dbl, vp]),
+        "yttm_api_decode_file": (i32, [vp, i32, cp, cp, i32, vp, u64, vp]),
         "yttm_api_vocab_cli": (None, [vp, i32]),
         "yttm_api_dump_order": (i32, [vp, u64, vp]),
         "yttm_api_redump": (i32, [cp, cp]),
@@ -132,6 +134,10 @@ def bind(L):
         "yttm_enc_stream_end": (i32, [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
         "yttm_dec_run": (i32, [vp, vp, vp, u64, vp, u64, vp, u64, vp, C.POINTER(u64)]),
         "yttm_dec_run_device": (i32, [vp, vp, u64, vp, u64, vp, u64, C.POINTER(vp), C.POINTER(vp), C.POINTER(u64)]),
+        "yttm_dec_stream_begin": (i32, [vp, i32, vp, u64, ENC_SINK, vp]),
+        "yttm_dec_stream_feed": (i32, [vp, vp, u64]),
+        "yttm_dec_stream_feed_ids": (i32, [vp, vp, u64, vp, u64]),
+        "yttm_dec_stream_end": (i32, [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
     }
     missing = []
     for name, (res, args) in sig.items():
@@ -156,7 +162,8 @@ EXPORTED_SYMBOLS_DEVICE_ABI = [
     "yttm_train_scan_once", "yttm_train_synth_words", "yttm_enc_create", "yttm_enc_destroy", "yttm_enc_run",
     "yttm_enc_run_device", "yttm_enc_run_spans", "yttm_enc_run_spans_device", "yttm_enc_run_subwords",
     "yttm_enc_run_subwords_device", "yttm_enc_run_padded", "yttm_enc_run_padded_device", "yttm_enc_stream_begin",
-    "yttm_enc_stream_feed", "yttm_enc_stream_end", "yttm_dec_run", "yttm_dec_run_device",
+    "yttm_enc_stream_feed", "yttm_enc_stream_end", "yttm_dec_run", "yttm_dec_run_device", "yttm_dec_stream_begin",
+    "yttm_dec_stream_feed", "yttm_dec_stream_feed_ids", "yttm_dec_stream_end",
 ]
 
 

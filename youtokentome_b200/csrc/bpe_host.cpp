@@ -18,6 +18,7 @@
 #include <thread>
 
 #include <fcntl.h>
+#include <sys/stat.h>
 #include <unistd.h>
 
 #include "../../include/bpe_b200.h"
@@ -961,6 +962,7 @@ namespace {
 // An output written under a temporary name in its directory and renamed on commit; "-" is stdout (no rename).
 class OutFile {
  public:
+  explicit OutFile(const char *who = "encode_file") : who_(who) {}
   ~OutFile() {
     if (fd_ >= 0 && fd_ != 1) ::close(fd_);
     if (!tmp_.empty()) ::unlink(tmp_.c_str());
@@ -1001,8 +1003,9 @@ class OutFile {
 
  private:
   Status error(const char *what) const {
-    return Status(1, std::string("encode_file: ") + what + " '" + path_ + "': " + std::strerror(errno));
+    return Status(1, std::string(who_) + ": " + what + " '" + path_ + "': " + std::strerror(errno));
   }
+  const char *who_;
   std::string path_, tmp_;
   int fd_ = -1;
 };
@@ -1079,6 +1082,185 @@ Status BaseEncoder::encode_file(int in_fd, const std::string &out_path, bool tex
   if (!(st = ids_file.commit()).ok() || (!text && !(st = offsets_file.commit()).ok())) return st;
   if (dropout_prob > 0) sentence_counter_ += *n_lines;
   return Status();
+}
+
+
+// ---------------------------------------------------------------------------------------------
+// decode_file: an .npy pair or id text through the device's decode stream (yttm_dec_stream_* of yttm_b200.h) into text
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+Status dec_error(const std::string &what) { return Status(1, "decode_file: " + what); }
+
+// A 1-D little-endian .npy array (format 1.0, 2.0 or 3.0) opened for reading: its type, length and data offset.
+struct NpyIn {
+  int fd = -1;
+  std::string path, descr;
+  uint64_t n = 0, data_at = 0, item = 0;
+  ~NpyIn() { if (fd >= 0) ::close(fd); }
+
+  Status open(const std::string &p, const std::vector<std::string> &types) {
+    path = p;
+    fd = ::open(p.c_str(), O_RDONLY | O_CLOEXEC);
+    if (fd < 0) return dec_error("cannot open '" + p + "': " + std::strerror(errno));
+    struct stat sb;
+    if (::fstat(fd, &sb) != 0) return dec_error("cannot read '" + p + "': " + std::strerror(errno));
+    char pre[12];
+    if (::pread(fd, pre, 12, 0) < 10 || std::memcmp(pre, "\x93NUMPY", 6) != 0) return bad("not an .npy file");
+    const int major = (uint8_t)pre[6];
+    if (major < 1 || major > 3) return bad("NPY format version " + std::to_string(major) + " is not 1, 2 or 3");
+    uint64_t hlen, at;
+    if (major == 1) {
+      hlen = (uint8_t)pre[8] | (uint64_t)(uint8_t)pre[9] << 8;
+      at = 10;
+    } else {
+      hlen = (uint8_t)pre[8] | (uint64_t)(uint8_t)pre[9] << 8 | (uint64_t)(uint8_t)pre[10] << 16 | (uint64_t)(uint8_t)pre[11] << 24;
+      at = 12;
+    }
+    if (at + hlen > (uint64_t)sb.st_size || hlen > (1u << 20)) return bad("truncated header");
+    std::string h(hlen, '\0');
+    if (::pread(fd, &h[0], hlen, (off_t)at) != (ssize_t)hlen) return bad("truncated header");
+    auto field = [&](const char *key) -> std::string {  // the text after "'key':" up to the next ',' outside brackets
+      const std::string k = std::string("'") + key + "'";
+      size_t i = h.find(k);
+      if (i == std::string::npos) return "";
+      i = h.find(':', i + k.size());
+      if (i == std::string::npos) return "";
+      size_t j = i + 1;
+      int depth = 0;
+      for (; j < h.size(); j++) {
+        if (h[j] == '(') depth++;
+        else if (h[j] == ')') { if (depth-- == 0) break; }
+        else if ((h[j] == ',' || h[j] == '}') && depth == 0) break;
+      }
+      std::string v = h.substr(i + 1, j - i - 1);
+      v.erase(0, v.find_first_not_of(" "));
+      v.erase(v.find_last_not_of(" ") + 1);
+      return v;
+    };
+    descr = field("descr");
+    if (descr.size() >= 2 && (descr[0] == '\'' || descr[0] == '"')) descr = descr.substr(1, descr.size() - 2);
+    if (std::find(types.begin(), types.end(), descr) == types.end()) {
+      std::string want;
+      for (auto &t : types) want += (want.empty() ? "" : " or ") + t;
+      return bad("dtype '" + descr + "' is not " + want +
+                 (descr == "<i8" || descr == "<u8" ? " (convert the ids with .astype(np.int32))" : ""));
+    }
+    item = descr == "<u2" ? 2 : descr == "<i4" ? 4 : 8;
+    if (field("fortran_order") != "False") return bad("the array is in Fortran order");
+    const std::string shape = field("shape");
+    size_t k = 0;
+    if (shape.size() < 4 || shape.front() != '(' || shape.back() != ')') return bad("shape " + shape + " is not 1-D");
+    const std::string in = shape.substr(1, shape.size() - 2);
+    const size_t comma = in.find(',');
+    if (comma == std::string::npos || in.find_first_not_of(" ", comma + 1) != std::string::npos)
+      return bad("shape " + shape + " is not 1-D");
+    const std::string num = in.substr(0, comma);
+    if (num.empty() || num.find_first_not_of("0123456789") != std::string::npos || num.size() > 18)
+      return bad("shape " + shape + " is not 1-D");
+    for (; k < num.size(); k++) n = n * 10 + (uint64_t)(num[k] - '0');
+    data_at = at + hlen;
+    if ((uint64_t)sb.st_size < data_at || ((uint64_t)sb.st_size - data_at) / item < n)
+      return bad("truncated: " + std::to_string(n) + " values need " + std::to_string(data_at + n * item) + " bytes, the file has " +
+                 std::to_string((uint64_t)sb.st_size));
+    return Status();
+  }
+  Status read(void *dst, uint64_t first, uint64_t count) const {
+    char *p = static_cast<char *>(dst);
+    uint64_t at = data_at + first * item, left = count * item;
+    while (left) {
+      const ssize_t k = ::pread(fd, p, std::min<uint64_t>(left, 1u << 30), (off_t)at);
+      if (k < 0 && errno == EINTR) continue;
+      if (k <= 0) return dec_error("cannot read '" + path + "': " + (k < 0 ? std::strerror(errno) : "truncated"));
+      p += k;
+      at += (uint64_t)k;
+      left -= (uint64_t)k;
+    }
+    return Status();
+  }
+  Status bad(const std::string &what) const { return dec_error("'" + path + "': " + what); }
+};
+
+int text_sink(void *user, const void *data, uint64_t n_bytes, const uint64_t *, uint64_t) {
+  auto *f = static_cast<FileSink *>(user);
+  if (f->stop) return 1;
+  f->st = f->ids->write(data, n_bytes);
+  return f->st.ok() ? 0 : 1;
+}
+
+}  // namespace
+
+Status BaseEncoder::decode_file(int in_fd, const std::string &in_prefix, const std::string &out_path, bool text,
+                                const std::vector<int32_t> &ignore, uint64_t *n_lines, uint64_t *n_ids,
+                                uint64_t *n_bytes) const {
+  *n_lines = *n_ids = *n_bytes = 0;
+  Status st = run_device("decode_file", false, false, 0, 0, [] { return 0; });  // the device checks
+  if (!st.ok()) return st;
+  NpyIn ids_in, offs_in;
+  if (!text) {
+    if (!(st = ids_in.open(in_prefix + ".ids.npy", {"<u2", "<i4"})).ok()) return st;
+    if (!(st = offs_in.open(in_prefix + ".offsets.npy", {"<u8"})).ok()) return st;
+    if (offs_in.n == 0) return offs_in.bad("no offsets (a file of n lines has n + 1)");
+  }
+  OutFile out("decode_file");
+  FileSink fs;
+  fs.text = true;
+  fs.ids = &out;
+  if (!(st = out.open(out_path)).ok()) return st;
+  const int format = text ? YTTM_STREAM_TEXT : ids_in.item == 2 ? YTTM_STREAM_IDS16 : YTTM_STREAM_IDS32;
+  if (yttm_dec_stream_begin(enc_, format, ignore.data(), ignore.size(), text_sink, &fs)) return Status(1, ctx_err(ctx_));
+  auto failed = [&]() { return fs.st.ok() ? Status(1, ctx_err(ctx_)) : fs.st; };
+  auto abandon = [&](const Status &why) {  // closes the stream without handing anything more to the sink
+    fs.stop = true;
+    uint64_t a, b, c;
+    yttm_dec_stream_end(enc_, &a, &b, &c);
+    return why;
+  };
+  if (text) {
+    std::vector<char> block((size_t)16 << 20);
+    while (true) {
+      const ssize_t k = ::read(in_fd, block.data(), block.size());
+      if (k < 0 && errno == EINTR) continue;
+      if (k < 0) return abandon(dec_error(std::string("cannot read the input: ") + std::strerror(errno)));
+      if (k == 0) break;
+      if (yttm_dec_stream_feed(enc_, block.data(), (uint64_t)k)) return failed();
+    }
+  } else {
+    // blocks of up to 1 M line ends and 16 MB of ids (a longer line is read whole)
+    const uint64_t L = offs_in.n - 1, max_lines = 1 << 20, max_ids = ((uint64_t)16 << 20) / ids_in.item;
+    std::vector<uint64_t> ends(max_lines + 1);
+    std::vector<char> ids;
+    if (!(st = offs_in.read(ends.data(), 0, 1)).ok()) return abandon(st);
+    if (ends[0] != 0) return abandon(offs_in.bad("offsets[0] is " + std::to_string(ends[0]) + ", not 0"));
+    uint64_t done = 0, prev = 0;  // lines fed, their ids
+    while (done < L) {
+      const uint64_t m = std::min(max_lines, L - done);
+      if (!(st = offs_in.read(ends.data(), done + 1, m)).ok()) return abandon(st);
+      uint64_t k = 0;
+      while (k < m) {
+        uint64_t j = k, last = prev;
+        for (; j < m; j++) {
+          if (ends[j] < last) return abandon(offs_in.bad("offsets decrease at " + std::to_string(done + j + 1)));
+          if (ends[j] > ids_in.n)
+            return abandon(offs_in.bad("offsets[" + std::to_string(done + j + 1) + "] = " + std::to_string(ends[j]) +
+                                       " is past the " + std::to_string(ids_in.n) + " ids"));
+          if (ends[j] - prev > max_ids && j > k) break;
+          last = ends[j];
+        }
+        ids.resize((last - prev) * ids_in.item + 1);
+        if (!(st = ids_in.read(ids.data(), prev, last - prev)).ok()) return abandon(st);
+        if (yttm_dec_stream_feed_ids(enc_, ids.data(), last - prev, ends.data() + k, j - k)) return failed();
+        prev = last;
+        k = j;
+      }
+      done += m;
+    }
+    if (prev != ids_in.n)
+      return abandon(offs_in.bad("offsets[-1] = " + std::to_string(prev) + " is not the number of ids (" +
+                                 std::to_string(ids_in.n) + ")"));
+  }
+  if (yttm_dec_stream_end(enc_, n_lines, n_ids, n_bytes)) return failed();
+  return out.commit();
 }
 
 }  // namespace vkcom

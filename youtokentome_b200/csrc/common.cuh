@@ -134,6 +134,8 @@ struct yttm_ctx {
   double enc_chunks = -1;       // chunks the last host-buffer encode call was cut into (encode.cu)
   // the last encode stream of the context (encode.cu): its pieces and the largest sum of its encoder's device buffers
   double enc_stream_pieces = -1, enc_stream_peak = -1;
+  // the same for the last decode stream (decode.cu)
+  double dec_stream_pieces = -1, dec_stream_peak = -1;
 
   yttm_train_stats stats{};
 };

@@ -76,7 +76,9 @@ __device__ __forceinline__ bool look(const DecArgs &a, int32_t id, uint32_t *src
   return false;
 }
 
-__global__ void __launch_bounds__(256) dec_count_kernel(DecArgs a) {
+// NL: every sentence is followed by one '\n' (the decode stream's lines)
+template <bool NL>
+__device__ __forceinline__ void dec_count(DecArgs a) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
@@ -109,9 +111,12 @@ __global__ void __launch_bounds__(256) dec_count_kernel(DecArgs a) {
       sum += len;
     }
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if (lane == 0) a.sent_bytes[s] = sum;
+    if (lane == 0) a.sent_bytes[s] = sum + (NL ? 1 : 0);
   }
 }
+
+__global__ void __launch_bounds__(256) dec_count_kernel(DecArgs a) { dec_count<false>(a); }
+__global__ void __launch_bounds__(256) dec_count_nl_kernel(DecArgs a) { dec_count<true>(a); }
 
 // Bytes [0, T) of a round go to out[R0 ..]; lane k holds the inclusive end `incl` of piece k in the round and
 // d = (first source byte of piece k) - (its start in the round), so round byte r of piece k is bytes[d + r].
@@ -144,8 +149,9 @@ __device__ __forceinline__ void emit_round(const DecArgs &a, uint8_t *__restrict
   }
 }
 
-__global__ void __launch_bounds__(256) dec_emit_kernel(DecArgs a, const unsigned long long *__restrict__ out_off,
-                                                       uint8_t *__restrict__ out) {
+template <bool NL>
+__device__ __forceinline__ void dec_emit(DecArgs a, const unsigned long long *__restrict__ out_off,
+                                         uint8_t *__restrict__ out) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
@@ -179,7 +185,197 @@ __global__ void __launch_bounds__(256) dec_emit_kernel(DecArgs a, const unsigned
       if (T) emit_round(a, out, pos, T, incl, (int64_t)src - (int64_t)(incl - len), lane);
       pos += T;
     }
+    if (NL && lane == 0) out[pos] = '\n';  // a byte store: no round wrote a full word over it
   }
+}
+
+__global__ void __launch_bounds__(256) dec_emit_kernel(DecArgs a, const unsigned long long *__restrict__ out_off,
+                                                       uint8_t *__restrict__ out) {
+  dec_emit<false>(a, out_off, out);
+}
+__global__ void __launch_bounds__(256) dec_emit_nl_kernel(DecArgs a, const unsigned long long *__restrict__ out_off,
+                                                          uint8_t *__restrict__ out) {
+  dec_emit<true>(a, out_off, out);
+}
+
+// ---- the decode stream's kernels ----
+
+__global__ void __launch_bounds__(256) widen_ids_kernel(const uint16_t *__restrict__ in, uint64_t n,
+                                                        int32_t *__restrict__ out) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = in[i];
+}
+
+// Id text: the ids of a line are what `std::stringstream >> int` reads from it (BaseEncoder::decode of a string):
+// tokens [+-]?[0-9]+ between whitespace (' ', \t, \v, \f, \r; the line's '\n' counts as whitespace) or right after the
+// previous token, read until the first stop: a byte that is neither whitespace, a digit nor a sign, a sign not followed by
+// a digit, or a token outside int32.  Every digit run before the first stop is a token, so a line's ids are its digit
+// runs that end before the first stop, and each is decided by bytes near its last digit: its value is its last 10
+// digits, unless a nonzero digit lies before them (found with a scan of the last byte that is not '0').  A warp reads
+// a line in rounds of 512 bytes (16 per lane, one 16-byte load); nothing walks a line byte by byte.
+constexpr uint32_t IDT_ROUND = 512;
+
+// bit k: byte q + k of the line [lo, hi) is a digit / a sign / another stop byte / not '0' (bytes outside the line are
+// whitespace, and not '0')
+__device__ __forceinline__ void id_text_classes(const uint8_t *__restrict__ p, uint64_t n, uint64_t q, uint64_t lo,
+                                                uint64_t hi, uint32_t *dig, uint32_t *sign, uint32_t *other,
+                                                uint32_t *nz) {
+  uint32_t w[4] = {0x0a0a0a0au, 0x0a0a0a0au, 0x0a0a0a0au, 0x0a0a0a0au};
+  if (q + 16 <= n) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p + q));
+    w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+  } else {
+    for (uint32_t k = 0; k < 16 && q + k < n; k++)
+      w[k >> 2] = (w[k >> 2] & ~(0xffu << (8 * (k & 3)))) | ((uint32_t)p[q + k] << (8 * (k & 3)));
+  }
+  uint32_t d = 0, s = 0, o = 0, z = 0;
+#pragma unroll
+  for (uint32_t k = 0; k < 16; k++) {
+    const uint32_t x = (w[k >> 2] >> (8 * (k & 3))) & 0xffu;
+    const bool isd = x - '0' < 10u, iss = x == '+' || x == '-', isw = x == ' ' || x - 9u < 5u;
+    d |= (uint32_t)isd << k;
+    s |= (uint32_t)iss << k;
+    o |= (uint32_t)(!isd && !iss && !isw) << k;
+    z |= (uint32_t)(x != '0') << k;
+  }
+  const uint32_t a = q < lo ? (uint32_t)(lo - q) : 0u, b = q + 16 <= hi ? 16u : hi > q ? (uint32_t)(hi - q) : 0u;
+  const uint32_t in = a < b ? ((1u << b) - 1u) & ~((1u << a) - 1u) : 0u;
+  *dig = d & in;
+  *sign = s & in;
+  *other = o & in;
+  *nz = (z | ~in) & 0xffffu;
+}
+
+// A lane's view of the last byte that is not '0': its chunk (q, z), the chunk before (zprev) and the scan values in
+// front of each
+struct NzWin {
+  int64_t q, excl, exclprev;
+  uint32_t z, zprev;
+};
+
+// the position of the last byte at or before x that is not '0' (x >= q - 16)
+__device__ __forceinline__ int64_t last_nonzero(const NzWin &w, int64_t x) {
+  if (x >= w.q) {
+    const uint32_t m = w.z & (0xffffu >> (15 - (uint32_t)(x - w.q)));
+    return m ? w.q + 31 - __clz((int)m) : w.excl;
+  }
+  const uint32_t m = w.zprev & (0xffffu >> (15 - (uint32_t)(x - w.q + 16)));
+  return m ? w.q - 16 + 31 - __clz((int)m) : w.exclprev;
+}
+
+// The token whose last digit is byte e of the line starting at lo: false when its value is outside int32.
+__device__ __forceinline__ bool token_value(const uint8_t *__restrict__ p, int64_t lo, int64_t e, const NzWin &w,
+                                            int32_t *out) {
+  uint64_t v = 0, mul = 1;
+  int64_t nd = 0;
+  for (; nd < 10 && e - nd >= lo; nd++) {
+    const uint32_t x = (uint32_t)__ldg(p + e - nd) - '0';
+    if (x >= 10u) break;
+    v += x * mul;
+    mul *= 10;
+  }
+  int64_t before = e - nd;  // the byte in front of the digits read
+  if (nd == 10 && before >= lo && (uint32_t)__ldg(p + before) - '0' < 10u) {  // a longer run: leading zeros or overflow
+    before = last_nonzero(w, before);
+    if (before >= lo && (uint32_t)__ldg(p + before) - '0' < 10u) return false;
+  }
+  const bool neg = before >= lo && __ldg(p + before) == '-';
+  if (v > (neg ? 2147483648ull : 2147483647ull)) return false;
+  *out = (int32_t)(neg ? 0u - (uint32_t)v : (uint32_t)v);
+  return true;
+}
+
+// The ids of the line [lo, hi) of the n bytes at p: their number (every lane); WRITE: to out[0 ..].
+template <bool WRITE>
+__device__ __forceinline__ uint64_t id_text_line(const uint8_t *__restrict__ p, uint64_t n, uint64_t lo, uint64_t hi,
+                                                 unsigned lane, int32_t *__restrict__ out) {
+  uint64_t count = 0;
+  int64_t carry_incl = (int64_t)lo - 1, carry_excl = (int64_t)lo - 1;  // the scan in front of the line: its boundary
+  uint32_t carry_z = 0xffffu;
+  for (uint64_t r = lo & ~15ull; r < hi; r += IDT_ROUND) {  // warp-uniform
+    const uint64_t q = r + 16 * lane;
+    uint32_t D, S, O, Z;
+    id_text_classes(p, n, q, lo, hi, &D, &S, &O, &Z);
+    uint32_t dn = __shfl_down_sync(0xffffffffu, D, 1) & 1u;  // the byte behind the chunk is a digit
+    if (lane == 31) dn = q + 16 < hi && (uint32_t)__ldg(p + q + 16) - '0' < 10u;
+    const uint32_t Dnext = (D >> 1) | (dn << 15);
+    const uint32_t E = D & ~Dnext, stop = O | (S & ~Dnext);  // last digits of tokens; stop bytes
+    int64_t incl = (int64_t)q + 31 - __clz((int)Z);  // Z has bits for the bytes outside the line: never 0 past it
+    if (!Z) incl = -1;
+    if (lane == 0) incl = max(incl, carry_incl);
+#pragma unroll
+    for (unsigned o = 1; o < 32; o <<= 1) {
+      const int64_t y = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl = max(incl, y);
+    }
+    NzWin w;
+    w.q = (int64_t)q;
+    w.z = Z;
+    w.excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    w.zprev = __shfl_up_sync(0xffffffffu, Z, 1);
+    if (lane == 0) { w.excl = carry_incl; w.zprev = carry_z; }
+    w.exclprev = __shfl_up_sync(0xffffffffu, w.excl, 1);
+    if (lane == 0) w.exclprev = carry_excl;
+    uint32_t ov = 0;
+    for (uint32_t m = E; m; m &= m - 1) {
+      const int k = __ffs((int)m) - 1;
+      int32_t v;
+      if (!token_value(p, (int64_t)lo, (int64_t)q + k, w, &v)) ov |= 1u << k;
+    }
+    const uint32_t kill = stop | ov;
+    const unsigned bk = __ballot_sync(0xffffffffu, kill != 0);
+    uint32_t keep = E;
+    if (bk) {
+      const unsigned first = (unsigned)__ffs((int)bk) - 1;
+      if (lane > first) keep = 0;
+      else if (lane == first) keep &= (1u << (__ffs((int)kill) - 1)) - 1u;
+    }
+    const uint32_t cnt = (uint32_t)__popc(keep);
+    uint32_t before = cnt;
+#pragma unroll
+    for (unsigned o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xffffffffu, before, o);
+      if (lane >= o) before += y;
+    }
+    if (WRITE) {
+      int32_t *dst = out + count + before - cnt;
+      for (uint32_t m = keep; m; m &= m - 1) {
+        int32_t v = 0;
+        token_value(p, (int64_t)lo, (int64_t)q + (__ffs((int)m) - 1), w, &v);
+        *dst++ = v;
+      }
+    }
+    count += __shfl_sync(0xffffffffu, before, 31);
+    if (bk) break;
+    carry_incl = __shfl_sync(0xffffffffu, incl, 31);
+    carry_excl = __shfl_sync(0xffffffffu, w.excl, 31);
+    carry_z = __shfl_sync(0xffffffffu, Z, 31);
+  }
+  return count;
+}
+
+// warp per line (offs: n_lines + 1 byte offsets of the lines): the number of its ids
+__global__ void __launch_bounds__(256) id_text_count_kernel(const uint8_t *__restrict__ p, uint64_t n,
+                                                            const unsigned long long *__restrict__ offs, uint64_t n_lines,
+                                                            unsigned long long *__restrict__ line_ids) {
+  const unsigned lane = threadIdx.x & 31;
+  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t s = warp; s < n_lines; s += nwarps) {
+    const uint64_t c = id_text_line<false>(p, n, offs[s], offs[s + 1], lane, nullptr);
+    if (lane == 0) line_ids[s] = c;
+  }
+}
+
+// warp per line: its ids at ids[id_off[s] ..]
+__global__ void __launch_bounds__(256) id_text_write_kernel(const uint8_t *__restrict__ p, uint64_t n,
+                                                            const unsigned long long *__restrict__ offs, uint64_t n_lines,
+                                                            const unsigned long long *__restrict__ id_off,
+                                                            int32_t *__restrict__ ids) {
+  const unsigned lane = threadIdx.x & 31;
+  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t s = warp; s < n_lines; s += nwarps) id_text_line<true>(p, n, offs[s], offs[s + 1], lane, ids + id_off[s]);
 }
 
 void append_utf8(uint32_t x, std::string *out) {  // the host encoder's token2word (bpe_host.cpp)
@@ -297,10 +493,11 @@ std::string offsets_error(uint64_t n_ids) {
 }
 
 // Runs the decode of a batch on the device.  Ids at absolute positions [id_base, id_lim) are d_ids[0 ..]; the results go
-// to out / out_off (n_sent + 1 offsets).  The bytes are only written when *total <= out_cap.
+// to out / out_off (n_sent + 1 offsets).  The bytes are only written when *total <= out_cap.  nl: every sentence's text
+// is followed by one '\n'.
 int dec_device(yttm_enc *e, const int32_t *d_ids, uint64_t id_base, uint64_t id_lim, const uint64_t *d_offs,
                uint64_t n_sent, const int32_t *ignore, uint64_t n_ignore, ytc::DevBuf *out, ytc::DevBuf *out_off_buf,
-               uint64_t out_cap, uint64_t *total) {
+               uint64_t out_cap, uint64_t *total, bool nl = false) {
   yttm_ctx *c = e->ctx;
   *total = 0;
   if (id_lim - id_base >= 0xfffffff0ull || n_sent >= 0xfffffff0ull)
@@ -344,7 +541,8 @@ int dec_device(yttm_enc *e, const int32_t *d_ids, uint64_t id_base, uint64_t id_
   ytc::timer_begin(c, "decode");
   const uint64_t sblocks = std::max<uint64_t>(std::min<uint64_t>((n_sent + 7) / 8, (uint64_t)c->n_sm * 8), 1);
   ytc::timer_begin(c, "dec_count");
-  dec_count_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a);
+  if (nl) dec_count_nl_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a);
+  else dec_count_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a);
   ytc::timer_end(c, "dec_count");
   c->launches++;
   unsigned long long *out_off = out_off_buf->as<unsigned long long>();
@@ -367,7 +565,8 @@ int dec_device(yttm_enc *e, const int32_t *d_ids, uint64_t id_base, uint64_t id_
   if (h_ctl[0] <= out_cap) {
     YT_CUDA(c, out->reserve(h_ctl[0] + 16));
     ytc::timer_begin(c, "dec_emit");
-    dec_emit_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a, out_off, out->as<uint8_t>());
+    if (nl) dec_emit_nl_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a, out_off, out->as<uint8_t>());
+    else dec_emit_kernel<<<(unsigned)sblocks, 256, 0, c->stream>>>(a, out_off, out->as<uint8_t>());
     ytc::timer_end(c, "dec_emit");
     c->launches++;
   }
@@ -378,7 +577,194 @@ int dec_device(yttm_enc *e, const int32_t *d_ids, uint64_t id_base, uint64_t id_
 
 }  // namespace
 
+// =====================================================================================================================
+// Decode stream (yttm_dec_stream_*): ids or id text fed in blocks runs through the shared piece pipeline of the encode
+// stream (yttm_piece_pipe), and each piece runs on the device as
+//   YTTM_STREAM_IDS16   widen_ids_kernel: the 16-bit ids copied in become int32
+//   YTTM_STREAM_TEXT    the line split of the encode stream (yttm_line_split), then
+//                       id_text_count_kernel   warp per line: the number of its ids
+//                       scan                   the lines' id offsets + the piece's ids (one 8-byte read-back)
+//                       id_text_write_kernel   warp per line: its ids
+//   dec_device, nl      the text of every line and its '\n' (dec_count_nl_kernel / scan / dec_emit_nl_kernel)
+//   add_base_kernel     line ends as global byte counts
+struct yttm_dec_stream {
+  yttm_enc *e = nullptr;
+  int format = YTTM_STREAM_IDS32;
+  std::vector<int32_t> ignore;
+  yttm_piece_pipe pipe;
+  ytc::DevBuf in[2], out[2], out_off[2];  // per slot: the piece copied in; its text and line offsets
+  ytc::DevBuf wide, tiles, offs, line_ids, id_off, ids;  // per piece (the pieces' kernels run in order on one stream)
+  uint64_t lines = 0, ids_out = 0, bytes = 0;
+};
+
+void yttm_dec_stream_free(yttm_dec_stream *s) {
+  if (!s) return;
+  yttm_pipe_free(&s->pipe);
+  ytc::DevBuf *b[] = {&s->in[0], &s->in[1], &s->out[0], &s->out[1], &s->out_off[0], &s->out_off[1], &s->wide, &s->tiles,
+                      &s->offs, &s->line_ids, &s->id_off, &s->ids};
+  for (auto *x : b) x->release();
+  s->e->dec_stream = nullptr;
+  delete s;
+}
+
+namespace {
+
+// "dec_stream_dev_peak_bytes": the decode tables and buffers of the encoder and the stream's, sampled after each piece
+void note_dec_stream_peak(yttm_dec_stream *S) {
+  yttm_dec *d = S->e->dec;
+  uint64_t sum = 0;
+  ytc::DevBuf *b[] = {&d->table, &d->ign, &d->sent_bytes, &d->ctl, &S->in[0], &S->in[1], &S->out[0], &S->out[1],
+                      &S->out_off[0], &S->out_off[1], &S->wide, &S->tiles, &S->offs, &S->line_ids, &S->id_off, &S->ids};
+  for (auto *x : b) sum += x->cap;
+  S->e->ctx->dec_stream_peak = std::max(S->e->ctx->dec_stream_peak, (double)sum);
+}
+
+// The kernels of the piece in slot s (yttm_piece_pipe::run).
+int dec_stream_run(void *owner, int s, const void **out_data, const unsigned long long **out_ends) {
+  yttm_dec_stream *S = static_cast<yttm_dec_stream *>(owner);
+  yttm_enc *e = S->e;
+  yttm_ctx *c = e->ctx;
+  yttm_piece_pipe::Piece &P = S->pipe.pc[s];
+  const uint8_t *d = S->in[s].as<uint8_t>();
+  const int32_t *ids = nullptr;
+  const uint64_t *offs = nullptr;
+  uint64_t id_base = 0, id_lim = 0;
+  if (S->format == YTTM_STREAM_TEXT) {
+    if (yttm_line_split(c, d, P.n_bytes, P.open_end, &S->tiles, &S->offs, &P.n_lines)) return 1;
+    YT_CUDA(c, S->line_ids.reserve((P.n_lines + 1) * 8));
+    unsigned long long *lc = S->line_ids.as<unsigned long long>(), *lo = S->offs.as<unsigned long long>();
+    ytc::timer_begin(c, "dec_stream_parse");
+    const unsigned blocks = (unsigned)std::max<uint64_t>(std::min<uint64_t>((P.n_lines + 7) / 8, (uint64_t)c->n_sm * 8), 1);
+    id_text_count_kernel<<<blocks, 256, 0, c->stream>>>(d, P.n_bytes, lo, P.n_lines, lc);
+    c->launches++;
+    YT_CUDA(c, S->id_off.reserve((P.n_lines + 1) * 8));
+    unsigned long long *id_off = S->id_off.as<unsigned long long>();
+    if (yttm_device_scan_u64(c, lc, P.n_lines, id_off, id_off + P.n_lines)) return 1;
+    unsigned long long n_ids = 0;
+    YT_CUDA(c, cudaMemcpyAsync(&n_ids, id_off + P.n_lines, 8, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    YT_CUDA(c, S->ids.reserve(n_ids * 4 + 16));
+    id_text_write_kernel<<<blocks, 256, 0, c->stream>>>(d, P.n_bytes, lo, P.n_lines, id_off, S->ids.as<int32_t>());
+    c->launches++;
+    ytc::timer_end(c, "dec_stream_parse");
+    ids = S->ids.as<int32_t>();
+    offs = reinterpret_cast<const uint64_t *>(id_off);
+    id_lim = n_ids;
+  } else {
+    // the piece: its ids, then its line ends as global id counts (yttm_piece_pipe)
+    const uint64_t n_ids = P.n_bytes / S->pipe.unit;
+    offs = reinterpret_cast<const uint64_t *>(d + ((P.n_bytes + 15) & ~15ull));
+    id_base = P.first_id;
+    id_lim = id_base + n_ids;
+    ids = reinterpret_cast<const int32_t *>(d);
+    if (S->format == YTTM_STREAM_IDS16) {
+      YT_CUDA(c, S->wide.reserve(n_ids * 4 + 16));
+      const unsigned blocks = (unsigned)std::max<uint64_t>(std::min<uint64_t>((n_ids + 255) / 256, (uint64_t)c->n_sm * 8), 1);
+      widen_ids_kernel<<<blocks, 256, 0, c->stream>>>(reinterpret_cast<const uint16_t *>(d), n_ids, S->wide.as<int32_t>());
+      c->launches++;
+      ids = S->wide.as<int32_t>();
+    }
+  }
+  uint64_t total = 0;
+  if (dec_device(e, ids, id_base, id_lim, offs, P.n_lines, S->ignore.data(), S->ignore.size(), &S->out[s], &S->out_off[s],
+                 ~0ull, &total, true))
+    return 1;
+  unsigned long long *ends = S->out_off[s].as<unsigned long long>() + 1;
+  if (S->bytes) yttm_add_base(c, ends, P.n_lines, (unsigned long long)S->bytes);
+  *out_data = S->out[s].p;
+  *out_ends = ends;
+  P.n_out = total;
+  S->lines += P.n_lines;
+  S->ids_out += id_lim - id_base;
+  S->bytes += total;
+  c->dec_stream_pieces += 1;
+  note_dec_stream_peak(S);
+  return 0;
+}
+
+// a failed stream call: the stream is closed, the error kept
+int dec_stream_failed(yttm_enc *e) {
+  const std::string err = e->ctx->err;
+  yttm_dec_stream_free(e->dec_stream);
+  cudaGetLastError();
+  e->ctx->err = err;
+  return 1;
+}
+
+// the stream of a feed / end call, or 1 with the error recorded
+int dec_stream_of(yttm_enc *e, const char *who, int text) {
+  if (!e) return yttm_enc_check(e, who, 0, 0);
+  if (!e->dec_stream) YT_FAIL(e->ctx, std::string(who) + ": yttm_dec_stream_begin has not run");
+  if (text >= 0 && (e->dec_stream->format == YTTM_STREAM_TEXT) != (text != 0)) {
+    e->ctx->err = std::string(who) + (text ? ": the stream takes ids (yttm_dec_stream_feed_ids)"
+                                           : ": the stream takes id text (yttm_dec_stream_feed)");
+    return dec_stream_failed(e);
+  }
+  return 0;
+}
+
+}  // namespace
+
 extern "C" {
+
+int yttm_dec_stream_begin(yttm_enc *e, int format, const int32_t *ignore, uint64_t n_ignore, yttm_enc_sink sink,
+                          void *user) {
+  if (yttm_enc_check(e, "yttm_dec_stream_begin", 0, 0)) return 1;
+  yttm_ctx *c = e->ctx;
+  if (format != YTTM_STREAM_IDS16 && format != YTTM_STREAM_IDS32 && format != YTTM_STREAM_TEXT)
+    YT_FAIL(c, "yttm_dec_stream_begin: format must be YTTM_STREAM_IDS16, YTTM_STREAM_IDS32 or YTTM_STREAM_TEXT");
+  if (!sink) YT_FAIL(c, "yttm_dec_stream_begin: no sink");
+  if (yttm_pipe_init(e)) return 1;
+  if (!e->dec) e->dec = new yttm_dec();
+  yttm_dec_stream *S = new yttm_dec_stream();
+  S->e = e;
+  S->format = format;
+  S->ignore.assign(ignore, ignore + n_ignore);
+  yttm_piece_pipe &p = S->pipe;
+  p.e = e;
+  p.piece = (uint64_t)ytc::env_int("YTTM_DEC_STREAM_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;
+  p.unit = format == YTTM_STREAM_TEXT ? 0 : format == YTTM_STREAM_IDS16 ? 2 : 4;
+  p.dev_in[0] = &S->in[0];
+  p.dev_in[1] = &S->in[1];
+  p.run = dec_stream_run;
+  p.owner = S;
+  p.sink = sink;
+  p.user = user;
+  p.who = "yttm_dec_stream";
+  e->dec_stream = S;
+  c->dec_stream_pieces = 0;
+  c->dec_stream_peak = 0;
+  return 0;
+}
+
+int yttm_dec_stream_feed(yttm_enc *e, const char *bytes, uint64_t n) {
+  if (dec_stream_of(e, "yttm_dec_stream_feed", 1)) return 1;
+  return yttm_pipe_feed_text(&e->dec_stream->pipe, bytes, n) ? dec_stream_failed(e) : 0;
+}
+
+int yttm_dec_stream_feed_ids(yttm_enc *e, const void *ids, uint64_t n_ids, const uint64_t *line_ends, uint64_t n_lines) {
+  if (dec_stream_of(e, "yttm_dec_stream_feed_ids", 0)) return 1;
+  yttm_piece_pipe &p = e->dec_stream->pipe;
+  uint64_t prev = p.ids_in;
+  bool ok = true;
+  for (uint64_t k = 0; k < n_lines; prev = line_ends[k++]) ok &= line_ends[k] >= prev;
+  if (!ok || prev != p.ids_in + n_ids) {
+    e->ctx->err = "yttm_dec_stream_feed_ids: line_ends must not decrease, start at the ids fed before (" +
+                  std::to_string(p.ids_in) + ") and end at those plus n_ids";
+    return dec_stream_failed(e);
+  }
+  return yttm_pipe_feed_lines(&p, ids, n_ids, line_ends, n_lines) ? dec_stream_failed(e) : 0;
+}
+
+int yttm_dec_stream_end(yttm_enc *e, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) {
+  if (dec_stream_of(e, "yttm_dec_stream_end", -1)) return 1;
+  if (yttm_pipe_end(&e->dec_stream->pipe)) return dec_stream_failed(e);
+  if (n_lines) *n_lines = e->dec_stream->lines;
+  if (n_ids) *n_ids = e->dec_stream->ids_out;
+  if (n_bytes) *n_bytes = e->dec_stream->bytes;
+  yttm_dec_stream_free(e->dec_stream);
+  return 0;
+}
 
 int yttm_dec_run_device(yttm_enc *e, const int32_t *d_ids, uint64_t n_ids, const uint64_t *d_offsets, uint64_t n_sent,
                         const int32_t *ignore, uint64_t n_ignore, const uint8_t **d_out, const uint64_t **d_out_offsets,

@@ -7,6 +7,8 @@
 
 struct yttm_enc_stream;  // an open encode stream (encode.cu, yttm_enc_stream_*)
 void yttm_enc_stream_free(yttm_enc_stream *s);
+struct yttm_dec_stream;  // an open decode stream (decode.cu, yttm_dec_stream_*)
+void yttm_dec_stream_free(yttm_dec_stream *s);
 struct yttm_dec;  // decode state (decode.cu): piece table + per-call buffers, made by the first decode call
 void yttm_dec_free(yttm_dec *d);
 struct yttm_enc;
@@ -50,4 +52,56 @@ struct yttm_enc {
   cudaStream_t s_in = nullptr, s_out = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
   yttm_enc_stream *stream = nullptr;  // open between yttm_enc_stream_begin and _end; owns both slots meanwhile
+  yttm_dec_stream *dec_stream = nullptr;  // open between yttm_dec_stream_begin and _end; owns s_in / s_out meanwhile
 };
+
+// The host side of the encode and decode streams (encode.cu).  Fed input is staged in two pinned buffers and cut into
+// pieces; piece i is copied into *dev_in[i & 1] on the encoder's s_in while piece i - 1 runs its kernels on the context
+// stream and piece i - 2 is copied out on s_out and handed to the sink, on the caller's thread, in order.
+struct yttm_piece_pipe {
+  yttm_enc *e = nullptr;
+  uint64_t piece = 0;  // nominal piece bytes
+  // 0: text, cut behind the last '\n' of the staged bytes (yttm_pipe_feed_text); else the bytes of one id, fed in whole
+  // lines with their ends (yttm_pipe_feed_lines): the piece is its ids, then from (ids bytes + 15) & ~15 its
+  // n_lines + 1 line ends as global id counts (the first: the ids before the piece)
+  uint32_t unit = 0;
+  ytc::DevBuf *dev_in[2] = {nullptr, nullptr};  // the device copy of the piece in slot s (16 spare bytes)
+  // The kernels of the piece in slot s (pc[s]: n_bytes and n_lines of an id piece, open_end of a text piece): sets
+  // pc[s].n_lines and pc[s].n_out, *data (n_out bytes for the sink) and *ends (n_lines line ends for the sink).
+  int (*run)(void *owner, int s, const void **data, const unsigned long long **ends) = nullptr;
+  void *owner = nullptr;
+  yttm_enc_sink sink = nullptr;
+  void *user = nullptr;
+  const char *who = "";                     // the stream's name in error texts
+  uint8_t *stage[2] = {nullptr, nullptr};   // pinned staging of the fed bytes: piece i is copied in from stage[i & 1]
+  uint64_t stage_cap[2] = {0, 0};
+  uint8_t *ends[2] = {nullptr, nullptr};    // id pieces: their staged line ends (uint64)
+  uint64_t ends_cap[2] = {0, 0};
+  int cur = 0;                              // staging buffer being filled
+  uint64_t len = 0, nonl = 0;               // its bytes; its first bytes known to hold no '\n'
+  uint64_t n_ends = 0;                      // id pieces: its lines
+  uint8_t *out[2] = {nullptr, nullptr};     // pinned results of the piece in slot s: data, then its line ends
+  uint64_t out_cap[2] = {0, 0};
+  struct Piece {
+    uint64_t n_bytes = 0, n_lines = 0, n_out = 0;
+    uint64_t first_id = 0;                  // id pieces: the ids fed before the piece
+    bool open_end = false;                  // the last line has no '\n' (the end of the stream)
+  } pc[2];
+  int to_run = -1, to_deliver = -1;         // slot copied in, not yet run; slot copied out, not yet given to the sink
+  uint64_t bytes_in = 0, ids_in = 0;        // fed bytes; id pieces: fed ids
+};
+// The copy streams and events of the two slots (made by the first call that pipelines).
+int yttm_pipe_init(yttm_enc *e);
+int yttm_pipe_feed_text(yttm_piece_pipe *p, const char *bytes, uint64_t n);
+// whole lines: ids (n_ids of p->unit bytes) and their ends as global id counts, checked by the caller
+int yttm_pipe_feed_lines(yttm_piece_pipe *p, const void *ids, uint64_t n_ids, const uint64_t *line_ends, uint64_t n_lines);
+// runs what is left and hands it to the sink
+int yttm_pipe_end(yttm_piece_pipe *p);
+// waits for the encoder's streams and frees the pinned buffers
+void yttm_pipe_free(yttm_piece_pipe *p);
+// The lines of the n bytes at d (device): *n_lines of them, offsets (n_lines + 1: 0, the byte behind every '\n', n when
+// open_end) in offs; tiles is scratch.  One 8-byte read-back.
+int yttm_line_split(yttm_ctx *c, const uint8_t *d, uint64_t n, bool open_end, ytc::DevBuf *tiles, ytc::DevBuf *offs,
+                    uint64_t *n_lines);
+// off[0, n) += base on the context stream
+void yttm_add_base(yttm_ctx *c, unsigned long long *off, uint64_t n, unsigned long long base);

@@ -1444,8 +1444,9 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   return 0;
 }
 
-// The copy streams and events of the two slots (made by the first call that pipelines).
-int pipe_init(yttm_enc *e) {
+}  // namespace
+
+int yttm_pipe_init(yttm_enc *e) {
   yttm_ctx *c = e->ctx;
   if (e->s_in) return 0;
   YT_CUDA(c, cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
@@ -1457,6 +1458,8 @@ int pipe_init(yttm_enc *e) {
   }
   return 0;
 }
+
+namespace {
 
 // Caller buffers of the host-buffer entry points; nullptr = not asked for.  ids_cap bounds ids / spans / pieces (one
 // piece per id), bytes_cap the piece bytes.
@@ -1487,7 +1490,7 @@ int enc_run_host(yttm_enc *e, const char *who, const char *bytes, const uint64_t
     if (o.piece_offsets) o.piece_offsets[0] = 0;
     return 0;
   }
-  if (pipe_init(e)) return 1;
+  if (yttm_pipe_init(e)) return 1;
   // chunks of about CHUNK bytes, cut at sentence boundaries; chunk i lives in slot i & 1
   const uint64_t total_bytes = offsets[n_sent] - offsets[0];
   const uint64_t chunk_bytes = (uint64_t)ytc::env_int("YTTM_ENC_CHUNK_MB", 32, 1, INT_MAX) << 20;
@@ -1605,6 +1608,8 @@ int yttm_enc_check(yttm_enc *e, const char *who, int bos, int eos) {
   YT_CUDA(c, cudaSetDevice(c->device));
   if (e->stream)  // the stream's pieces are in flight in both slots between its calls
     YT_FAIL(c, std::string(who) + ": an encode stream is open on this encoder (yttm_enc_stream_end closes it)");
+  if (e->dec_stream)  // its pieces are in flight on the encoder's copy streams
+    YT_FAIL(c, std::string(who) + ": a decode stream is open on this encoder (yttm_dec_stream_end closes it)");
   ytc::timers_reset(c);   // every encode and decode call starts here: the stage times describe this call alone
   if (bos && e->bos == -1) YT_FAIL(c, "Can't add <BOS> token. Model was trained without it.");
   if (eos && e->eos == -1) YT_FAIL(c, "Can't add <EOS> token. Model was trained without it.");
@@ -1666,6 +1671,7 @@ void yttm_enc_destroy(yttm_enc *e) {
   if (!e) return;
   cudaSetDevice(e->ctx->device);
   yttm_enc_stream_free(e->stream);
+  yttm_dec_stream_free(e->dec_stream);
   e->cp2id.release();
   e->rules.release();
   e->sub_table.release();
@@ -1943,44 +1949,45 @@ unsigned warp_blocks(yttm_ctx *c, uint64_t n_warps) {  // blocks of 256 threads 
 
 }  // namespace
 
-struct yttm_enc_stream {
-  yttm_enc *e = nullptr;
-  int bos = 0, eos = 0, reverse = 0, format = YTTM_STREAM_IDS32;
-  double dropout = 0;
-  uint64_t seed = 0, first = 0;
-  yttm_enc_sink sink = nullptr;
-  void *user = nullptr;
-  uint64_t piece = 0;                       // nominal piece bytes
-  uint8_t *stage[2] = {nullptr, nullptr};   // pinned staging of the fed bytes: piece i is copied in from stage[i & 1]
-  uint64_t stage_cap[2] = {0, 0};
-  int cur = 0;                              // staging buffer being filled
-  uint64_t len = 0, nonl = 0;               // its bytes; its first bytes known to hold no '\n'
-  uint8_t *out[2] = {nullptr, nullptr};     // pinned results of the piece in slot s: data, then its line ends
-  uint64_t out_cap[2] = {0, 0};
-  struct Piece {
-    uint64_t n_bytes = 0, n_lines = 0, n_out = 0;
-    bool open_end = false;                  // the last line has no '\n' (the end of the stream)
-  } pc[2];
-  int to_encode = -1, to_deliver = -1;      // slot copied in, not yet encoded; slot copied out, not yet given to the sink
-  ytc::DevBuf tiles[2], fmt[2], lines_buf[2];  // per slot: '\n' per tile + bases; 16-bit ids or text; text per line
-  uint64_t lines = 0, ids = 0, bytes_in = 0;
-};
+// ---- the shared host pipeline of the encode and decode streams (yttm_piece_pipe of enc_state.cuh) ----
 
-void yttm_enc_stream_free(yttm_enc_stream *s) {
-  if (!s) return;
-  yttm_enc *e = s->e;
+int yttm_line_split(yttm_ctx *c, const uint8_t *d, uint64_t n, bool open_end, ytc::DevBuf *tiles, ytc::DevBuf *offs,
+                    uint64_t *n_lines) {
+  const uint64_t nt = (n + LS_TILE - 1) / LS_TILE;
+  YT_CUDA(c, tiles->reserve((2 * nt + 2) * 8));
+  unsigned long long *tile_nl = tiles->as<unsigned long long>(), *tile_base = tile_nl + nt, *n_nl = tile_base + nt;
+  ytc::timer_begin(c, "stream_lines");
+  line_count_kernel<<<(unsigned)nt, LS_T, 0, c->stream>>>(d, n, tile_nl);
+  c->launches++;
+  if (yttm_device_scan_u64(c, tile_nl, nt, tile_base, n_nl)) return 1;
+  unsigned long long h_nl = 0;
+  YT_CUDA(c, cudaMemcpyAsync(&h_nl, n_nl, 8, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  *n_lines = h_nl + (open_end ? 1 : 0);
+  YT_CUDA(c, offs->reserve((*n_lines + 2) * 8));
+  line_write_kernel<<<(unsigned)nt, LS_T, 0, c->stream>>>(d, n, tile_base, n_nl, offs->as<unsigned long long>());
+  c->launches++;
+  ytc::timer_end(c, "stream_lines");
+  return 0;
+}
+
+void yttm_add_base(yttm_ctx *c, unsigned long long *off, uint64_t n, unsigned long long base) {
+  add_base_kernel<<<(unsigned)std::max<uint64_t>(std::min<uint64_t>((n + 255) / 256, (uint64_t)c->n_sm * 4), 1), 256, 0,
+                    c->stream>>>(off, n, base);
+  c->launches++;
+}
+
+void yttm_pipe_free(yttm_piece_pipe *p) {
+  yttm_enc *e = p->e;
   cudaStreamSynchronize(e->ctx->stream);
   cudaStreamSynchronize(e->s_in);
   cudaStreamSynchronize(e->s_out);
   for (int i = 0; i < 2; i++) {
-    if (s->stage[i]) cudaFreeHost(s->stage[i]);
-    if (s->out[i]) cudaFreeHost(s->out[i]);
-    s->tiles[i].release();
-    s->fmt[i].release();
-    s->lines_buf[i].release();
+    if (p->stage[i]) cudaFreeHost(p->stage[i]);
+    if (p->ends[i]) cudaFreeHost(p->ends[i]);
+    if (p->out[i]) cudaFreeHost(p->out[i]);
+    p->stage[i] = p->ends[i] = p->out[i] = nullptr;
   }
-  e->stream = nullptr;
-  delete s;
 }
 
 namespace {
@@ -1998,6 +2005,169 @@ int pinned_reserve(yttm_ctx *c, uint8_t **p, uint64_t *cap, uint64_t need, uint6
   return 0;
 }
 
+// The kernels of the piece in slot s, then its copy out (line ends after the data, 8-byte aligned).
+int pipe_run(yttm_piece_pipe *p, int s) {
+  yttm_enc *e = p->e;
+  yttm_ctx *c = e->ctx;
+  yttm_piece_pipe::Piece &P = p->pc[s];
+  YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_in[s], 0));
+  const void *data = nullptr;
+  const unsigned long long *ends = nullptr;
+  if (p->run(p->owner, s, &data, &ends)) return 1;
+  YT_CUDA(c, cudaGetLastError());
+  YT_CUDA(c, cudaEventRecord(e->ev_done[s], c->stream));
+  const uint64_t ends_at = (P.n_out + 7) & ~7ull;
+  if (pinned_reserve(c, &p->out[s], &p->out_cap[s], ends_at + P.n_lines * 8, 0)) return 1;
+  YT_CUDA(c, cudaStreamWaitEvent(e->s_out, e->ev_done[s], 0));
+  if (P.n_out) YT_CUDA(c, cudaMemcpyAsync(p->out[s], data, P.n_out, cudaMemcpyDeviceToHost, e->s_out));
+  YT_CUDA(c, cudaMemcpyAsync(p->out[s] + ends_at, ends, P.n_lines * 8, cudaMemcpyDeviceToHost, e->s_out));
+  YT_CUDA(c, cudaEventRecord(e->ev_out[s], e->s_out));
+  return 0;
+}
+
+// The results of the piece in slot s to the sink, once their copy out has completed.
+int pipe_deliver(yttm_piece_pipe *p, int s) {
+  yttm_ctx *c = p->e->ctx;
+  const yttm_piece_pipe::Piece &P = p->pc[s];
+  YT_CUDA(c, cudaEventSynchronize(p->e->ev_out[s]));
+  const int rc = p->sink(p->user, p->out[s], P.n_out, reinterpret_cast<const uint64_t *>(p->out[s] + ((P.n_out + 7) & ~7ull)),
+                         P.n_lines);
+  if (rc) YT_FAIL(c, std::string(p->who) + ": the sink failed (it returned " + std::to_string(rc) + ")");
+  return 0;
+}
+
+// Staging buffer cur holds a piece in its first `cut` bytes (and, for id pieces, its n_ends line ends): copy it in (slot
+// cur), move what follows to the other staging buffer, run the piece before it and hand the one before that to the sink.
+int pipe_submit(yttm_piece_pipe *p, uint64_t cut) {
+  yttm_enc *e = p->e;
+  yttm_ctx *c = e->ctx;
+  const int s = p->cur, o = s ^ 1;
+  const uint64_t tail = p->len - cut;
+  YT_CUDA(c, cudaEventSynchronize(e->ev_in[o]));  // the piece before has been copied in from staging buffer o
+  if (pinned_reserve(c, &p->stage[o], &p->stage_cap[o], std::max(tail, p->piece), 0)) return 1;
+  if (tail) std::memcpy(p->stage[o], p->stage[s] + cut, tail);
+  const uint64_t ends_at = (cut + 15) & ~15ull, need = p->unit ? ends_at + (p->n_ends + 1) * 8 + 16 : cut + 16;
+  ytc::DevBuf &in = *p->dev_in[s];
+  if (need > in.cap) YT_CUDA(c, cudaEventSynchronize(e->ev_done[s]));  // replaced: the kernels of piece i-2 are done with it
+  YT_CUDA(c, in.reserve(need));
+  YT_CUDA(c, cudaStreamWaitEvent(e->s_in, e->ev_done[s], 0));
+  if (cut) YT_CUDA(c, cudaMemcpyAsync(in.p, p->stage[s], cut, cudaMemcpyHostToDevice, e->s_in));
+  yttm_piece_pipe::Piece next;  // pc[s] still describes piece i - 2 until it is delivered
+  next.n_bytes = cut;
+  if (p->unit) {
+    YT_CUDA(c, cudaMemcpyAsync(in.as<uint8_t>() + ends_at, p->ends[s], (p->n_ends + 1) * 8, cudaMemcpyHostToDevice, e->s_in));
+    if (pinned_reserve(c, &p->ends[o], &p->ends_cap[o], 8, 0)) return 1;
+    next.first_id = reinterpret_cast<const uint64_t *>(p->ends[s])[0];
+    reinterpret_cast<uint64_t *>(p->ends[o])[0] = reinterpret_cast<const uint64_t *>(p->ends[s])[p->n_ends];
+    next.n_lines = p->n_ends;
+    p->n_ends = 0;
+  } else {
+    next.open_end = p->stage[s][cut - 1] != '\n';
+  }
+  YT_CUDA(c, cudaEventRecord(e->ev_in[s], e->s_in));
+  if (p->to_run >= 0 && pipe_run(p, p->to_run)) return 1;
+  if (p->to_deliver >= 0 && pipe_deliver(p, p->to_deliver)) return 1;
+  p->pc[s] = next;
+  p->to_deliver = p->to_run;
+  p->to_run = s;
+  p->cur = o;
+  p->len = p->nonl = tail;  // what follows the last '\n' holds none
+  return 0;
+}
+
+}  // namespace
+
+int yttm_pipe_feed_text(yttm_piece_pipe *p, const char *bytes, uint64_t n) {
+  yttm_ctx *c = p->e->ctx;
+  YT_CUDA(c, cudaSetDevice(c->device));
+  while (n) {
+    const uint64_t room = p->len < p->piece ? p->piece - p->len : p->piece;
+    const uint64_t take = std::min(n, room);
+    if (pinned_reserve(c, &p->stage[p->cur], &p->stage_cap[p->cur], p->len + take, p->len)) return 1;
+    std::memcpy(p->stage[p->cur] + p->len, bytes, take);
+    p->len += take;
+    p->bytes_in += take;
+    bytes += take;
+    n -= take;
+    if (p->len < p->piece) continue;
+    const void *nl = memrchr(p->stage[p->cur] + p->nonl, '\n', p->len - p->nonl);
+    if (!nl) { p->nonl = p->len; continue; }  // no '\n' yet: the piece grows until one comes
+    if (pipe_submit(p, (uint64_t)(static_cast<const uint8_t *>(nl) - p->stage[p->cur]) + 1)) return 1;
+  }
+  return 0;
+}
+
+// A piece holds lines while its ids and line ends (8 bytes each) fit the nominal size; a longer line is a piece alone.
+int yttm_pipe_feed_lines(yttm_piece_pipe *p, const void *ids, uint64_t n_ids, const uint64_t *line_ends, uint64_t n_lines) {
+  yttm_ctx *c = p->e->ctx;
+  YT_CUDA(c, cudaSetDevice(c->device));
+  const uint64_t call_base = p->ids_in;
+  uint64_t at = 0;
+  while (at < n_lines) {
+    const uint64_t first = at ? line_ends[at - 1] : call_base;
+    uint64_t size = p->len + 8 * p->n_ends, prev = first, k = at;
+    for (; k < n_lines; k++) {
+      const uint64_t b = (line_ends[k] - prev) * p->unit + 8;
+      if (size + b > p->piece && size > 0) break;
+      size += b;
+      prev = line_ends[k];
+    }
+    const uint64_t nb = (prev - first) * p->unit, s = p->cur;
+    if (!p->ends[s]) {  // the first piece: its line ends start at 0
+      if (pinned_reserve(c, &p->ends[s], &p->ends_cap[s], 8, 0)) return 1;
+      reinterpret_cast<uint64_t *>(p->ends[s])[0] = 0;
+    }
+    if (pinned_reserve(c, &p->stage[s], &p->stage_cap[s], p->len + nb, p->len)) return 1;
+    if (nb) std::memcpy(p->stage[s] + p->len, static_cast<const uint8_t *>(ids) + (first - call_base) * p->unit, nb);
+    if (pinned_reserve(c, &p->ends[s], &p->ends_cap[s], (p->n_ends + 1 + k - at) * 8, (p->n_ends + 1) * 8)) return 1;
+    std::memcpy(p->ends[s] + (p->n_ends + 1) * 8, line_ends + at, (k - at) * 8);
+    p->len += nb;
+    p->n_ends += k - at;
+    at = k;
+    if (at < n_lines && pipe_submit(p, p->len)) return 1;  // the next line does not fit
+  }
+  p->ids_in += n_ids;
+  return 0;
+}
+
+int yttm_pipe_end(yttm_piece_pipe *p) {
+  yttm_ctx *c = p->e->ctx;
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if ((p->unit ? p->n_ends : p->len) && pipe_submit(p, p->len)) return 1;  // the last piece ends with the stream
+  const int last = p->to_run;
+  if (last >= 0 && pipe_run(p, last)) return 1;
+  if (p->to_deliver >= 0 && pipe_deliver(p, p->to_deliver)) return 1;
+  if (last >= 0 && pipe_deliver(p, last)) return 1;
+  return 0;
+}
+
+// ---- the encode stream ----
+
+struct yttm_enc_stream {
+  yttm_enc *e = nullptr;
+  int bos = 0, eos = 0, reverse = 0, format = YTTM_STREAM_IDS32;
+  double dropout = 0;
+  uint64_t seed = 0, first = 0;
+  yttm_piece_pipe pipe;
+  ytc::DevBuf tiles[2], fmt[2], lines_buf[2];  // per slot: '\n' per tile + bases; 16-bit ids or text; text per line
+  uint64_t lines = 0, ids = 0;
+};
+
+void yttm_enc_stream_free(yttm_enc_stream *s) {
+  if (!s) return;
+  yttm_enc *e = s->e;
+  yttm_pipe_free(&s->pipe);
+  for (int i = 0; i < 2; i++) {
+    s->tiles[i].release();
+    s->fmt[i].release();
+    s->lines_buf[i].release();
+  }
+  e->stream = nullptr;
+  delete s;
+}
+
+namespace {
+
 // "stream_dev_peak_bytes": every device buffer of the encoder, sampled after each piece
 void note_stream_peak(yttm_enc *e) {
   uint64_t sum = e->cp2id.cap + e->rules.cap + e->sub_table.cap;
@@ -2006,29 +2176,16 @@ void note_stream_peak(yttm_enc *e) {
   e->ctx->enc_stream_peak = std::max(e->ctx->enc_stream_peak, (double)sum);
 }
 
-// The kernels of the piece in slot s, then its copy out (line ends after the data, 8-byte aligned).
-int stream_encode(yttm_enc *e, int s) {
+// The kernels of the piece in slot s (yttm_piece_pipe::run).
+int stream_encode(void *owner, int s, const void **out_data, const unsigned long long **out_ends) {
+  yttm_enc_stream *S = static_cast<yttm_enc_stream *>(owner);
+  yttm_enc *e = S->e;
   yttm_ctx *c = e->ctx;
-  yttm_enc_stream *S = e->stream;
-  yttm_enc_stream::Piece &P = S->pc[s];
+  yttm_piece_pipe::Piece &P = S->pipe.pc[s];
   yttm_enc::Slot &sl = e->slot[s];
   const uint8_t *d = sl.d_bytes.as<uint8_t>();
-  const uint64_t n = P.n_bytes, nt = (n + LS_TILE - 1) / LS_TILE;
-  YT_CUDA(c, cudaStreamWaitEvent(c->stream, e->ev_in[s], 0));
-  YT_CUDA(c, S->tiles[s].reserve((2 * nt + 2) * 8));
-  unsigned long long *tile_nl = S->tiles[s].as<unsigned long long>(), *tile_base = tile_nl + nt, *n_nl = tile_base + nt;
-  ytc::timer_begin(c, "stream_lines");
-  line_count_kernel<<<(unsigned)nt, LS_T, 0, c->stream>>>(d, n, tile_nl);
-  c->launches++;
-  if (yttm_device_scan_u64(c, tile_nl, nt, tile_base, n_nl)) return 1;
-  unsigned long long h_nl = 0;
-  YT_CUDA(c, cudaMemcpyAsync(&h_nl, n_nl, 8, cudaMemcpyDeviceToHost, c->stream));
-  YT_CUDA(c, cudaStreamSynchronize(c->stream));
-  P.n_lines = h_nl + (P.open_end ? 1 : 0);
-  YT_CUDA(c, sl.d_offs.reserve((P.n_lines + 2) * 8));
-  line_write_kernel<<<(unsigned)nt, LS_T, 0, c->stream>>>(d, n, tile_base, n_nl, sl.d_offs.as<unsigned long long>());
-  c->launches++;
-  ytc::timer_end(c, "stream_lines");
+  const uint64_t n = P.n_bytes;
+  if (yttm_line_split(c, d, n, P.open_end, &S->tiles[s], &sl.d_offs, &P.n_lines)) return 1;
   uint64_t n_ids = 0;
   if (enc_device(e, &sl, d, sl.d_offs.as<uint64_t>(), n, P.n_lines, S->bos, S->eos, S->reverse, S->dropout, S->seed,
                  S->first + S->lines, &n_ids))
@@ -2060,95 +2217,14 @@ int stream_encode(yttm_enc *e, int s) {
     data = S->fmt[s].p;
     P.n_out = text_bytes;
   }
-  if (S->ids)
-    add_base_kernel<<<(unsigned)std::max<uint64_t>(std::min<uint64_t>((P.n_lines + 255) / 256, (uint64_t)c->n_sm * 4), 1),
-                      256, 0, c->stream>>>(id_off + 1, P.n_lines, (unsigned long long)S->ids);
-  c->launches += S->ids ? 1 : 0;
+  if (S->ids) yttm_add_base(c, id_off + 1, P.n_lines, (unsigned long long)S->ids);
   ytc::timer_end(c, "stream_format");
-  YT_CUDA(c, cudaGetLastError());
-  YT_CUDA(c, cudaEventRecord(e->ev_done[s], c->stream));
-  const uint64_t ends_at = (P.n_out + 7) & ~7ull;
-  if (pinned_reserve(c, &S->out[s], &S->out_cap[s], ends_at + P.n_lines * 8, 0)) return 1;
-  YT_CUDA(c, cudaStreamWaitEvent(e->s_out, e->ev_done[s], 0));
-  if (P.n_out) YT_CUDA(c, cudaMemcpyAsync(S->out[s], data, P.n_out, cudaMemcpyDeviceToHost, e->s_out));
-  YT_CUDA(c, cudaMemcpyAsync(S->out[s] + ends_at, id_off + 1, P.n_lines * 8, cudaMemcpyDeviceToHost, e->s_out));
-  YT_CUDA(c, cudaEventRecord(e->ev_out[s], e->s_out));
+  *out_data = data;
+  *out_ends = id_off + 1;
   S->lines += P.n_lines;
   S->ids += n_ids;
   c->enc_stream_pieces += 1;
   note_stream_peak(e);
-  return 0;
-}
-
-// The results of the piece in slot s to the sink, once their copy out has completed.
-int stream_deliver(yttm_enc *e, int s) {
-  yttm_ctx *c = e->ctx;
-  yttm_enc_stream *S = e->stream;
-  const yttm_enc_stream::Piece &P = S->pc[s];
-  YT_CUDA(c, cudaEventSynchronize(e->ev_out[s]));
-  const int rc = S->sink(S->user, S->out[s], P.n_out, reinterpret_cast<const uint64_t *>(S->out[s] + ((P.n_out + 7) & ~7ull)),
-                         P.n_lines);
-  if (rc) YT_FAIL(c, "yttm_enc_stream: the sink failed (it returned " + std::to_string(rc) + ")");
-  return 0;
-}
-
-// Staging buffer cur holds a piece in its first `cut` bytes: copy it in (slot cur), move what follows to the other
-// staging buffer, encode the piece before it and hand the one before that to the sink.
-int stream_submit(yttm_enc *e, uint64_t cut) {
-  yttm_ctx *c = e->ctx;
-  yttm_enc_stream *S = e->stream;
-  const int s = S->cur, o = s ^ 1;
-  const uint64_t tail = S->len - cut;
-  YT_CUDA(c, cudaEventSynchronize(e->ev_in[o]));  // the piece before has been copied in from staging buffer o
-  if (pinned_reserve(c, &S->stage[o], &S->stage_cap[o], std::max(tail, S->piece), 0)) return 1;
-  if (tail) std::memcpy(S->stage[o], S->stage[s] + cut, tail);
-  yttm_enc::Slot &sl = e->slot[s];
-  if (cut + 16 > sl.d_bytes.cap) YT_CUDA(c, cudaEventSynchronize(e->ev_done[s]));  // replaced: the kernels of piece i-2 are done with it
-  YT_CUDA(c, sl.d_bytes.reserve(cut + 16));
-  YT_CUDA(c, cudaStreamWaitEvent(e->s_in, e->ev_done[s], 0));
-  YT_CUDA(c, cudaMemcpyAsync(sl.d_bytes.p, S->stage[s], cut, cudaMemcpyHostToDevice, e->s_in));
-  YT_CUDA(c, cudaEventRecord(e->ev_in[s], e->s_in));
-  S->pc[s].n_bytes = cut;
-  S->pc[s].open_end = S->stage[s][cut - 1] != '\n';
-  if (S->to_encode >= 0 && stream_encode(e, S->to_encode)) return 1;
-  if (S->to_deliver >= 0 && stream_deliver(e, S->to_deliver)) return 1;
-  S->to_deliver = S->to_encode;
-  S->to_encode = s;
-  S->cur = o;
-  S->len = S->nonl = tail;  // what follows the last '\n' holds none
-  return 0;
-}
-
-int stream_feed(yttm_enc *e, const char *bytes, uint64_t n) {
-  yttm_ctx *c = e->ctx;
-  yttm_enc_stream *S = e->stream;
-  YT_CUDA(c, cudaSetDevice(c->device));
-  while (n) {
-    const uint64_t room = S->len < S->piece ? S->piece - S->len : S->piece;
-    const uint64_t take = std::min(n, room);
-    if (pinned_reserve(c, &S->stage[S->cur], &S->stage_cap[S->cur], S->len + take, S->len)) return 1;
-    std::memcpy(S->stage[S->cur] + S->len, bytes, take);
-    S->len += take;
-    S->bytes_in += take;
-    bytes += take;
-    n -= take;
-    if (S->len < S->piece) continue;
-    const void *nl = memrchr(S->stage[S->cur] + S->nonl, '\n', S->len - S->nonl);
-    if (!nl) { S->nonl = S->len; continue; }  // no '\n' yet: the piece grows until one comes
-    if (stream_submit(e, (uint64_t)(static_cast<const uint8_t *>(nl) - S->stage[S->cur]) + 1)) return 1;
-  }
-  return 0;
-}
-
-int stream_end(yttm_enc *e) {
-  yttm_ctx *c = e->ctx;
-  yttm_enc_stream *S = e->stream;
-  YT_CUDA(c, cudaSetDevice(c->device));
-  if (S->len && stream_submit(e, S->len)) return 1;  // the last piece ends with the stream
-  const int last = S->to_encode;
-  if (last >= 0 && stream_encode(e, last)) return 1;
-  if (S->to_deliver >= 0 && stream_deliver(e, S->to_deliver)) return 1;
-  if (last >= 0 && stream_deliver(e, last)) return 1;
   return 0;
 }
 
@@ -2175,12 +2251,21 @@ int yttm_enc_stream_begin(yttm_enc *e, int bos, int eos, int reverse, double dro
   if (format == YTTM_STREAM_IDS16 && e->vocab > 65536)
     YT_FAIL(c, "yttm_enc_stream_begin: 16-bit ids need a vocabulary of at most 65536 (this model has " +
                    std::to_string(e->vocab) + ")");
-  if (pipe_init(e)) return 1;
+  if (yttm_pipe_init(e)) return 1;
   yttm_enc_stream *S = new yttm_enc_stream();
   S->e = e;
   S->bos = bos; S->eos = eos; S->reverse = reverse; S->dropout = dropout; S->seed = seed;
-  S->first = first_sentence_index; S->format = format; S->sink = sink; S->user = user;
-  S->piece = (uint64_t)ytc::env_int("YTTM_ENC_STREAM_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;
+  S->first = first_sentence_index; S->format = format;
+  yttm_piece_pipe &p = S->pipe;
+  p.e = e;
+  p.piece = (uint64_t)ytc::env_int("YTTM_ENC_STREAM_PIECE_KB", 32 << 10, 1, INT_MAX) << 10;
+  p.dev_in[0] = &e->slot[0].d_bytes;
+  p.dev_in[1] = &e->slot[1].d_bytes;
+  p.run = stream_encode;
+  p.owner = S;
+  p.sink = sink;
+  p.user = user;
+  p.who = "yttm_enc_stream";
   e->stream = S;
   c->enc_stream_pieces = 0;
   c->enc_stream_peak = 0;
@@ -2190,16 +2275,16 @@ int yttm_enc_stream_begin(yttm_enc *e, int bos, int eos, int reverse, double dro
 int yttm_enc_stream_feed(yttm_enc *e, const char *bytes, uint64_t n) {
   if (!e) return yttm_enc_check(e, "yttm_enc_stream_feed", 0, 0);
   if (!e->stream) YT_FAIL(e->ctx, "yttm_enc_stream_feed: yttm_enc_stream_begin has not run");
-  return stream_feed(e, bytes, n) ? stream_failed(e) : 0;
+  return yttm_pipe_feed_text(&e->stream->pipe, bytes, n) ? stream_failed(e) : 0;
 }
 
 int yttm_enc_stream_end(yttm_enc *e, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes_in) {
   if (!e) return yttm_enc_check(e, "yttm_enc_stream_end", 0, 0);
   if (!e->stream) YT_FAIL(e->ctx, "yttm_enc_stream_end: yttm_enc_stream_begin has not run");
-  if (stream_end(e)) return stream_failed(e);
+  if (yttm_pipe_end(&e->stream->pipe)) return stream_failed(e);
   if (n_lines) *n_lines = e->stream->lines;
   if (n_ids) *n_ids = e->stream->ids;
-  if (n_bytes_in) *n_bytes_in = e->stream->bytes_in;
+  if (n_bytes_in) *n_bytes_in = e->stream->pipe.bytes_in;
   yttm_enc_stream_free(e->stream);
   return 0;
 }

@@ -1037,6 +1037,8 @@ double yttm_stage_ms(const yttm_ctx *c, const char *stage) {
   if (!std::strcmp(stage, "enc_chunks")) return c->enc_chunks;
   if (!std::strcmp(stage, "stream_pieces")) return c->enc_stream_pieces;
   if (!std::strcmp(stage, "stream_dev_peak_bytes")) return c->enc_stream_peak;
+  if (!std::strcmp(stage, "dec_stream_pieces")) return c->dec_stream_pieces;
+  if (!std::strcmp(stage, "dec_stream_dev_peak_bytes")) return c->dec_stream_peak;
   if (!std::strcmp(stage, "loop_refreshes")) return (double)c->loop_sweeps;
   if (!std::strcmp(stage, "loop_launches")) return (double)c->loop_relaunches;
   if (!std::strcmp(stage, "table_capacity")) return (double)c->pcap;

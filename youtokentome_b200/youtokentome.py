@@ -4,7 +4,8 @@ meaning, return types and exceptions (ValueError(status.message), TypeError for 
 types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path, optionally with the source byte
 span of every id), `encode_padded` (the same ids as padded, truncated [N, L] rows with their lengths),
 `encode_subwords_packed` (the subword pieces on the GPU), `encode_file` (a file of any size, line by line, to .npy files
-or the CLI's text), `decode_packed` (the inverse of `encode_packed`, on the GPU) and `dropout_seed`."""
+or the CLI's text), `decode_packed` (the inverse of `encode_packed`, on the GPU), `decode_file` (the inverse of
+`encode_file`: either of its outputs, of any size, back to text on the GPU) and `dropout_seed`."""
 import ctypes as C
 import os
 import sys
@@ -505,6 +506,52 @@ class BPE:
                 sys.stdout.flush()
             rc = _lib.lib().yttm_api_encode_file(self._h, fd, os.fsencode(output), int(text), int(bos), int(eos),
                                                  int(reverse), float(dropout_prob), stats.ctypes.data)
+        finally:
+            if opened is not None:
+                os.close(opened)
+        if rc != 0:
+            raise self._err()
+        return {"lines": int(stats[0]), "ids": int(stats[1]), "bytes": int(stats[2])}
+
+    def decode_file(self, input, output, ignore_ids: Optional[Collection] = None, text=False) -> dict:
+        """Decodes ids of any size on the GPU, line by line, to what `yttm decode` prints for them: every line's decode
+        followed by "\\n", to <output> or to stdout when output is "-".  `input`:
+          text=False  the prefix of the pair encode_file writes (or np.save does): <input>.ids.npy, 1-D uint16 or int32,
+                      and <input>.offsets.npy, 1-D uint64 from 0, non-decreasing, ending at len(ids): line i is
+                      ids[offsets[i]:offsets[i+1]];
+          text=True   id text (a path, an int file descriptor or an object with fileno(), read to its end), split into
+                      lines as std::getline splits it; a line's ids are those `yttm decode` reads from it.
+        ignore_ids as for decode.  A failed call leaves nothing at <output> (with "-", lines before the failing piece
+        may have been written).  Returns {"lines", "ids", "bytes"} (text bytes written)."""
+        if not isinstance(ignore_ids, Collection) and ignore_ids is not None:
+            raise TypeError("{} is not a Collection instance".format(type(ignore_ids)))
+        ign = np.asarray(sorted({int(i) for i in ignore_ids if -2**31 <= int(i) < 2**31}) if ignore_ids else [],
+                         dtype=np.int32)
+        output = os.fspath(output)
+        opened, fd, prefix = None, -1, None
+        if not text:
+            if not isinstance(input, (str, bytes, os.PathLike)):
+                raise TypeError("input must be the prefix of <input>.ids.npy and <input>.offsets.npy, not %s" %
+                                type(input).__name__)
+            prefix = os.fsencode(input)
+        elif isinstance(input, (str, bytes, os.PathLike)):
+            try:
+                fd = opened = os.open(input, os.O_RDONLY | getattr(os, "O_CLOEXEC", 0))
+            except OSError as e:
+                raise ValueError("decode_file: cannot open '%s': %s" % (os.fsdecode(input), e.strerror)) from None
+        elif isinstance(input, int) and not isinstance(input, bool):
+            fd = input
+        elif hasattr(input, "fileno"):
+            fd = input.fileno()
+        else:
+            raise TypeError("input must be a path, a file descriptor or an object with fileno(), not %s" %
+                            type(input).__name__)
+        stats = np.zeros(3, dtype=np.uint64)
+        try:
+            if output == "-":
+                sys.stdout.flush()
+            rc = _lib.lib().yttm_api_decode_file(self._h, fd, prefix, os.fsencode(output), int(bool(text)),
+                                                 ign.ctypes.data, len(ign), stats.ctypes.data)
         finally:
             if opened is not None:
                 os.close(opened)

@@ -1,4 +1,4 @@
-"""`yttm bpe | encode | encode_file | decode | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
+"""`yttm bpe | encode | encode_file | decode | decode_file | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
 same sub-commands, option names, defaults and stdin/stdout framing) over the CUDA library.
 Run as `python -m youtokentome_b200.yttm_cli ...`.  `--n_threads` is accepted and ignored."""
 import sys
@@ -79,6 +79,23 @@ def _ignore_ids(ctx, param, value):
 def decode(model, ignore_ids):
     """Decode ids to text."""
     BPE(model).decode_cli(ignore_ids)
+
+
+@main.command("decode_file")
+@click.option("--model", type=click.Path(exists=True), required=True, help="Path to file with learned model.")
+@click.option("--input", "input_", type=click.STRING, required=True,
+              help="Prefix of <input>.ids.npy and <input>.offsets.npy; with --text the id text file, '-' for stdin.")
+@click.option("--output", type=click.STRING, required=True, help="Text file to write, '-' for stdout.")
+@click.option("--text", is_flag=True, help="Read the ids as text, as `decode` does.")
+@click.option("--ignore_ids", type=click.STRING, callback=_ignore_ids, required=False,
+              help="List of indices to ignore for decoding. Example: --ignore_ids=1,2,3")
+def decode_file(model, input_, output, text, ignore_ids):
+    """Decode ids of any size on the GPU, line by line."""
+    if input_ == "-" and not text:
+        raise click.BadParameter("'-' (stdin) needs --text", param_hint="--input")
+    src = sys.stdin.buffer if input_ == "-" else input_
+    r = BPE(model).decode_file(src, output, ignore_ids=ignore_ids, text=text)
+    click.echo("decode_file: %d lines, %d ids, %d bytes" % (r["lines"], r["ids"], r["bytes"]), err=True)
 
 
 @main.command()
