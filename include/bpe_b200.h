@@ -118,6 +118,30 @@ Status train_bpe(const std::string &input_path, const std::string &model_path, i
 Status learn_bpe_from_string(std::string &text_utf8, int n_tokens, const std::string &output_file,
                              BpeConfig bpe_config, BPEState *bpe_state);
 
+// A word-count table: word i is bytes[offsets[i], offsets[i+1]) occurring counts[i] times; `separators` separator units
+// and data_len decode units in the text it stands for.
+struct WordCounts {
+  std::string bytes;
+  std::vector<uint64_t> offsets{0}, counts;
+  uint64_t separators = 0, data_len = 0;
+};
+// Feeds the text of in_fd (a file or a pipe; in_fd < 0: the buffer text[n]) through the GPU as train_bpe feeds a
+// corpus and gives its table, sorted by count descending, then by bytes ascending.  tsv_path ("" none, "-" stdout)
+// receives it as TSV: the line "\t<separators>", then one "word\tcount" line per entry.
+Status count_words(int in_fd, const char *text, uint64_t n, const std::string &tsv_path, WordCounts *out);
+// Trains from a word-count table and writes the model train_bpe writes for any text with the same words, counts and
+// separators.  The table is the arrays of yttm_train_feed_words (on_device: device memory; separators UINT64_MAX: the
+// sum of the counts) or, when tsv_path is not empty, a TSV file as count_words writes it, read in blocks (without the
+// separator line: one separator per occurrence).
+struct CountsInput {
+  const uint8_t *bytes = nullptr;
+  const uint64_t *offsets = nullptr, *counts = nullptr;
+  uint64_t n = 0, separators = UINT64_MAX;
+  int on_device = 0;
+  std::string tsv_path;
+};
+Status train_counts(const CountsInput &in, const std::string &model_path, int vocab_size, BpeConfig config);
+
 // compute_alphabet_helper (bpe.cpp:316-355) on a sparse histogram.
 flat_hash_map<uint32_t, uint32_t> compute_alphabet_helper(const flat_hash_map<uint32_t, uint64_t> &char_cnt,
                                                           uint64_t data_len,

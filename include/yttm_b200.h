@@ -67,6 +67,26 @@ int yttm_train_feed_begin(yttm_ctx *ctx);
 int yttm_train_feed(yttm_ctx *ctx, const char *bytes, uint64_t n);
 int yttm_train_feed_end(yttm_ctx *ctx, uint64_t *data_len, uint64_t *n_distinct);
 
+/* A word-count table fed between feed_begin and feed_end, any number of times and mixed with feed's text blocks
+ * (everything fed adds up; a list does not split the text fed around it).  Entry i is the word
+ * bytes[offsets[i], offsets[i+1]) occurring counts[i] times (n entries, n + 1 offsets, uint64 counts; 0 contributes
+ * nothing, equal words add up); `separators` is the number of separator units of the text the list stands for
+ * (UINT64_MAX: the sum of its counts).  After feed_end the context holds what feeding such a text would leave:
+ * data_len = sum of counts x units (invalid bytes included) + separators, the histogram = counts x code points.
+ * on_device != 0: the three arrays are device memory, read in place; else they are host memory, copied through the
+ * feed's pinned staging before the call returns.  A list longer than a piece (YTTM_TRAIN_FEED_PIECE_KB) is processed
+ * in pieces.  Fails, naming the entry, on an empty entry or one holding a separator unit (whitespace byte or U+2581),
+ * and when data_len or the separators would pass 2^64; feed_end fails when the lists' separators are fewer than their
+ * occurrences minus one (no text has them).  A failed list ends the feed (feed_begin again). */
+int yttm_train_feed_words(yttm_ctx *ctx, const uint8_t *bytes, const uint64_t *offsets, const uint64_t *counts,
+                          uint64_t n, uint64_t separators, int on_device);
+/* After feed_end and before build: the fed unique words (in no particular order), each once, into caller buffers:
+ * bytes[offsets[i], offsets[i+1]) occurring counts[i] times, offsets holding cap + 1 values; *separators (may be NULL)
+ * = data_len - sum of counts x units.  *n_unique and *n_bytes always receive the sizes.  0 ok, 1 error, 2 a buffer too
+ * small (nothing written; *separators is still set when asked for). */
+int yttm_train_fed_words(yttm_ctx *ctx, uint8_t *bytes, uint64_t bytes_cap, uint64_t *offsets, uint64_t *counts,
+                         uint64_t cap, uint64_t *n_unique, uint64_t *n_bytes, uint64_t *separators);
+
 /* Phase 1 — compute_char_count (bpe.cpp:839-857): *data_len = number of decode units (spaces
  * and invalid bytes included); histogram of valid non-space code points.  *n_distinct = number
  * of code points with a non-zero count. */

@@ -19,6 +19,19 @@ int yttm_api_train(const char *data_path, const char *model_path, int vocab_size
 /* learn_bpe_from_string (bpe.cpp:859) on an in-memory corpus; model_path may be "" */
 int yttm_api_train_memory(const char *text, uint64_t n, const char *model_path, int vocab_size, double coverage,
                           int pad_id, int unk_id, int bos_id, int eos_id);
+/* count_words (bpe_b200.h): the word-count table of the text of in_fd (a file or a pipe; in_fd < 0: text[n]), also
+ * written as TSV to tsv_path when it is not NULL ("-" = stdout).  sizes[4] = unique words, their bytes, separators,
+ * data_len.  0 ok, 1 error.  yttm_api_result_words then copies the table, sorted by count descending and bytes
+ * ascending, of this thread's last count_words: bytes[sizes[1]], offsets[sizes[0] + 1], counts[sizes[0]]. */
+int yttm_api_count_words(int in_fd, const char *text, uint64_t n, const char *tsv_path, uint64_t *sizes);
+void yttm_api_result_words(uint8_t *bytes, uint64_t *offsets, uint64_t *counts);
+/* train_counts (bpe_b200.h): trains from a word-count table, the arrays of yttm_train_feed_words (on_device != 0:
+ * device memory; separators UINT64_MAX: one per occurrence) or, when tsv_path is not NULL, a TSV file as count_words
+ * writes it.  The model and the errors are train_bpe's on any text with the same words, counts and separators. */
+int yttm_api_train_counts(const uint8_t *bytes, const uint64_t *offsets, const uint64_t *counts, uint64_t n,
+                          uint64_t separators, int on_device, const char *tsv_path, const char *model_path,
+                          int vocab_size, double coverage, int n_threads, int pad_id, int unk_id, int bos_id,
+                          int eos_id);
 /* sizes and stage times of the last training on this thread (see TrainReport); returns #values */
 int yttm_api_train_report(double *out, int n);
 /* frees the device buffers train_bpe keeps cached for the calling thread (vkcom::release_training_cache) */

@@ -8,6 +8,6 @@
 Both hot paths (training merge loop, batch encode) run as sm_90a CUDA kernels behind the C ABI
 in include/yttm_b200.h; there is no CPU fallback.
 """
-from .youtokentome import BPE, OutputType, release_training_cache, train_report  # noqa: F401
+from .youtokentome import BPE, OutputType, WordCounts, release_training_cache, train_report  # noqa: F401
 
-__all__ = ["BPE", "OutputType", "release_training_cache", "train_report"]
+__all__ = ["BPE", "OutputType", "WordCounts", "release_training_cache", "train_report"]

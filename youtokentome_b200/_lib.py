@@ -47,6 +47,9 @@ def bind(L):
         "yttm_api_train": (i32, [cp, cp, i32, dbl, i32, i32, i32, i32, i32]),
         "yttm_api_train_memory": (i32, [cp, u64, cp, i32, dbl, i32, i32, i32, i32]),
         "yttm_api_train_report": (i32, [vp, i32]),
+        "yttm_api_count_words": (i32, [i32, vp, u64, cp, vp]),
+        "yttm_api_result_words": (None, [vp, vp, vp]),
+        "yttm_api_train_counts": (i32, [vp, vp, vp, u64, u64, i32, cp, cp, i32, dbl, i32, i32, i32, i32, i32]),
         "yttm_api_release_training_cache": (None, []),
         "yttm_api_training_cache_held": (i32, []),
         "yttm_api_open": (vp, [cp, i32]),
@@ -97,6 +100,8 @@ def bind(L):
         "yttm_train_feed_begin": (i32, [vp]),
         "yttm_train_feed": (i32, [vp, vp, u64]),
         "yttm_train_feed_end": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),
+        "yttm_train_feed_words": (i32, [vp, vp, vp, vp, u64, u64, i32]),
+        "yttm_train_fed_words": (i32, [vp, vp, u64, vp, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
         "yttm_train_char_hist": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),
         "yttm_train_get_char_hist": (i32, [vp, vp, vp]),
         "yttm_train_char_hist_devptr": (i32, [vp, C.POINTER(vp), C.POINTER(u64)]),
@@ -155,6 +160,7 @@ def bind(L):
 EXPORTED_SYMBOLS_DEVICE_ABI = [
     "yttm_ctx_create", "yttm_ctx_destroy", "yttm_last_error", "yttm_device_count", "yttm_stage_ms",
     "yttm_launch_count", "yttm_train_load_corpus", "yttm_train_feed_begin", "yttm_train_feed", "yttm_train_feed_end",
+    "yttm_train_feed_words", "yttm_train_fed_words",
     "yttm_train_char_hist", "yttm_train_get_char_hist",
     "yttm_train_char_hist_devptr", "yttm_train_char_hist_refresh", "yttm_train_set_alphabet", "yttm_train_build",
     "yttm_train_export_words", "yttm_train_import_words", "yttm_train_dist_init", "yttm_train_dist_connect",

@@ -15,6 +15,7 @@
 #include <fstream>
 #include <functional>
 #include <sstream>
+#include <string_view>
 #include <thread>
 
 #include <fcntl.h>
@@ -506,6 +507,179 @@ Status train_bpe(const std::string &input_path, const std::string &model_path, i
   }, vocab_size, model_path, cfg, &state);
   g_report.read_s = read_s;
   return status;
+}
+
+// ---------------------------------------------------------------------------------------------
+// word-count tables
+// ---------------------------------------------------------------------------------------------
+static bool read_block(int fd, std::vector<char> &buf, size_t *got) {
+  *got = 0;
+  while (*got < buf.size()) {
+    const ssize_t r = ::read(fd, buf.data() + *got, buf.size() - *got);
+    if (r < 0 && errno == EINTR) continue;
+    if (r < 0) return false;
+    if (r == 0) break;
+    *got += (size_t)r;
+  }
+  return true;
+}
+
+static Status write_tsv(const WordCounts &t, const std::string &path) {
+  FILE *f = path == "-" ? stdout : std::fopen(path.c_str(), "wb");
+  if (!f) return Status(1, "count_words: cannot open '" + path + "' for writing");
+  std::fprintf(f, "\t%llu\n", (unsigned long long)t.separators);
+  for (size_t i = 0; i + 1 < t.offsets.size(); i++) {
+    std::fwrite(t.bytes.data() + t.offsets[i], 1, t.offsets[i + 1] - t.offsets[i], f);
+    std::fprintf(f, "\t%llu\n", (unsigned long long)t.counts[i]);
+  }
+  const bool ok = std::fflush(f) == 0 && !std::ferror(f);
+  if (f != stdout) std::fclose(f);
+  return ok ? Status() : Status(1, "count_words: failed to write '" + path + "'");
+}
+
+Status count_words(int in_fd, const char *text, uint64_t n, const std::string &tsv_path, WordCounts *out) {
+  yttm_ctx *ctx = nullptr;
+  if (yttm_ctx_create(default_device(), &ctx)) return Status(1, yttm_last_error(nullptr));
+  struct Destroy { yttm_ctx *c; ~Destroy() { yttm_ctx_destroy(c); } } destroy{ctx};
+  if (yttm_train_feed_begin(ctx)) return Status(1, ctx_err(ctx));
+  if (in_fd >= 0) {
+    std::vector<char> block(FEED_BLOCK);
+    for (size_t got = 0;;) {
+      if (!read_block(in_fd, block, &got)) return Status(1, std::string("count_words: read failed: ") + std::strerror(errno));
+      if (!got) break;
+      if (yttm_train_feed(ctx, block.data(), got)) return Status(1, ctx_err(ctx));
+    }
+  } else {
+    for (uint64_t at = 0; at < n; at += FEED_BLOCK)
+      if (yttm_train_feed(ctx, text + at, std::min(FEED_BLOCK, n - at))) return Status(1, ctx_err(ctx));
+  }
+  uint64_t data_len = 0, n_distinct = 0, U = 0, nb = 0, seps = 0;
+  if (yttm_train_feed_end(ctx, &data_len, &n_distinct)) return Status(1, ctx_err(ctx));
+  if (yttm_train_fed_words(ctx, nullptr, 0, nullptr, nullptr, 0, &U, &nb, nullptr) == 1) return Status(1, ctx_err(ctx));
+  std::string bytes(nb, '\0');
+  std::vector<uint64_t> offs(U + 1), cnts(U);
+  if (yttm_train_fed_words(ctx, reinterpret_cast<uint8_t *>(&bytes[0]), nb, offs.data(), cnts.data(), U, &U, &nb, &seps))
+    return Status(1, ctx_err(ctx));
+  std::vector<uint64_t> order(U);
+  for (uint64_t i = 0; i < U; i++) order[i] = i;
+  auto word = [&](uint64_t i) { return std::string_view(bytes.data() + offs[i], offs[i + 1] - offs[i]); };
+  std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) {
+    return cnts[a] != cnts[b] ? cnts[a] > cnts[b] : word(a) < word(b);
+  });
+  WordCounts &t = *out;
+  t = WordCounts();
+  t.bytes.reserve(nb);
+  t.counts.reserve(U);
+  t.offsets.reserve(U + 1);
+  for (uint64_t i : order) {
+    t.bytes += word(i);
+    t.offsets.push_back(t.bytes.size());
+    t.counts.push_back(cnts[i]);
+  }
+  t.separators = seps;
+  t.data_len = data_len;
+  return tsv_path.empty() ? Status() : write_tsv(t, tsv_path);
+}
+
+// A TSV word-count table read in blocks of FEED_BLOCK bytes and fed as word lists; the separator line ("\t<n>") may
+// stand anywhere, once.
+static std::string feed_tsv(yttm_ctx *ctx, const std::string &path) {
+  const int fd = ::open(path.c_str(), O_RDONLY);
+  if (fd < 0) return "train_from_counts: cannot open '" + path + "': " + std::strerror(errno);
+  struct Closer { int fd; ~Closer() { ::close(fd); } } closer{fd};
+  std::vector<char> block(FEED_BLOCK);
+  std::string carry;                       // a line cut by the end of a block
+  std::string wbytes;                      // the entries gathered for the next feed
+  std::vector<uint64_t> woff{0}, wcnt;
+  uint64_t line = 0, total = 0, seps = 0;
+  bool have_seps = false;
+  auto flush = [&]() -> std::string {
+    if (wcnt.empty()) return "";
+    if (yttm_train_feed_words(ctx, reinterpret_cast<const uint8_t *>(wbytes.data()), woff.data(), wcnt.data(),
+                              wcnt.size(), 0, 0))
+      return ctx_err(ctx);
+    wbytes.clear(); woff.assign(1, 0); wcnt.clear();
+    return "";
+  };
+  auto parse = [&](const char *p, size_t len) -> std::string {
+    line++;
+    const char *tab = static_cast<const char *>(std::memchr(p, '\t', len));
+    const std::string at = path + ", line " + std::to_string(line) + ": ";
+    if (!tab) return at + "no tab between the word and its count";
+    const char *c = tab + 1, *e = p + len;
+    if (c == e) return at + "the count is missing";
+    uint64_t v = 0;
+    for (const char *q = c; q < e; q++) {
+      if (*q < '0' || *q > '9') return at + "the count '" + std::string(c, e) + "' is not a non-negative integer";
+      const uint64_t d = (uint64_t)(*q - '0');
+      if (v > (UINT64_MAX - d) / 10) return at + "the count " + std::string(c, e) + " does not fit in 64 bits";
+      v = v * 10 + d;
+    }
+    const uint64_t wl = (uint64_t)(tab - p);
+    if (!wl) {
+      if (have_seps) return at + "a second separator line (empty word)";
+      have_seps = true;
+      seps = v;
+      return "";
+    }
+    for (uint64_t i = 0; i < wl; i++) {
+      const uint8_t b = (uint8_t)p[i];
+      if (yt::is_space_byte(b) || (b == 0xe2 && i + 2 < wl && (uint8_t)p[i + 1] == 0x96 && (uint8_t)p[i + 2] == 0x81))
+        return at + "the word contains a separator (a whitespace byte or U+2581)";
+    }
+    if (total + v < total) return at + "the counts sum past 2^64";
+    total += v;
+    wbytes.append(p, wl);
+    woff.push_back(wbytes.size());
+    wcnt.push_back(v);
+    return wbytes.size() >= FEED_BLOCK ? flush() : "";
+  };
+  for (size_t got = 0;;) {
+    if (!read_block(fd, block, &got)) return "train_from_counts: cannot read '" + path + "': " + std::strerror(errno);
+    if (!got) break;
+    const char *p = block.data(), *e = p + got;
+    while (p < e) {
+      const char *nl = static_cast<const char *>(std::memchr(p, '\n', e - p));
+      if (!nl) { carry.append(p, e); break; }
+      std::string err;
+      if (!carry.empty()) {
+        carry.append(p, nl);
+        err = parse(carry.data(), carry.size());
+        carry.clear();
+      } else {
+        err = parse(p, nl - p);
+      }
+      if (!err.empty()) return err;
+      p = nl + 1;
+    }
+  }
+  if (!carry.empty()) {   // a last line without its newline
+    std::string err = parse(carry.data(), carry.size());
+    if (!err.empty()) return err;
+  }
+  std::string err = flush();
+  if (!err.empty()) return err;
+  if (yttm_train_feed_words(ctx, nullptr, woff.data(), nullptr, 0, have_seps ? seps : total, 0)) return ctx_err(ctx);
+  return "";
+}
+
+Status train_counts(const CountsInput &in, const std::string &model_path, int vocab_size, BpeConfig cfg) {
+  Status status = check_config(cfg, vocab_size);
+  if (!status.ok()) return status;
+  print_config(in.tsv_path.empty() ? "<word counts>" : in.tsv_path, model_path, vocab_size, cfg);
+  g_report = TrainReport();
+  BPEState state;
+  return train_on_ctx([&](yttm_ctx *ctx) -> std::string {
+    std::cerr << "learning bpe from word counts..." << std::endl;
+    if (yttm_train_feed_begin(ctx)) return ctx_err(ctx);
+    if (!in.tsv_path.empty()) {
+      std::string err = feed_tsv(ctx, in.tsv_path);
+      if (!err.empty()) return err;
+    } else if (yttm_train_feed_words(ctx, in.bytes, in.offsets, in.counts, in.n, in.separators, in.on_device)) {
+      return ctx_err(ctx);
+    }
+    return yttm_train_feed_end(ctx, nullptr, nullptr) ? ctx_err(ctx) : "";
+  }, vocab_size, model_path, cfg, &state);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -63,6 +63,39 @@ int yttm_api_train_memory(const char *text, uint64_t n, const char *model_path, 
   return 0;
 }
 
+thread_local WordCounts g_counts;   // the table of the last yttm_api_count_words of this thread
+
+int yttm_api_count_words(int in_fd, const char *text, uint64_t n, const char *tsv_path, uint64_t *sizes) {
+  Status st = count_words(in_fd, text, n, tsv_path ? tsv_path : "", &g_counts);
+  if (!st.ok()) { g_counts = WordCounts(); return fail(nullptr, st.message); }
+  sizes[0] = g_counts.counts.size();
+  sizes[1] = g_counts.bytes.size();
+  sizes[2] = g_counts.separators;
+  sizes[3] = g_counts.data_len;
+  return 0;
+}
+
+void yttm_api_result_words(uint8_t *bytes, uint64_t *offsets, uint64_t *counts) {
+  std::memcpy(bytes, g_counts.bytes.data(), g_counts.bytes.size());
+  std::memcpy(offsets, g_counts.offsets.data(), g_counts.offsets.size() * 8);
+  std::memcpy(counts, g_counts.counts.data(), g_counts.counts.size() * 8);
+  g_counts = WordCounts();
+}
+
+int yttm_api_train_counts(const uint8_t *bytes, const uint64_t *offsets, const uint64_t *counts, uint64_t n,
+                          uint64_t separators, int on_device, const char *tsv_path, const char *model_path,
+                          int vocab_size, double coverage, int n_threads, int pad_id, int unk_id, int bos_id,
+                          int eos_id) {
+  CountsInput in;
+  in.bytes = bytes; in.offsets = offsets; in.counts = counts; in.n = n; in.separators = separators;
+  in.on_device = on_device;
+  in.tsv_path = tsv_path ? tsv_path : "";
+  BpeConfig cfg(coverage, n_threads, SpecialTokens(pad_id, unk_id, bos_id, eos_id));
+  Status st = train_counts(in, model_path, vocab_size, cfg);
+  if (!st.ok()) return fail(nullptr, st.message);
+  return 0;
+}
+
 void yttm_api_release_training_cache(void) { release_training_cache(); }
 int yttm_api_training_cache_held(void) { return training_cache_held(); }
 

@@ -102,6 +102,13 @@ struct yttm_ctx {
   cudaEvent_t ev_feed_copied[2] = {nullptr, nullptr}, ev_feed_done[2] = {nullptr, nullptr};
   uint64_t feed_wcap = 0, feed_fcap = 0, feed_fn = 0;   // per-piece / persistent table slots, persistent words
   uint64_t arena_len = 0, n_fed = 0, feed_pieces = 0;
+  // word lists fed between feed_begin and feed_end (yttm_train_feed_words): a piece of entries in wl_in (the staged
+  // host list), laid out as words each followed by one space in wl_text (positions in wl_pos); wl_acc = {units x counts,
+  // overflow flag, first bad entry}.  Their occurrences and separators add up on the host.
+  ytc::DevBuf wl_in, wl_text, wl_pos, wl_acc;
+  uint64_t wl_occ = 0, wl_seps = 0;
+  bool wl_fed = false;
+  bool fed_table = false;       // wpos / wfreq still hold the words feed_end left (no build has consumed them)
   uint64_t dev_peak = 0;        // largest sum of the DevBuf capacities of the current training
 
   // ---- packed words (double buffered for compaction)

@@ -20,6 +20,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <unistd.h>
 
 #include "common.cuh"
@@ -273,11 +274,81 @@ __global__ void __launch_bounds__(256) word_insert_list_kernel(const uint8_t *__
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   unsigned long long occ = 0;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_list; i += stride) {
+    if (!freq[i]) continue;   // a word listed with count 0 (yttm_train_feed_words) is no word of the text
     occ += freq[i];
     word_table_insert(s, n, base + pos[i], wt, counters, max_unique, (unsigned long long)freq[i]);
   }
   for (int o = 16; o > 0; o >>= 1) occ += __shfl_xor_sync(0xffffffffu, occ, o);
   if ((threadIdx.x & 31) == 0 && occ) atomicAdd(counters + 0, occ);
+}
+
+// a + b into *sum, raising *ovf when the true sum does not fit in 64 bits
+__device__ __forceinline__ void add_checked(uint64_t *sum, uint64_t b, bool *ovf) {
+  const uint64_t s = *sum + b;
+  if (s < b) *ovf = true;
+  *sum = s;
+}
+
+// A weighted word list (yttm_train_feed_words): entry i is bytes[off[i], off[i+1]) occurring cnt[i] times.  One pass
+// that lays the entries out as words each followed by one space (out, positions in pos: off[i] - off[0] + i), adds
+// cnt[i] per valid non-separator unit to the dense histogram, and adds cnt[i] x units to acc[0], the list's share of
+// data_len (acc[1] set when it would pass 2^64).  acc[2] receives the smallest index (plus first_index) of an entry
+// that is empty or holds a separator unit.  Units are decode_unit's, bounded by the entry: a sequence cut by the
+// entry's end is invalid there exactly as before the space that follows the word in a text.
+// Thread per entry (entries are short, about 6 - 10 bytes).  Unlike the text pass, one unit adds a count, not 1, so
+// the block bins for the hot low code points are 64-bit; a bin cannot overflow unless data_len does, which acc[1]
+// reports.
+__global__ void __launch_bounds__(256) word_list_layout_kernel(const uint8_t *__restrict__ bytes,
+                                                               const uint64_t *__restrict__ off,
+                                                               const uint64_t *__restrict__ cnt, uint64_t n_list,
+                                                               uint64_t first_index, uint8_t *__restrict__ out,
+                                                               uint64_t *__restrict__ pos,
+                                                               unsigned long long *__restrict__ hist,
+                                                               unsigned long long *acc) {
+  __shared__ unsigned long long sh[HIST_SMEM_BINS];
+  for (int i = threadIdx.x; i < HIST_SMEM_BINS; i += blockDim.x) sh[i] = 0;
+  __syncthreads();
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x, o0 = off[0];
+  uint64_t units_total = 0;
+  bool ovf = false;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_list; i += stride) {
+    const uint64_t a = off[i], len = off[i + 1] - a, c = cnt[i], p = a - o0 + i;
+    const uint8_t *w = bytes + a;
+    uint8_t *o = out + p;
+    pos[i] = p;
+    uint64_t units = 0;
+    bool bad = len == 0;
+    for (uint64_t q = 0; q < len;) {
+      uint32_t l;
+      const uint32_t cp = decode_unit(w, q, len, &l);
+      for (uint32_t k = 0; k < l; k++) o[q + k] = w[q + k];
+      q += l;
+      units++;
+      if (cp == INVALID_CP) continue;
+      if (is_space_cp(cp)) { bad = true; continue; }
+      if (!c) continue;
+      if (cp < HIST_SMEM_BINS) atomicAdd(&sh[cp], (unsigned long long)c);
+      else atomicAdd(hist + cp, (unsigned long long)c);
+    }
+    o[len] = ' ';
+    if (bad) atomicMin(acc + 2, (unsigned long long)(first_index + i));
+    if (c && ((c | units) >> 32) && units > ~0ull / c) ovf = true;
+    add_checked(&units_total, units * c, &ovf);
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    add_checked(&units_total, __shfl_xor_sync(0xffffffffu, units_total, o), &ovf);
+    ovf = __shfl_xor_sync(0xffffffffu, ovf ? 1 : 0, o) || ovf;
+  }
+  if ((threadIdx.x & 31) == 0) {
+    if (units_total) {
+      const unsigned long long was = atomicAdd(acc + 0, (unsigned long long)units_total);
+      if (was + units_total < was) ovf = true;
+    }
+    if (ovf) atomicExch(acc + 1, 1ull);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < HIST_SMEM_BINS; i += blockDim.x)
+    if (sh[i]) atomicAdd(hist + i, sh[i]);
 }
 
 // Multi-GPU export: unique word w of this rank goes to rank owner(w) = hash(bytes) % world (every rank uses the same
@@ -931,7 +1002,8 @@ std::vector<ytc::DevBuf *> ctx_bufs(yttm_ctx *c) {
   return {&c->text_buf, &c->hist, &c->cp2id, &c->wkey, &c->wcnt, &c->wpos, &c->wfreq, &c->wlen, &c->scan_tmp,
           &c->counters, &c->tok[0], &c->tok[1], &c->off[0], &c->off[1], &c->freq[0], &c->freq[1], &c->pkey, &c->pcnt,
           &c->scratch_key, &c->scratch_cnt, &c->ctl, &c->frontbuf, &c->tiles, &c->defer, &c->d_rules, &c->d_rfreq,
-          &c->xq_arrive, &c->xq_buf, &c->feed_dev[0], &c->feed_dev[1], &c->fkey, &c->fcnt, &c->arena};
+          &c->xq_arrive, &c->xq_buf, &c->feed_dev[0], &c->feed_dev[1], &c->fkey, &c->fcnt, &c->arena,
+          &c->wl_in, &c->wl_text, &c->wl_pos, &c->wl_acc};
 }
 
 // The device memory high-water mark of the current training ("dev_peak_bytes"): sampled after every phase and every fed
@@ -1123,6 +1195,7 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
   ytc::timers_reset(c);
   if ((c->feeding || c->arena.p) && feed_release(c)) return 1;   // an abandoned feed
   c->fed_words = false;
+  c->fed_table = false;
   c->feed_pieces = 0;
   c->dev_peak = 0;
   if (on_device) {
@@ -1162,9 +1235,12 @@ int yttm_train_load_corpus(yttm_ctx *c, const char *bytes, uint64_t n, int on_de
 static int feed_release(yttm_ctx *c) {
   if (c->stream2) YT_CUDA(c, cudaStreamSynchronize(c->stream2));
   YT_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (ytc::DevBuf *b : {&c->feed_dev[0], &c->feed_dev[1], &c->fkey, &c->fcnt, &c->arena}) b->release();
+  for (ytc::DevBuf *b : {&c->feed_dev[0], &c->feed_dev[1], &c->fkey, &c->fcnt, &c->arena, &c->wl_in, &c->wl_text,
+                         &c->wl_pos, &c->wl_acc})
+    b->release();
   c->feeding = false;
   c->fed_words = false;
+  c->fed_table = false;
   c->feed_pending = -1;
   return 0;
 }
@@ -1217,13 +1293,12 @@ static int ftab_reserve(yttm_ctx *c, uint64_t more) {
   return 0;
 }
 
-// Phase 1 and the word split of piece buffer s (m bytes), then its distinct words into the persistent table.
-static int feed_process(yttm_ctx *c, int s, uint64_t m) {
-  const uint8_t *d = c->feed_dev[s].as<uint8_t>();
+// The distinct words of piece d (m bytes) into the persistent table and the arena: insert(wt, counters, max_unique)
+// launches the pass that builds the per-piece table (retried in a larger one on overflow).  Returns 0 / 1; *occ = the
+// piece's word occurrences.
+using PieceInsert = std::function<void(WordTab, unsigned long long *, uint64_t)>;
+static int feed_piece_words(yttm_ctx *c, const uint8_t *d, uint64_t m, const PieceInsert &insert, uint64_t *occ) {
   auto *counters = c->counters.as<unsigned long long>();
-  YT_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_feed_copied[s], 0));
-  char_hist_kernel<<<grid_for(c, m / 16 + 1, 512, 4), 512, 0, c->stream>>>(d, m, c->hist.as<unsigned long long>());
-  c->launches++;
   unsigned long long h[6] = {0, 0, 0, 0, 0, 0};
   for (int attempt = 0;; attempt++) {   // a piece that overflows the per-piece table is split again in a larger one
     if (attempt > 10) YT_FAIL(c, "word table: too many retries");
@@ -1233,8 +1308,7 @@ static int feed_process(yttm_ctx *c, int s, uint64_t m) {
     YT_CUDA(c, cudaMemsetAsync(c->wkey.p, 0, cap * 8, c->stream));
     YT_CUDA(c, cudaMemsetAsync(c->wcnt.p, 0, cap * 8, c->stream));
     YT_CUDA(c, cudaMemsetAsync(counters, 0, 64, c->stream));
-    WordTab wt{c->wkey.as<unsigned long long>(), c->wcnt.as<unsigned long long>(), cap - 1};
-    word_insert_kernel<<<grid_for(c, m, 256, 8), 256, 0, c->stream>>>(d, m, 0, m, wt, counters, cap / 2);
+    insert(WordTab{c->wkey.as<unsigned long long>(), c->wcnt.as<unsigned long long>(), cap - 1}, counters, cap / 2);
     c->launches++;
     YT_CUDA(c, cudaGetLastError());
     YT_CUDA(c, cudaMemcpyAsync(h, counters, 32, cudaMemcpyDeviceToHost, c->stream));
@@ -1243,6 +1317,7 @@ static int feed_process(yttm_ctx *c, int s, uint64_t m) {
     c->feed_wcap *= 4;
   }
   c->n_word_occ += h[0];
+  *occ = h[0];
   const uint64_t U = h[1];
   if (U) {
     YT_CUDA(c, c->wpos.reserve((U + 1) * 8));
@@ -1274,9 +1349,23 @@ static int feed_process(yttm_ctx *c, int s, uint64_t m) {
     }
   }
   YT_CUDA(c, cudaGetLastError());
-  YT_CUDA(c, cudaEventRecord(c->ev_feed_done[s], c->stream));
   c->feed_pieces++;
   note_peak(c);
+  return 0;
+}
+
+// Phase 1 and the word split of piece buffer s (m bytes), then its distinct words into the persistent table.
+static int feed_process(yttm_ctx *c, int s, uint64_t m) {
+  const uint8_t *d = c->feed_dev[s].as<uint8_t>();
+  YT_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_feed_copied[s], 0));
+  char_hist_kernel<<<grid_for(c, m / 16 + 1, 512, 4), 512, 0, c->stream>>>(d, m, c->hist.as<unsigned long long>());
+  c->launches++;
+  uint64_t occ;
+  if (feed_piece_words(c, d, m, [&](WordTab wt, unsigned long long *counters, uint64_t max_unique) {
+        word_insert_kernel<<<grid_for(c, m, 256, 8), 256, 0, c->stream>>>(d, m, 0, m, wt, counters, max_unique);
+      }, &occ))
+    return 1;
+  YT_CUDA(c, cudaEventRecord(c->ev_feed_done[s], c->stream));
   return 0;
 }
 
@@ -1327,6 +1416,8 @@ int yttm_train_feed_begin(yttm_ctx *c) {
   c->feed_cur = 0;
   c->feed_len = c->feed_nows = 0;
   c->arena_len = c->n_fed = c->feed_pieces = c->feed_fn = 0;
+  c->wl_occ = c->wl_seps = 0;
+  c->wl_fed = false;
   // per-piece table: one slot per 32 bytes (a piece's distinct words are far fewer than its words); the persistent
   // table and the arena start small and grow with the unique words
   c->feed_wcap = std::min<uint64_t>(std::max<uint64_t>(ytc::pow2ceil(c->feed_piece / 32), 1u << 10), 1ull << 26);
@@ -1340,6 +1431,8 @@ int yttm_train_feed_begin(yttm_ctx *c) {
   YT_CUDA(c, cudaMemsetAsync(c->fcnt.p, 0, c->feed_fcap * 8, c->stream));
   YT_CUDA(c, c->arena.reserve(1u << 16));
   YT_CUDA(c, cudaMemsetAsync(c->arena.p, ' ', 16, c->stream));
+  YT_CUDA(c, c->wl_acc.reserve(24));
+  YT_CUDA(c, cudaMemsetAsync(c->wl_acc.p, 0, 24, c->stream));
   c->feeding = true;
   note_peak(c);
   return 0;
@@ -1366,12 +1459,128 @@ int yttm_train_feed(yttm_ctx *c, const char *bytes, uint64_t n) {
   return 0;
 }
 
+// entries [i0, i0 + k) of a word list (ho: their k + 1 offsets on the host) -> the persistent table, the arena and the
+// histogram; *occ = their occurrences
+static int feed_words_piece(yttm_ctx *c, const uint8_t *bytes, const uint64_t *offsets, const uint64_t *counts,
+                            const uint64_t *ho, uint64_t i0, uint64_t k, int on_device, uint64_t *occ) {
+  const uint64_t B = ho[k] - ho[0], m = B + k;   // laid out: every entry followed by one space
+  const uint8_t *d_bytes = bytes;
+  const uint64_t *d_off = offsets + i0, *d_cnt = counts + i0;
+  if (!on_device) {   // offsets (from 0), counts and bytes through the staging buffer that is not being filled
+    const int o = c->feed_cur ^ 1;
+    const uint64_t need = (2 * k + 1) * 8 + B;
+    YT_CUDA(c, cudaEventSynchronize(c->ev_feed_copied[o]));
+    if (stage_reserve(c, o, need)) return 1;
+    uint64_t *so = reinterpret_cast<uint64_t *>(c->feed_stage[o]);
+    for (uint64_t j = 0; j <= k; j++) so[j] = ho[j] - ho[0];
+    std::memcpy(so + k + 1, counts + i0, k * 8);
+    std::memcpy(so + 2 * k + 1, bytes + ho[0], B);
+    YT_CUDA(c, c->wl_in.reserve(need));
+    YT_CUDA(c, cudaMemcpyAsync(c->wl_in.p, so, need, cudaMemcpyHostToDevice, c->stream));
+    d_off = c->wl_in.as<uint64_t>();
+    d_cnt = d_off + k + 1;
+    d_bytes = reinterpret_cast<const uint8_t *>(d_cnt + k);
+  }
+  YT_CUDA(c, c->wl_text.reserve(m));
+  YT_CUDA(c, c->wl_pos.reserve(k * 8));
+  auto *acc = c->wl_acc.as<unsigned long long>();
+  YT_CUDA(c, cudaMemsetAsync(acc + 2, 0xff, 8, c->stream));
+  uint8_t *text = c->wl_text.as<uint8_t>();
+  uint64_t *pos = c->wl_pos.as<uint64_t>();
+  word_list_layout_kernel<<<grid_for(c, k, 256, 8), 256, 0, c->stream>>>(d_bytes, d_off, d_cnt, k, i0, text, pos,
+                                                                         c->hist.as<unsigned long long>(), acc);
+  c->launches++;
+  YT_CUDA(c, cudaGetLastError());
+  unsigned long long h[3];
+  YT_CUDA(c, cudaMemcpyAsync(h, acc, 24, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (h[2] != ~0ull) {
+    const uint64_t j = h[2] - i0, len = ho[j + 1] - ho[j];
+    if (!len) YT_FAIL(c, "word list: entry " + std::to_string(h[2]) + " is empty (separators are given apart)");
+    std::string w(std::min<uint64_t>(len, 64), '\0');
+    if (on_device) YT_CUDA(c, cudaMemcpy(&w[0], bytes + ho[j], w.size(), cudaMemcpyDeviceToHost));
+    else std::memcpy(&w[0], bytes + ho[j], w.size());
+    std::string shown;
+    for (unsigned char ch : w) {
+      char e[8];
+      if (ch >= 0x21 && ch < 0x7f && ch != '\\') shown += (char)ch;
+      else { std::snprintf(e, sizeof(e), "\\x%02x", ch); shown += e; }
+    }
+    YT_FAIL(c, "word list: entry " + std::to_string(h[2]) + " (b'" + shown + (len > w.size() ? "...'" : "'") +
+                   ") contains a separator (a whitespace byte or U+2581)");
+  }
+  if (h[1]) YT_FAIL(c, "word list: data_len (count x units summed over the words) would pass 2^64");
+  return feed_piece_words(c, text, m, [&](WordTab wt, unsigned long long *counters, uint64_t max_unique) {
+    word_insert_list_kernel<<<grid_for(c, k, 256, 8), 256, 0, c->stream>>>(text, m, 0, pos, d_cnt, k, wt, counters,
+                                                                           max_unique);
+  }, occ);
+}
+
+static int feed_words(yttm_ctx *c, const uint8_t *bytes, const uint64_t *offsets, const uint64_t *counts, uint64_t n,
+                      uint64_t separators, int on_device) {
+  // a piece holds at most feed_piece laid-out bytes and at least one entry; a window of entries whose offsets the
+  // host reads (a laid-out entry takes 2 bytes or more; 8 bounds the host copy of device offsets)
+  const uint64_t window = c->feed_piece / 8 + 1;
+  std::vector<uint64_t> hoff;
+  uint64_t sum = 0;
+  for (uint64_t i0 = 0; i0 < n;) {
+    const uint64_t win = std::min(n - i0, window);
+    const uint64_t *ho = offsets + i0;
+    if (on_device) {
+      hoff.resize(win + 1);
+      YT_CUDA(c, cudaMemcpy(hoff.data(), offsets + i0, (win + 1) * 8, cudaMemcpyDeviceToHost));
+      ho = hoff.data();
+    }
+    uint64_t k = 0;
+    for (; k < win; k++) {
+      if (ho[k + 1] < ho[k]) YT_FAIL(c, "word list: offsets decrease at entry " + std::to_string(i0 + k));
+      if (k && ho[k + 1] - ho[0] + k + 1 > c->feed_piece) break;
+    }
+    uint64_t occ = 0;
+    if (feed_words_piece(c, bytes, offsets, counts, ho, i0, k, on_device, &occ)) return 1;
+    sum += occ;
+    i0 += k;
+  }
+  const uint64_t seps = separators == UINT64_MAX ? sum : separators;
+  if (c->wl_seps + seps < seps) YT_FAIL(c, "word list: the separators would pass 2^64");
+  c->wl_seps += seps;
+  c->wl_occ += sum;
+  c->wl_fed = true;
+  return 0;
+}
+
+int yttm_train_feed_words(yttm_ctx *c, const uint8_t *bytes, const uint64_t *offsets, const uint64_t *counts,
+                          uint64_t n, uint64_t separators, int on_device) {
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (!c->feeding) YT_FAIL(c, "yttm_train_feed_words: yttm_train_feed_begin has not run");
+  if (!feed_words(c, bytes, offsets, counts, n, separators, on_device)) return 0;
+  const std::string err = c->err;   // a failed list leaves part of it counted: the feed ends here
+  feed_release(c);
+  c->err = err;
+  return 1;
+}
+
 int yttm_train_feed_end(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct) {
   YT_CUDA(c, cudaSetDevice(c->device));
   if (!c->feeding) YT_FAIL(c, "yttm_train_feed_end: yttm_train_feed_begin has not run");
   if (c->feed_len && feed_submit(c, c->feed_len)) return 1;   // the last piece ends with the corpus
   if (c->feed_pending >= 0 && feed_process(c, c->feed_pending, c->feed_pending_len)) return 1;
   c->feed_pending = -1;
+  if (c->wl_fed) {   // data_len = the text's units + the lists' count x units + their separators, never wrapped
+    if (c->wl_seps + 1 < c->wl_occ)
+      YT_FAIL(c, "word list: " + std::to_string(c->wl_seps) + " separators for " + std::to_string(c->wl_occ) +
+                     " word occurrences; a text of these words holds at least " + std::to_string(c->wl_occ - 1));
+    unsigned long long t = 0, units = 0;
+    auto *slot = c->hist.as<unsigned long long>() + CP_LIMIT;
+    YT_CUDA(c, cudaMemcpyAsync(&t, slot, 8, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaMemcpyAsync(&units, c->wl_acc.p, 8, cudaMemcpyDeviceToHost, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+    const uint64_t a = t + units, b = a + c->wl_seps;
+    if (a < t || b < a) YT_FAIL(c, "word list: data_len would pass 2^64");
+    t = b;
+    YT_CUDA(c, cudaMemcpyAsync(slot, &t, 8, cudaMemcpyHostToDevice, c->stream));
+    YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
   // the persistent table -> wpos / wfreq (arena positions); the arena with its pads becomes the text
   const uint64_t U = c->feed_fn;
   auto *counters = c->counters.as<unsigned long long>();
@@ -1395,7 +1604,44 @@ int yttm_train_feed_end(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct) {
   c->n_text = c->arena_len;
   c->n_unique = U;
   c->fed_words = true;
+  c->fed_table = true;
   return hist_summarise(c, data_len, n_distinct);
+}
+
+int yttm_train_fed_words(yttm_ctx *c, uint8_t *bytes, uint64_t bytes_cap, uint64_t *offsets, uint64_t *counts,
+                         uint64_t cap, uint64_t *n_unique, uint64_t *n_bytes, uint64_t *separators) {
+  YT_CUDA(c, cudaSetDevice(c->device));
+  if (!c->fed_table) YT_FAIL(c, "yttm_train_fed_words: no fed words (yttm_train_feed_end has not run, or a build used them)");
+  const uint64_t U = c->n_unique, nb = c->n_text - U;   // the arena: every word followed by one space
+  *n_unique = U;
+  *n_bytes = nb;
+  const bool fits = bytes_cap >= nb && cap >= U && offsets && (counts || !U) && (bytes || !nb);
+  if (!fits && !separators) return 2;
+  std::vector<uint8_t> a(c->n_text);
+  std::vector<uint64_t> pos(U), freq(U);
+  YT_CUDA(c, cudaMemcpyAsync(a.data(), c->d_text, c->n_text, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaMemcpyAsync(pos.data(), c->wpos.p, U * 8, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaMemcpyAsync(freq.data(), c->wfreq.p, U * 8, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  uint64_t at = 0, units = 0;
+  for (uint64_t i = 0; i < U; i++) {
+    const uint8_t *w = a.data() + pos[i];
+    const uint64_t len = static_cast<const uint8_t *>(std::memchr(w, ' ', c->n_text - pos[i])) - w;
+    for (uint64_t q = 0; q < len; units += freq[i]) {
+      uint32_t l;
+      decode_unit(w, q, len, &l);
+      q += l;
+    }
+    if (fits) {
+      offsets[i] = at;
+      counts[i] = freq[i];
+      std::memcpy(bytes + at, w, len);
+    }
+    at += len;
+  }
+  if (fits) offsets[U] = at;
+  if (separators) *separators = c->data_len - units;
+  return fits ? 0 : 2;
 }
 
 static int hist_summarise(yttm_ctx *c, uint64_t *data_len, uint64_t *n_distinct) {
@@ -1496,6 +1742,7 @@ static int finish_build(yttm_ctx *c, yttm_train_stats *stats) {
 struct WordList { const uint64_t *pos, *freq; const uint64_t *word_off, *byte_off; uint32_t n_src; };
 static int build_word_table(yttm_ctx *c, const WordList *list, uint64_t *n_unique) {
   const uint64_t n = c->n_text;
+  c->fed_table = false;
   YT_CUDA(c, c->counters.reserve(64));
   auto *counters = c->counters.as<unsigned long long>();
   ytc::timer_begin(c, list ? "word_import" : "word_count");
@@ -1610,6 +1857,7 @@ int yttm_train_build(yttm_ctx *c, yttm_train_stats *stats) {
   if (c->feeding) YT_FAIL(c, "yttm_train_build: yttm_train_feed_end has not run");
   if (!c->have_alphabet) YT_FAIL(c, "yttm_train_build: alphabet not set");
   uint64_t U = c->n_unique;   // a fed corpus: its words are in wpos / wfreq already
+  c->fed_table = false;
   if (c->fed_words) {
     if (c->pcap) YT_FAIL(c, "yttm_train_build: the fed words were built already (feed the corpus again)");
   } else if (build_word_table(c, nullptr, &U)) {

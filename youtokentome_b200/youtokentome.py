@@ -5,12 +5,14 @@ types).  Additions are additive only: `encode_packed` (zero-marshalling numpy pa
 span of every id), `encode_padded` (the same ids as padded, truncated [N, L] rows with their lengths),
 `encode_subwords_packed` (the subword pieces on the GPU), `encode_file` (a file of any size, line by line, to .npy files
 or the CLI's text), `decode_packed` (the inverse of `encode_packed`, on the GPU), `decode_file` (the inverse of
-`encode_file`: either of its outputs, of any size, back to text on the GPU) and `dropout_seed`."""
+`encode_file`: either of its outputs, of any size, back to text on the GPU), `count_words` / `train_from_counts` (a
+corpus's word-count table, and training from such a table) and `dropout_seed`."""
 import ctypes as C
 import os
 import sys
 import threading
-from collections.abc import Collection
+from collections import namedtuple
+from collections.abc import Collection, Mapping, Sequence
 from enum import Enum
 from typing import List, Optional, Union
 
@@ -128,6 +130,122 @@ def _host_buffers(out, pinned, *specs):
     return bufs, [b.ctypes.data for b in bufs]
 
 
+WordCounts = namedtuple("WordCounts", ["word_bytes", "word_offsets", "counts", "separators", "data_len"])
+WordCounts.__doc__ = """A corpus's word-count table: word i is word_bytes[word_offsets[i]:word_offsets[i+1]] (uint8, uint64 offsets
+from 0) occurring counts[i] times (uint64); `separators` separator units (space, \\t .. \\r, U+2581) and `data_len` decode
+units in the text.  Training on it gives the model of training on the text."""
+
+
+def _open_input(data, what):
+    """(fd, fd to close or None, bytes or None) for a path, a file descriptor, an object with fileno() or bytes-like."""
+    if isinstance(data, (str, os.PathLike)):
+        try:
+            fd = os.open(data, os.O_RDONLY | getattr(os, "O_CLOEXEC", 0))
+        except OSError as e:
+            raise ValueError("%s: cannot open '%s': %s" % (what, os.fsdecode(data), e.strerror)) from None
+        return fd, fd, None
+    if isinstance(data, int) and not isinstance(data, bool):
+        return data, None, None
+    if hasattr(data, "fileno"):
+        return data.fileno(), None, None
+    if isinstance(data, (bytes, bytearray, memoryview)):
+        return -1, None, bytes(data)
+    raise TypeError("data must be a path, a file descriptor, an object with fileno() or bytes-like, not %s" %
+                    type(data).__name__)
+
+
+def _int_array(x, name):
+    """An integer numpy array or torch tensor -> (uint64 numpy array or int64 CUDA tensor, on_device); negative values
+    raise ValueError."""
+    if _is_torch(x):
+        if x.dtype.is_floating_point or x.dtype.is_complex or x.dtype == __import__("torch").bool:
+            raise TypeError("%s must hold integers, not %s" % (name, x.dtype))
+        if x.numel() and bool((x < 0).any()):
+            raise ValueError("%s must not be negative" % name)
+        if x.is_cuda:
+            import torch
+            return x.to(torch.int64).contiguous(), True
+        x = x.numpy()
+    x = np.asarray(x)
+    if x.dtype.kind not in "iu" and not (x.size == 0 and x.dtype.kind == "f"):
+        raise TypeError("%s must hold integers, not %s" % (name, x.dtype))
+    if x.dtype.kind == "i" and x.size and x.min() < 0:
+        raise ValueError("%s must not be negative" % name)
+    return np.ascontiguousarray(x.astype(np.uint64)).reshape(-1), False
+
+
+def _pack_words(words):
+    enc = []
+    for w in words:
+        if isinstance(w, str):
+            enc.append(w.encode())
+        elif isinstance(w, (bytes, bytearray, memoryview)):
+            enc.append(bytes(w))
+        else:
+            raise TypeError("a word must be str or bytes, not %s" % type(w).__name__)
+    offs = np.zeros(len(enc) + 1, dtype=np.uint64)
+    if enc:
+        np.cumsum([len(b) for b in enc], out=offs[1:])
+    return np.frombuffer(b"".join(enc), dtype=np.uint8), offs
+
+
+def _table_arrays(counts):
+    """train_from_counts' `counts` other than a TSV path -> (bytes, offsets, counts, separators or None, on_device)."""
+    if isinstance(counts, WordCounts):
+        if counts.separators is not None and (not isinstance(counts.separators, (int, np.integer)) or
+                                              isinstance(counts.separators, bool)):
+            raise TypeError("separators must be an int or None, not %s" % type(counts.separators).__name__)
+        b, offs, cnt = counts.word_bytes, counts.word_offsets, counts.counts
+        seps = None if counts.separators is None else int(counts.separators)
+        if all(_is_torch(t) and t.is_cuda for t in (b, offs, cnt)):
+            import torch
+            if b.dtype != torch.uint8:
+                raise TypeError("word_bytes must be uint8, not %s" % b.dtype)
+            offs, _ = _int_array(offs, "word_offsets")
+            cnt, _ = _int_array(cnt, "counts")
+            return b.contiguous(), offs, cnt, seps, True
+        if _is_torch(b):
+            b = b.cpu().numpy()
+        b = np.ascontiguousarray(np.asarray(b))
+        if b.dtype != np.uint8:
+            raise TypeError("word_bytes must be uint8, not %s" % b.dtype)
+        offs, _ = _int_array(offs.cpu() if _is_torch(offs) else offs, "word_offsets")
+        cnt, _ = _int_array(cnt.cpu() if _is_torch(cnt) else cnt, "counts")
+    elif isinstance(counts, Mapping):
+        seps, words, vals = None, [], []
+        for w, c in counts.items():
+            if not isinstance(c, (int, np.integer)) or isinstance(c, bool):
+                raise TypeError("a count must be an int, not %s" % type(c).__name__)
+            if c < 0:
+                raise ValueError("the count of %r is negative" % (w,))
+            if w in ("", b""):
+                seps = (seps or 0) + int(c)
+                continue
+            words.append(w)
+            vals.append(int(c))
+        if any(v >= 2 ** 64 for v in vals) or (seps or 0) >= 2 ** 64:
+            raise ValueError("a count does not fit in 64 bits")
+        b, offs = _pack_words(words)
+        cnt = np.array(vals, dtype=np.uint64)
+    elif isinstance(counts, (tuple, list)) and len(counts) == 2 and not isinstance(counts[0], (str, bytes)):
+        words, c = counts
+        if not isinstance(words, Sequence) or isinstance(words, (str, bytes)):
+            raise TypeError("words must be a sequence of str or bytes, not %s" % type(words).__name__)
+        if not (_is_torch(c) or isinstance(c, np.ndarray)):
+            raise TypeError("counts must be a numpy array or a torch tensor, not %s" % type(c).__name__)
+        b, offs = _pack_words(words)
+        cnt, _ = _int_array(c.cpu() if _is_torch(c) else c, "counts")
+        seps = None
+    else:
+        raise TypeError("counts must be a TSV path, a WordCounts, a dict or a pair (words, counts), not %s" %
+                        type(counts).__name__)
+    if len(offs) != len(cnt) + 1:
+        raise ValueError("word_offsets must hold one value more than counts (%d and %d)" % (len(offs), len(cnt)))
+    if len(offs) and int(offs[-1]) > len(b):
+        raise ValueError("word_offsets pass the end of word_bytes")
+    return b, offs, cnt, seps, False
+
+
 class BPE:
     def __init__(self, model: str, n_threads: int = -1):
         self.model = model
@@ -159,6 +277,56 @@ class BPE:
         L = _lib.lib()
         rc = L.yttm_api_train(data.encode(), model.encode(), vocab_size, coverage, n_threads, pad_id, unk_id, bos_id,
                               eos_id)
+        if rc != 0:
+            raise ValueError(L.yttm_api_last_error(None).decode())
+        return BPE(model=model, n_threads=n_threads)
+
+    @staticmethod
+    def count_words(data, output=None) -> WordCounts:
+        """The word-count table of a corpus, counted on the GPU as BPE.train feeds it: `data` is a path, a file
+        descriptor, an object with fileno() (a pipe works) or bytes-like.  Entries are sorted by count descending, then
+        by bytes ascending.  With `output` (a path, "-" for stdout) the table is also written as TSV: the line
+        "\\t<separators>", then one "word\\tcount" line per entry."""
+        fd, opened, buf = _open_input(data, "count_words")
+        sizes = np.zeros(4, dtype=np.uint64)
+        L = _lib.lib()
+        out = None if output is None else os.fsencode(output)
+        try:
+            if output is not None and os.fspath(output) == "-":
+                sys.stdout.flush()
+            rc = L.yttm_api_count_words(fd, buf, len(buf) if buf is not None else 0, out, sizes.ctypes.data)
+        finally:
+            if opened is not None:
+                os.close(opened)
+        if rc != 0:
+            raise ValueError(L.yttm_api_last_error(None).decode())
+        n, nb = int(sizes[0]), int(sizes[1])
+        words = np.empty(nb, dtype=np.uint8)
+        offs = np.empty(n + 1, dtype=np.uint64)
+        cnt = np.empty(n, dtype=np.uint64)
+        L.yttm_api_result_words(words.ctypes.data, offs.ctypes.data, cnt.ctypes.data)
+        return WordCounts(words, offs, cnt, int(sizes[2]), int(sizes[3]))
+
+    @staticmethod
+    def train_from_counts(counts, model: str, vocab_size: int, coverage: float = 1.0, n_threads: int = -1,
+                          pad_id: int = 0, unk_id: int = 1, bos_id: int = 2, eos_id: int = 3) -> "BPE":
+        """Trains from a word-count table and writes the model BPE.train writes for any text with the same words,
+        counts and separators (the same errors too).  `counts`: a TSV path as count_words writes it, a WordCounts
+        (whose arrays may be CUDA tensors, read in place), a dict {word: count} whose key "" holds the separators, or a
+        pair (words, counts) of str / bytes words and a numpy array or torch tensor.  Without separators there is one
+        per occurrence."""
+        L = _lib.lib()
+        if isinstance(counts, (str, os.PathLike)):
+            rc = L.yttm_api_train_counts(None, None, None, 0, 2 ** 64 - 1, 0, os.fsencode(counts), model.encode(),
+                                         vocab_size, coverage, n_threads, pad_id, unk_id, bos_id, eos_id)
+        else:
+            b, offs, cnt, seps, on_device = _table_arrays(counts)
+            if seps is not None and seps >= 2 ** 64 - 1:
+                raise ValueError("separators must be below 2^64 - 1")
+            ptr = (lambda t: t.data_ptr()) if on_device else (lambda a: a.ctypes.data)
+            rc = L.yttm_api_train_counts(ptr(b), ptr(offs), ptr(cnt), len(cnt), 2 ** 64 - 1 if seps is None else seps,
+                                         int(on_device), None, model.encode(), vocab_size, coverage, n_threads, pad_id,
+                                         unk_id, bos_id, eos_id)
         if rc != 0:
             raise ValueError(L.yttm_api_last_error(None).decode())
         return BPE(model=model, n_threads=n_threads)

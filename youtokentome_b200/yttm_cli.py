@@ -1,4 +1,4 @@
-"""`yttm bpe | encode | encode_file | decode | decode_file | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
+"""`yttm bpe | bpe_counts | count_words | encode | encode_file | decode | decode_file | vocab` — the reference's command line (youtokentome/yttm_cli.py:1-169:
 same sub-commands, option names, defaults and stdin/stdout framing) over the CUDA library.
 Run as `python -m youtokentome_b200.yttm_cli ...`.  `--n_threads` is accepted and ignored."""
 import sys
@@ -28,6 +28,34 @@ def bpe(data, model, vocab_size, coverage, n_threads, pad_id, unk_id, bos_id, eo
     """Train BPE model."""
     BPE.train(data=data, model=model, vocab_size=vocab_size, coverage=coverage, n_threads=n_threads, pad_id=pad_id,
               unk_id=unk_id, bos_id=bos_id, eos_id=eos_id)
+
+
+@main.command("count_words")
+@click.option("--data", type=click.STRING, required=True, help="Text file to count, '-' for stdin.")
+@click.option("--output", type=click.STRING, required=True, help="TSV file to write, '-' for stdout.")
+def count_words(data, output):
+    """Count the words of a corpus on the GPU into a TSV word-count table."""
+    src = sys.stdin.buffer if data == "-" else data
+    t = BPE.count_words(src, output=output)
+    click.echo("count_words: %d unique words, %d occurrences, %d separators, data_len %d" %
+               (len(t.counts), int(t.counts.sum(dtype="uint64")), t.separators, t.data_len), err=True)
+
+
+@main.command("bpe_counts")
+@click.option("--data", type=click.Path(exists=True), required=True, help="TSV word-count table (count_words).")
+@click.option("--model", type=click.Path(), required=True, help="Output model file path.")
+@click.option("--vocab_size", type=click.INT, required=True, help="Number of tokens in the final vocabulary.")
+@click.option("--coverage", type=click.FLOAT, default=1.0, show_default=True,
+              help="Percentage of characters covered by the model.")
+@click.option("--n_threads", type=click.INT, default=-1, show_default=True, help="Number of threads (ignored).")
+@click.option("--pad_id", type=click.INT, default=0, show_default=True, help="Padding token id.")
+@click.option("--unk_id", type=click.INT, default=1, show_default=True, help="Unknown token id.")
+@click.option("--bos_id", type=click.INT, default=2, show_default=True, help="Begin of sentence token id.")
+@click.option("--eos_id", type=click.INT, default=3, show_default=True, help="End of sentence token id.")
+def bpe_counts(data, model, vocab_size, coverage, n_threads, pad_id, unk_id, bos_id, eos_id):
+    """Train BPE model from a word-count table."""
+    BPE.train_from_counts(data, model=model, vocab_size=vocab_size, coverage=coverage, n_threads=n_threads,
+                          pad_id=pad_id, unk_id=unk_id, bos_id=bos_id, eos_id=eos_id)
 
 
 @main.command()
