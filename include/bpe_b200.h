@@ -269,6 +269,11 @@ class BaseEncoder {
   // renamed on success, so a failed call leaves nothing at the output names.  *n_bytes = input bytes.
   Status encode_file(int in_fd, const std::string &out_path, bool text, bool bos, bool eos, bool reverse,
                      double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const;
+  // encode_file's lines, pieces and outputs as `yttm encode --output_type subword` prints them: every piece of the line
+  // (as encode_subwords_packed gives it) followed by one space, then "\n", to out_path ("-" = stdout).  Any vocabulary
+  // size.  *n_ids = pieces (one per id).
+  Status encode_file_subwords(int in_fd, const std::string &out_path, bool bos, bool eos, bool reverse,
+                              double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const;
 
   // Decodes ids of any size on the GPU, line by line, to the text of `yttm decode` (every line's decode and '\n') at
   // out_path ("-" = stdout).  text: in_fd is id text, read to its end and split as encode_file splits it, and a line's
@@ -288,6 +293,9 @@ class BaseEncoder {
 
  private:
   Status init_device();
+  // the body of encode_file and encode_file_subwords: format is the encode stream's (YTTM_STREAM_* of yttm_b200.h)
+  Status encode_file_as(int in_fd, const std::string &out_path, int format, bool bos, bool eos, bool reverse,
+                        double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const;
   Status resolve_pad(int64_t pad_id, int32_t *out) const;  // encode_padded_*: kModelPad -> the model's pad id
   // The frame of every encode_*_into / _device and decode_packed_* call: the <BOS> / <EOS> check, `checked` (an argument
   // error the caller found), the device status, then call() (a yttm_enc_run* / yttm_dec_run* call): its return code 2 is

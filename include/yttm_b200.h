@@ -284,16 +284,19 @@ int yttm_enc_run_subwords_device(yttm_enc *enc, const char *d_bytes, const uint6
  * handed to the sink, so device memory is bounded by two pieces and the longest line.
  * Formats of the sink's data: YTTM_STREAM_IDS16 (uint16 ids; the vocabulary must not exceed 65536), YTTM_STREAM_IDS32
  * (int32 ids), YTTM_STREAM_TEXT (`yttm encode --output_type id`'s text: every id in decimal followed by one space, then
- * '\n' per line).  While a stream is open every other encode and decode call on the encoder fails; any failure closes
- * the stream (the next begin works) and yttm_enc_destroy frees an open one.  yttm_stage_ms(ctx, "stream_pieces") /
+ * '\n' per line), YTTM_STREAM_SUBWORD (`yttm encode --output_type subword`'s text: every piece yttm_enc_run_subwords
+ * gives the line followed by one space, then '\n' per line; any vocabulary size).  While a stream is open every other
+ * encode and decode call on the encoder fails; any failure closes the stream (the next begin works) and
+ * yttm_enc_destroy frees an open one.  yttm_stage_ms(ctx, "stream_pieces") /
  * ("stream_dev_peak_bytes"): pieces of the last stream and the largest sum of the encoder's device buffers, sampled
  * after every piece. */
 #define YTTM_STREAM_IDS16 0
 #define YTTM_STREAM_IDS32 1
 #define YTTM_STREAM_TEXT 2
+#define YTTM_STREAM_SUBWORD 3 /* encode streams only */
 /* Called on the calling thread of feed / end, in line order, with library-owned host memory valid until it returns.
  * data: the ids (2 or 4 bytes each) or the text bytes of the lines that completed; line_ends[k]: the global id count
- * at the end of the k-th of those lines (the same in every format).  Non-zero fails the stream. */
+ * at the end of the k-th of those lines (the same in every format; one piece per id).  Non-zero fails the stream. */
 typedef int (*yttm_enc_sink)(void *user, const void *data, uint64_t n_bytes, const uint64_t *line_ends, uint64_t n_lines);
 int yttm_enc_stream_begin(yttm_enc *enc, int bos, int eos, int reverse, double dropout, uint64_t seed,
                           uint64_t first_sentence_index, int format, yttm_enc_sink sink, void *user);

@@ -129,6 +129,11 @@ int yttm_api_decode_cli(void *handle, const int32_t *ignore, uint64_t n_ignore);
  * stats[3] = lines, ids, input bytes.  0 ok, 1 error. */
 int yttm_api_encode_file(void *handle, int in_fd, const char *out_path, int text, int bos, int eos, int reverse,
                          double dropout, uint64_t *stats);
+/* BaseEncoder::encode_file_subwords: the lines of in_fd to out_path ("-" = stdout) as `yttm encode --output_type
+ * subword` writes them; uses the handle's dropout seed and counter.  stats[3] = lines, pieces, input bytes.  0 ok,
+ * 1 error. */
+int yttm_api_encode_file_subwords(void *handle, int in_fd, const char *out_path, int bos, int eos, int reverse,
+                                  double dropout, uint64_t *stats);
 /* BaseEncoder::decode_file: with text != 0 the id text of in_fd, else the pair <in_prefix>.ids.npy +
  * <in_prefix>.offsets.npy, decoded to out_path ("-" = stdout) as `yttm decode` prints it; ignore[n_ignore] as for
  * decode.  stats[3] = lines, ids, text bytes written.  0 ok, 1 error. */

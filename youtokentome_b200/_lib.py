@@ -35,7 +35,7 @@ def lib():
 # yttm_enc_sink of include/yttm_b200.h (the sink of both streams): (user, data, n_bytes, line_ends, n_lines) -> 0 or a
 # failure
 ENC_SINK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_uint64)
-STREAM_IDS16, STREAM_IDS32, STREAM_TEXT = 0, 1, 2
+STREAM_IDS16, STREAM_IDS32, STREAM_TEXT, STREAM_SUBWORD = 0, 1, 2, 3
 
 
 def bind(L):
@@ -83,6 +83,7 @@ def bind(L):
         "yttm_api_encode_cli": (i32, [vp, cp, i32, i32, i32, i32, dbl]),
         "yttm_api_decode_cli": (i32, [vp, vp, u64]),
         "yttm_api_encode_file": (i32, [vp, i32, cp, i32, i32, i32, i32, dbl, vp]),
+        "yttm_api_encode_file_subwords": (i32, [vp, i32, cp, i32, i32, i32, dbl, vp]),
         "yttm_api_decode_file": (i32, [vp, i32, cp, cp, i32, vp, u64, vp]),
         "yttm_api_vocab_cli": (None, [vp, i32]),
         "yttm_api_dump_order": (i32, [vp, u64, vp]),

@@ -1129,7 +1129,7 @@ Status BaseEncoder::decode_cli(const std::unordered_set<int> *ignore_ids) const 
 
 // ---------------------------------------------------------------------------------------------
 // encode_file: a file or pipe through the device's encode stream (yttm_enc_stream_* of yttm_b200.h) into .npy files or
-// the text of `yttm encode --output_type id`
+// the text of `yttm encode --output_type id` or `--output_type subword`
 // ---------------------------------------------------------------------------------------------
 namespace {
 
@@ -1212,11 +1212,23 @@ int file_sink(void *user, const void *data, uint64_t n_bytes, const uint64_t *li
 
 Status BaseEncoder::encode_file(int in_fd, const std::string &out_path, bool text, bool bos, bool eos, bool reverse,
                                 double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const {
+  const int format = text ? YTTM_STREAM_TEXT : vocab_size() <= 65536 ? YTTM_STREAM_IDS16 : YTTM_STREAM_IDS32;
+  return encode_file_as(in_fd, out_path, format, bos, eos, reverse, dropout_prob, n_lines, n_ids, n_bytes);
+}
+
+Status BaseEncoder::encode_file_subwords(int in_fd, const std::string &out_path, bool bos, bool eos, bool reverse,
+                                         double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const {
+  return encode_file_as(in_fd, out_path, YTTM_STREAM_SUBWORD, bos, eos, reverse, dropout_prob, n_lines, n_ids, n_bytes);
+}
+
+Status BaseEncoder::encode_file_as(int in_fd, const std::string &out_path, int format, bool bos, bool eos, bool reverse,
+                                   double dropout_prob, uint64_t *n_lines, uint64_t *n_ids, uint64_t *n_bytes) const {
   *n_lines = *n_ids = *n_bytes = 0;
   Status st = run_device("encode_file", bos, eos, 0, 0, [] { return 0; });  // the <BOS> / <EOS> and device checks
   if (!st.ok()) return st;
+  const bool text = format == YTTM_STREAM_TEXT || format == YTTM_STREAM_SUBWORD;
   if (!text && out_path == "-") return Status(1, "encode_file: the .npy form needs an output prefix, not '-'");
-  const bool narrow = vocab_size() <= 65536;
+  const bool narrow = format == YTTM_STREAM_IDS16;
   OutFile ids_file, offsets_file;
   FileSink fs;
   fs.text = text;
@@ -1231,7 +1243,6 @@ Status BaseEncoder::encode_file(int in_fd, const std::string &out_path, bool tex
              !(st = offsets_file.write(npy_header("<u8", 0).data(), 128)).ok() || !(st = offsets_file.write(&zero, 8)).ok()) {
     return st;
   }
-  const int format = text ? YTTM_STREAM_TEXT : narrow ? YTTM_STREAM_IDS16 : YTTM_STREAM_IDS32;
   if (yttm_enc_stream_begin(enc_, bos, eos, reverse, dropout_prob, dropout_seed_, sentence_counter_, format, file_sink, &fs))
     return Status(1, ctx_err(ctx_));
   auto failed = [&]() { return fs.st.ok() ? Status(1, ctx_err(ctx_)) : fs.st; };

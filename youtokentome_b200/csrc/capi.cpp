@@ -340,6 +340,13 @@ int yttm_api_encode_file(void *hv, int in_fd, const char *out_path, int text, in
   return ret(h, h->enc->encode_file(in_fd, out_path, text != 0, bos != 0, eos != 0, reverse != 0, dropout, stats,
                                     stats + 1, stats + 2));
 }
+int yttm_api_encode_file_subwords(void *hv, int in_fd, const char *out_path, int bos, int eos, int reverse,
+                                  double dropout, uint64_t *stats) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  return ret(h, h->enc->encode_file_subwords(in_fd, out_path, bos != 0, eos != 0, reverse != 0, dropout, stats,
+                                             stats + 1, stats + 2));
+}
 int yttm_api_decode_file(void *hv, int in_fd, const char *in_prefix, const char *out_path, int text,
                          const int32_t *ignore, uint64_t n_ignore, uint64_t *stats) {
   auto *h = static_cast<Handle *>(hv);

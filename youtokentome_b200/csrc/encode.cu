@@ -28,7 +28,7 @@
 //   emit_ids_kernel<true>       ... and the spans at the occurrences' positions
 //   sub_count_kernel / scan / sub_emit_kernel   one thread per id: piece lengths, offsets, piece bytes
 // An encode stream (yttm_enc_stream_*, the section at the end of this file) finds the lines of each fed piece on the
-// device, runs this flow on them and narrows the ids to uint16 or formats them as text.
+// device, runs this flow on them and narrows the ids to uint16, formats them as text or lays out their pieces as text.
 // The ids of a word are kept in its private slots of a scratch buffer (a word of k bytes owns k+1 slots), at a
 // position that is a pure function of its byte position, so no kernel depends on another block's progress.
 #include <algorithm>
@@ -1809,6 +1809,8 @@ int yttm_enc_run_subwords(yttm_enc *e, const char *bytes, const uint64_t *offset
 //   text_count_kernel   YTTM_STREAM_TEXT, warp per line: its bytes, "<id> " per id and the '\n'
 //   scan                line byte offsets + the piece's text bytes (one 8-byte read-back: the size of the copy out)
 //   text_emit_kernel    warp per line, 32 ids per round: a warp scan places each id's decimal digits
+//   subword_text_kernel YTTM_STREAM_SUBWORD: enc_device's pieces (ENC_SUBWORDS), each followed by ' ', '\n' per line;
+//                       the text size n_piece_bytes + n_ids + n_lines is known without a read-back
 //   add_base_kernel     line ends as global id counts
 // Piece i lives in slot i & 1: its copy in overlaps the kernels of piece i - 1 and the copy out and sink call of piece
 // i - 2.  The sink runs on the caller's thread, in line order, from pinned host buffers of the stream.
@@ -1940,6 +1942,43 @@ __global__ void __launch_bounds__(256) text_emit_kernel(const int32_t *__restric
       pos += __shfl_sync(0xffffffffu, incl, 31);
     }
     if (lane == 0) out[pos] = '\n';
+  }
+}
+
+constexpr uint64_t SUB_SHORT = 32;  // subword_text_kernel: longer pieces are copied by the whole warp
+
+// YTTM_STREAM_SUBWORD, warp per line, 32 ids per round: the pieces of line s (ids [off[s], off[s+1]) of enc_device's
+// sub_off / sub_out), each followed by ' ', then '\n'.  Piece j of line s starts at sub_off[j] + j + s.  A lane copies
+// a piece of at most SUB_SHORT bytes alone; a longer one (a model trained on text without spaces has pieces of
+// thousands of bytes) is copied by all 32 lanes, a byte each per step, so it does not hold 31 lanes idle.
+__global__ void __launch_bounds__(256) subword_text_kernel(const unsigned long long *__restrict__ off, uint64_t n_lines,
+                                                           const unsigned long long *__restrict__ sub_off,
+                                                           const uint8_t *__restrict__ pieces,
+                                                           uint8_t *__restrict__ out) {
+  const unsigned lane = threadIdx.x & 31;
+  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t s = warp; s < n_lines; s += nwarps) {
+    const uint64_t hi = off[s + 1];
+    for (uint64_t j0 = off[s]; j0 < hi; j0 += 32) {  // warp-uniform
+      const uint64_t j = j0 + lane;
+      uint64_t b = 0, n = 0;
+      if (j < hi) {
+        b = sub_off[j];
+        n = sub_off[j + 1] - b;
+        uint8_t *dst = out + b + j + s;
+        if (n <= SUB_SHORT)
+          for (uint64_t k = 0; k < n; k++) dst[k] = pieces[b + k];
+        dst[n] = ' ';
+      }
+      for (unsigned m = __ballot_sync(0xffffffffu, n > SUB_SHORT); m; m &= m - 1) {
+        const int src = __ffs((int)m) - 1;
+        const uint64_t wb = __shfl_sync(0xffffffffu, b, src), wn = __shfl_sync(0xffffffffu, n, src);
+        uint8_t *dst = out + wb + j0 + (uint64_t)src + s;
+        for (uint64_t k = lane; k < wn; k += 32) dst[k] = pieces[wb + k];
+      }
+    }
+    if (lane == 0) out[sub_off[hi] + hi + s] = '\n';
   }
 }
 
@@ -2186,9 +2225,9 @@ int stream_encode(void *owner, int s, const void **out_data, const unsigned long
   const uint8_t *d = sl.d_bytes.as<uint8_t>();
   const uint64_t n = P.n_bytes;
   if (yttm_line_split(c, d, n, P.open_end, &S->tiles[s], &sl.d_offs, &P.n_lines)) return 1;
-  uint64_t n_ids = 0;
+  uint64_t n_ids = 0, n_piece_bytes = 0;
   if (enc_device(e, &sl, d, sl.d_offs.as<uint64_t>(), n, P.n_lines, S->bos, S->eos, S->reverse, S->dropout, S->seed,
-                 S->first + S->lines, &n_ids))
+                 S->first + S->lines, &n_ids, S->format == YTTM_STREAM_SUBWORD ? ENC_SUBWORDS : ENC_IDS, &n_piece_bytes))
     return 1;
   const int32_t *ids = sl.out_ids.as<int32_t>();
   unsigned long long *id_off = sl.out_off.as<unsigned long long>();
@@ -2213,6 +2252,14 @@ int stream_encode(void *owner, int s, const void **out_data, const unsigned long
     YT_CUDA(c, cudaStreamSynchronize(c->stream));
     YT_CUDA(c, S->fmt[s].reserve(text_bytes + 16));
     text_emit_kernel<<<warp_blocks(c, P.n_lines), 256, 0, c->stream>>>(ids, id_off, P.n_lines, ls, S->fmt[s].as<uint8_t>());
+    c->launches++;
+    data = S->fmt[s].p;
+    P.n_out = text_bytes;
+  } else if (S->format == YTTM_STREAM_SUBWORD) {
+    const uint64_t text_bytes = n_piece_bytes + n_ids + P.n_lines;
+    YT_CUDA(c, S->fmt[s].reserve(text_bytes + 16));
+    subword_text_kernel<<<warp_blocks(c, P.n_lines), 256, 0, c->stream>>>(
+        id_off, P.n_lines, sl.sub_off.as<unsigned long long>(), sl.sub_out.as<uint8_t>(), S->fmt[s].as<uint8_t>());
     c->launches++;
     data = S->fmt[s].p;
     P.n_out = text_bytes;
@@ -2245,8 +2292,10 @@ int yttm_enc_stream_begin(yttm_enc *e, int bos, int eos, int reverse, double dro
                           uint64_t first_sentence_index, int format, yttm_enc_sink sink, void *user) {
   if (yttm_enc_check(e, "yttm_enc_stream_begin", bos, eos)) return 1;
   yttm_ctx *c = e->ctx;
-  if (format != YTTM_STREAM_IDS16 && format != YTTM_STREAM_IDS32 && format != YTTM_STREAM_TEXT)
-    YT_FAIL(c, "yttm_enc_stream_begin: format must be YTTM_STREAM_IDS16, YTTM_STREAM_IDS32 or YTTM_STREAM_TEXT");
+  if (format != YTTM_STREAM_IDS16 && format != YTTM_STREAM_IDS32 && format != YTTM_STREAM_TEXT &&
+      format != YTTM_STREAM_SUBWORD)
+    YT_FAIL(c, "yttm_enc_stream_begin: format must be YTTM_STREAM_IDS16, YTTM_STREAM_IDS32, YTTM_STREAM_TEXT or "
+               "YTTM_STREAM_SUBWORD");
   if (!sink) YT_FAIL(c, "yttm_enc_stream_begin: no sink");
   if (format == YTTM_STREAM_IDS16 && e->vocab > 65536)
     YT_FAIL(c, "yttm_enc_stream_begin: 16-bit ids need a vocabulary of at most 65536 (this model has " +

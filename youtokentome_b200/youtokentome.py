@@ -4,7 +4,7 @@ meaning, return types and exceptions (ValueError(status.message), TypeError for 
 types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path, optionally with the source byte
 span of every id), `encode_padded` (the same ids as padded, truncated [N, L] rows with their lengths),
 `encode_subwords_packed` (the subword pieces on the GPU), `encode_file` (a file of any size, line by line, to .npy files
-or the CLI's text), `decode_packed` (the inverse of `encode_packed`, on the GPU), `decode_file` (the inverse of
+or the CLI's id or subword text), `decode_packed` (the inverse of `encode_packed`, on the GPU), `decode_file` (the inverse of
 `encode_file`: either of its outputs, of any size, back to text on the GPU), `count_words` / `train_from_counts` (a
 corpus's word-count table, and training from such a table) and `dropout_seed`."""
 import ctypes as C
@@ -642,18 +642,27 @@ class BPE:
             return np.ascontiguousarray(np.where(big, -1, ids).astype(np.int32)), [-1]
         return torch.where(big, torch.full_like(ids, -1), ids).to(torch.int32).contiguous(), [-1]
 
-    def encode_file(self, input, output, bos=False, eos=False, reverse=False, dropout_prob=0.0, text=False) -> dict:
+    def encode_file(self, input, output, bos=False, eos=False, reverse=False, dropout_prob=0.0, text=False,
+                    output_type: OutputType = OutputType.ID) -> dict:
         """Encodes a text file of any size on the GPU, line by line: a line ends at "\\n" and nowhere else, the text
         after the last "\\n" (if any) is a last line, and line i gets the ids encode_packed gives it without its
         "\\n".  Lines are the next sentences of the dropout stream, as for encode_packed.  `input`: a path, an int file
-        descriptor or an object with fileno() (sys.stdin.buffer, a pipe), read to its end.  Writes
+        descriptor or an object with fileno() (sys.stdin.buffer, a pipe), read to its end.  With output_type
+        OutputType.ID, writes
           text=False  <output>.ids.npy (1-D uint16 when vocab_size() <= 65536, else int32) and <output>.offsets.npy
                       (uint64, lines + 1 values from 0: line i = ids[offsets[i]:offsets[i+1]]), both loadable with
                       np.load(..., mmap_mode="r");
           text=True   the text of `yttm encode --output_type id` (every id and one space, "\\n" per line) to
                       <output>, or to stdout when output is "-".
-        A failed call leaves nothing at the output names.  Returns {"lines", "ids", "bytes"} (bytes read)."""
+        OutputType.SUBWORD always writes text, whatever `text` says (it only chooses between the two id forms): the
+        text of `yttm encode --output_type subword` (every piece encode_subwords_packed gives the line and one space,
+        "\\n" per line) to <output>, or to stdout when output is "-".
+        A failed call leaves nothing at the output names.  Returns {"lines", "ids", "bytes"} (bytes read; "ids" counts
+        the pieces of the subword form, one per id)."""
+        if not isinstance(output_type, OutputType):
+            raise TypeError("parameter output_type must be youtokentome.OutputType, not %s}" % str(type(output_type)))
         _check_dropout(dropout_prob)
+        subword = output_type == OutputType.SUBWORD
         output = os.fspath(output)
         opened = None
         if isinstance(input, (str, bytes, os.PathLike)):
@@ -670,10 +679,14 @@ class BPE:
                             type(input).__name__)
         stats = np.zeros(3, dtype=np.uint64)
         try:
-            if text and output == "-":
+            if (text or subword) and output == "-":
                 sys.stdout.flush()
-            rc = _lib.lib().yttm_api_encode_file(self._h, fd, os.fsencode(output), int(text), int(bos), int(eos),
-                                                 int(reverse), float(dropout_prob), stats.ctypes.data)
+            if subword:
+                rc = _lib.lib().yttm_api_encode_file_subwords(self._h, fd, os.fsencode(output), int(bos), int(eos),
+                                                              int(reverse), float(dropout_prob), stats.ctypes.data)
+            else:
+                rc = _lib.lib().yttm_api_encode_file(self._h, fd, os.fsencode(output), int(text), int(bos), int(eos),
+                                                     int(reverse), float(dropout_prob), stats.ctypes.data)
         finally:
             if opened is not None:
                 os.close(opened)

@@ -5,7 +5,7 @@ import sys
 
 import click
 
-from .youtokentome import BPE
+from .youtokentome import BPE, OutputType
 
 
 @click.group()
@@ -79,17 +79,22 @@ def encode(model, output_type, n_threads, bos, eos, reverse, stream, dropout_pro
 @click.option("--model", type=click.Path(exists=True), required=True, help="Path to file with learned model.")
 @click.option("--input", "input_", type=click.STRING, required=True, help="Text file to encode, '-' for stdin.")
 @click.option("--output", type=click.STRING, required=True,
-              help="Prefix of <output>.ids.npy and <output>.offsets.npy; with --text the output file, '-' for stdout.")
+              help="Prefix of <output>.ids.npy and <output>.offsets.npy; with --text or --output_type subword the "
+                   "output file, '-' for stdout.")
 @click.option("--text", is_flag=True, help="Write the ids as text, as `encode --output_type id` does.")
+@click.option("--output_type", type=click.Choice(["id", "subword"]), default="id", show_default=True,
+              help="'subword' writes the pieces as text, as `encode --output_type subword` does (with or without --text).")
 @click.option("--bos", is_flag=True, help="Add tab 'begin of sentence'.")
 @click.option("--eos", is_flag=True, help="Add tab 'end of sentence'.")
 @click.option("--reverse", is_flag=True, help="Reverse output sequence of tokens.")
 @click.option("--dropout_prob", type=click.FLOAT, default=0, show_default=True,
               help="BPE-dropout probability (the probability of a merge being dropped)")
-def encode_file(model, input_, output, text, bos, eos, reverse, dropout_prob):
+def encode_file(model, input_, output, text, output_type, bos, eos, reverse, dropout_prob):
     """Encode a text file of any size on the GPU, line by line."""
     src = sys.stdin.buffer if input_ == "-" else input_
-    r = BPE(model).encode_file(src, output, bos=bos, eos=eos, reverse=reverse, dropout_prob=dropout_prob, text=text)
+    ot = OutputType.SUBWORD if output_type == "subword" else OutputType.ID
+    r = BPE(model).encode_file(src, output, bos=bos, eos=eos, reverse=reverse, dropout_prob=dropout_prob, text=text,
+                               output_type=ot)
     click.echo("encode_file: %d lines, %d ids, %d bytes" % (r["lines"], r["ids"], r["bytes"]), err=True)
 
 
