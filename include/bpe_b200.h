@@ -218,6 +218,15 @@ class BaseEncoder {
                               uint64_t width, bool with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
                               const uint64_t **d_spans, uint32_t *out_width, bool bos = false, bool eos = false,
                               bool reverse = false, double dropout_prob = 0, int64_t pad_id = kModelPad) const;
+  // encode_packed as overlapping windows of width ids with `stride` content ids of overlap, instead of truncated rows
+  // (yttm_enc_run_windows_device in yttm_b200.h gives the definition): *n_rows rows, and per row its length, sentence
+  // and start.  DEVICE-resident input; the results point into library-owned memory that stays valid until the next
+  // encode call on this object.  pad_id and dropout as for encode_padded_device.
+  Status encode_windows_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sentences,
+                               uint64_t width, uint64_t stride, bool with_spans, const int32_t **d_ids,
+                               const uint64_t **d_lengths, const uint64_t **d_sentence, const uint64_t **d_start,
+                               const uint64_t **d_spans, uint64_t *n_rows, bool bos = false, bool eos = false,
+                               bool reverse = false, double dropout_prob = 0, int64_t pad_id = kModelPad) const;
   // encode_as_subwords of a packed batch on the GPU, the pieces back to back: piece k = pieces[piece_offsets[k],
   // piece_offsets[k+1]), the pieces of sentence i = [sent_offsets[i], sent_offsets[i+1]).  Status code 2 (nothing
   // written, *n_pieces / *n_bytes = sizes needed) when pieces_cap (piece_offsets holds pieces_cap + 1) or bytes_cap

@@ -261,6 +261,36 @@ int yttm_enc_run_padded_device(yttm_enc *enc, const char *d_bytes, const uint64_
                                uint64_t first_sentence_index, uint64_t width /* 0 = longest */, int32_t pad_id,
                                int with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
                                const uint64_t **d_spans, uint32_t *out_width);
+/* ---- overlapping windows of an encode ---------------------------------------------------------------------------
+ * Same batches, arguments, checks and dropout stream as yttm_enc_run_device; every sentence becomes one or more rows of
+ * a W x width matrix instead of being truncated.  With c_i = the ids yttm_enc_run gives sentence i with
+ * bos = eos = reverse = 0, n_i = |c_i|, L = width, K = L - bos - eos content ids per window, S = stride (the overlap, in
+ * content ids) and D = K - S (the step); K >= 1 and 0 <= S < K:
+ *   sentence i gives w_i = 1 window if n_i <= K, else w_i = 1 + ceil((n_i - K) / D); window k (0 <= k < w_i) has the
+ *   content c_i[k D : min(k D + K, n_i)] (an empty sentence gives one window with empty content);
+ *   the windows are the rows of the matrix, in sentence order, then window order; W = sum_i w_i.  For row r, window k of
+ *   sentence i:
+ *     row_r = [<BOS>]? + content + [<EOS>]?, reversed as a whole with reverse (every window gets its own <BOS> / <EOS>);
+ *     cells [lengths[r], L) hold pad_id;  lengths[r] = len(row_r);  sentence[r] = i (non-decreasing, every sentence
+ *     owns at least one row);  start[r] = k D, the index in c_i of the window's first content id (before reversal);
+ *     spans (with_spans): a content id keeps its yttm_enc_run_spans span, <BOS> gets [offsets[i], offsets[i]), <EOS>
+ *     and pad cells [offsets[i+1], offsets[i+1]); with reverse each (id, span) pair moves as one unit.
+ *   Hence a batch whose sentences all have at most K ids gives yttm_enc_run_padded_device's rows at width L, and the
+ *   first window of every sentence is its padded row.  Cell j of row r is ids[r * width + j], its span
+ *   (spans[2 (r width + j)], spans[2 (r width + j) + 1]).
+ * Dropout draws once per word occurrence, so overlapping windows repeat the same ids; the sentence index of the draws
+ * is first_sentence_index + i as for yttm_enc_run.  Device memory: the packed output is built first (20 bytes per
+ * bound id with spans, 4 without, at n_bytes + n_sent ids), then W x width cells (20 bytes per cell with spans, 4
+ * without) and 24 bytes per row; W x width above 2^40, or rows that do not fit, fail with an error.  DEVICE-resident
+ * input; width >= bos + eos + 1 and below 2^31, stride < width - bos - eos.  *d_ids / *d_lengths / *d_sentence /
+ * *d_start / *d_spans (with_spans, else NULL) point into library-owned memory, complete when the call returns and
+ * valid until the next encode call; *n_rows = W. */
+int yttm_enc_run_windows_device(yttm_enc *enc, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                                uint64_t first_sentence_index, uint64_t width, uint64_t stride, int32_t pad_id,
+                                int with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
+                                const uint64_t **d_sentence, const uint64_t **d_start, const uint64_t **d_spans,
+                                uint64_t *n_rows);
 /* encode_as_subwords (bpe.cpp:1757) of a batch: one piece per id, piece k = pieces[piece_offsets[k],
  * piece_offsets[k+1]) (UTF-8): the recipe of an ordinary id with its leading U+2581 kept, "<BOS>" / "<EOS>", and for
  * <UNK> the characters of its run (its span's bytes without invalid units).  The pieces of sentence i are

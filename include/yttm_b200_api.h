@@ -93,6 +93,14 @@ int yttm_api_encode_padded_device(void *handle, const char *d_bytes, const uint6
                                   uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t width,
                                   int64_t pad_id, int with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
                                   const uint64_t **d_spans, uint32_t *out_width);
+/* encode as overlapping windows (yttm_enc_run_windows_device of yttm_b200.h): *n_rows rows of width ids, stride content
+ * ids of overlap between the windows of a sentence, and per row its length, sentence and start; pad_id as for the padded
+ * rows.  Results are library-owned device memory valid until the next encode call.  0 ok, 1 error. */
+int yttm_api_encode_windows_device(void *handle, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                   uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t width,
+                                   uint64_t stride, int64_t pad_id, int with_spans, const int32_t **d_ids,
+                                   const uint64_t **d_lengths, const uint64_t **d_sentence, const uint64_t **d_start,
+                                   const uint64_t **d_spans, uint64_t *n_rows);
 /* encode(output_type='subword') on the GPU (yttm_enc_run_subwords): the same pieces as yttm_api_encode_subwords, into
  * caller-owned buffers; 0 ok, 1 error, 2 a capacity too small (*n_pieces / *n_bytes = sizes needed) */
 int yttm_api_encode_subwords_into(void *handle, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos,

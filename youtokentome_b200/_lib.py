@@ -70,6 +70,9 @@ def bind(L):
         "yttm_api_encode_padded_into": (i32, [vp, vp, vp, u64, i32, i32, i32, dbl, u64, i64, vp, vp, vp]),
         "yttm_api_encode_padded_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, u64, i64, i32, C.POINTER(vp),
                                                 C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_uint32)]),
+        "yttm_api_encode_windows_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, u64, u64, i64, i32,
+                                                 C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                                 C.POINTER(u64)]),
         "yttm_api_encode_subwords_into": (i32, [vp, vp, vp, u64, i32, i32, i32, dbl, vp, u64, vp, u64, vp, C.POINTER(u64),
                                                 C.POINTER(u64)]),
         "yttm_api_encode_subwords_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, C.POINTER(vp), C.POINTER(vp),
@@ -131,6 +134,9 @@ def bind(L):
         "yttm_enc_run_padded": (i32, [vp, vp, vp, u64, i32, i32, i32, dbl, u64, u64, u64, C.c_int32, vp, vp, vp]),
         "yttm_enc_run_padded_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, u64, u64, u64, C.c_int32, i32,
                                              C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_uint32)]),
+        "yttm_enc_run_windows_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, u64, u64, u64, u64, C.c_int32,
+                                              i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                              C.POINTER(vp), C.POINTER(u64)]),
         "yttm_enc_run_subwords": (i32, [vp, vp, vp, u64, i32, i32, i32, dbl, u64, u64, vp, u64, vp, u64, vp,
                                         C.POINTER(u64), C.POINTER(u64)]),
         "yttm_enc_run_subwords_device": (i32, [vp, vp, vp, u64, u64, i32, i32, i32, dbl, u64, u64, C.POINTER(vp),
@@ -168,7 +174,8 @@ EXPORTED_SYMBOLS_DEVICE_ABI = [
     "yttm_train_dist_word_table", "yttm_train_dist_export_words", "yttm_train_dist_import_words", "yttm_train_run", "yttm_train_dump_pairs",
     "yttm_train_scan_once", "yttm_train_synth_words", "yttm_enc_create", "yttm_enc_destroy", "yttm_enc_run",
     "yttm_enc_run_device", "yttm_enc_run_spans", "yttm_enc_run_spans_device", "yttm_enc_run_subwords",
-    "yttm_enc_run_subwords_device", "yttm_enc_run_padded", "yttm_enc_run_padded_device", "yttm_enc_stream_begin",
+    "yttm_enc_run_subwords_device", "yttm_enc_run_padded", "yttm_enc_run_padded_device", "yttm_enc_run_windows_device",
+    "yttm_enc_stream_begin",
     "yttm_enc_stream_feed", "yttm_enc_stream_end", "yttm_dec_run", "yttm_dec_run_device", "yttm_dec_stream_begin",
     "yttm_dec_stream_feed", "yttm_dec_stream_feed_ids", "yttm_dec_stream_end",
 ]

@@ -848,6 +848,19 @@ Status BaseEncoder::encode_padded_device(const char *d_bytes, const uint64_t *d_
   }, resolve_pad(pad_id, &pad));
 }
 
+Status BaseEncoder::encode_windows_device(const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes, uint64_t n_sent,
+                                          uint64_t width, uint64_t stride, bool with_spans, const int32_t **d_ids,
+                                          const uint64_t **d_lengths, const uint64_t **d_sentence, const uint64_t **d_start,
+                                          const uint64_t **d_spans, uint64_t *n_rows, bool bos, bool eos, bool reverse,
+                                          double dropout_prob, int64_t pad_id) const {
+  int32_t pad = 0;
+  return run_device("encode_windows_device", bos, eos, dropout_prob, n_sent, [&] {
+    return yttm_enc_run_windows_device(enc_, d_bytes, d_offsets, n_bytes, n_sent, bos, eos, reverse, dropout_prob,
+                                       dropout_seed_, sentence_counter_, width, stride, pad, with_spans, d_ids, d_lengths,
+                                       d_sentence, d_start, d_spans, n_rows);
+  }, resolve_pad(pad_id, &pad));
+}
+
 Status BaseEncoder::encode_subwords_into(const char *bytes, const uint64_t *offsets, uint64_t n_sent, uint8_t *pieces,
                                          uint64_t bytes_cap, uint64_t *piece_offsets, uint64_t pieces_cap,
                                          uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes, bool bos, bool eos,

@@ -238,6 +238,19 @@ int yttm_api_encode_padded_device(void *hv, const char *d_bytes, const uint64_t 
                                              d_spans, out_width, bos != 0, eos != 0, reverse != 0, dropout, pad_id));
 }
 
+// Overlapping windows (yttm_enc_run_windows_device): pad_id as for the padded rows
+int yttm_api_encode_windows_device(void *hv, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                   uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t width,
+                                   uint64_t stride, int64_t pad_id, int with_spans, const int32_t **d_ids,
+                                   const uint64_t **d_lengths, const uint64_t **d_sentence, const uint64_t **d_start,
+                                   const uint64_t **d_spans, uint64_t *n_rows) {
+  auto *h = static_cast<Handle *>(hv);
+  std::lock_guard<std::mutex> lock(h->mu);
+  return ret(h, h->enc->encode_windows_device(d_bytes, d_offsets, n_bytes, n_sent, width, stride, with_spans != 0, d_ids,
+                                              d_lengths, d_sentence, d_start, d_spans, n_rows, bos != 0, eos != 0,
+                                              reverse != 0, dropout, pad_id));
+}
+
 int yttm_api_encode_subwords_into(void *hv, const char *bytes, const uint64_t *offsets, uint64_t n_sent, int bos, int eos,
                                   int reverse, double dropout, uint8_t *pieces, uint64_t bytes_cap, uint64_t *piece_offsets,
                                   uint64_t pieces_cap, uint64_t *sent_offsets, uint64_t *n_pieces, uint64_t *n_bytes) {

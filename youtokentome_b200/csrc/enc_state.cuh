@@ -42,9 +42,13 @@ struct yttm_enc {
     ytc::DevBuf swb, swc, rec;             // per-sentence word ranges, per-word records (id count, first ids)
     ytc::DevBuf rel, out_spans;            // spans: per-slot span relative to the word start, (start, end) per id
     ytc::DevBuf sub_len, sub_off, sub_out; // subwords: piece length per id, piece offsets, piece bytes
+    // windows (the packed output above is their source): rows per sentence, row bases, then the rows and per row
+    // its length, sentence and start
+    ytc::DevBuf win_cnt, win_base, win_ids, win_spans, win_len, win_sent, win_start;
     template <class F> void each(F f) {
       ytc::DevBuf *b[] = {&d_bytes, &d_offs, &slots, &ranks, &aux, &wpos, &wsent, &wlen, &lookback, &out_off, &out_ids, &counter, &longw,
-                          &dd_tab, &dd_rep, &dd_list, &swb, &swc, &rec, &rel, &out_spans, &sub_len, &sub_off, &sub_out};
+                          &dd_tab, &dd_rep, &dd_list, &swb, &swc, &rec, &rel, &out_spans, &sub_len, &sub_off, &sub_out,
+                          &win_cnt, &win_base, &win_ids, &win_spans, &win_len, &win_sent, &win_start};
       for (auto *x : b) f(x);
     }
     void release() { each([](ytc::DevBuf *x) { x->release(); }); }

@@ -22,6 +22,9 @@
 // yttm_enc_run_padded* replace it with
 //   emit_padded_kernel          block per tile of 256 sentences, row i of an [n_sent, L] matrix at i L: the tiles need
 //                               nothing from each other (no look-back); a counting form finds L when it is not given
+// yttm_enc_run_windows_device keeps it (without bos / eos / reverse) and cuts its output into overlapping rows:
+//   win_count_kernel / scan     windows per sentence, row bases and the row count (one 8-byte read-back)
+//   win_gather_kernel           block per tile of rows: every cell of an [W, L] matrix from the packed ids and spans
 // On request (yttm_enc_run_spans* / yttm_enc_run_subwords*) the same flow also gives the source span of every id and
 // the subword pieces:
 //   span_words_kernel           one thread per encoded word: the span of each of its ids relative to the word start
@@ -1123,6 +1126,96 @@ __global__ void __launch_bounds__(EMIT_T) emit_padded_kernel(EncArgs a, PadArgs 
   }
 }
 
+// ---- overlapping windows ----------------------------------------------------------------------------------------
+// encode_windows (yttm_enc_run_windows_device in yttm_b200.h gives the definition): the packed ids and spans of
+// emit_ids_kernel with bos = eos = reverse = 0 are cut into rows of width L.  With K = L - bos - eos content ids per
+// window, step D = K - stride and n_i packed ids, sentence i has w_i = 1 window if n_i <= K, else
+// 1 + ceil((n_i - K) / D); window k holds the packed ids [k D, min(k D + K, n_i)).
+//   win_count_kernel   a thread per sentence: w_i; a device scan makes them row bases (and W, read back)
+//   win_gather_kernel  a block per tile of rows: each row's sentence (binary search of the row bases), its lengths /
+//                      sentence / start, then every cell of the tile's rows from the packed ids (and spans), a thread
+//                      per cell, so stores stay coalesced however much the windows overlap
+constexpr int WIN_T = 256;           // threads per gather block
+constexpr uint64_t WIN_CELLS = 4096; // cells per gather tile (at least one row, at most WIN_T rows)
+struct WinArgs {
+  const unsigned long long *pk_off;  // packed id offsets, n_sent + 1
+  const int32_t *pk_ids;
+  const Span64 *pk_spans;            // SPANS only
+  const uint64_t *offs;              // the caller's sentence offsets, n_sent + 1
+  const unsigned long long *row_base;  // first row of each sentence, n_sent
+  uint64_t n_sent, n_rows, width, content, step, rows_per_tile;  // rows W, L, K, D
+  int bos, eos, reverse;
+  int32_t bos_id, eos_id, pad_id;
+  int32_t *ids;                      // n_rows x width
+  Span64 *spans;                     // SPANS only, n_rows x width
+  unsigned long long *lengths, *sentence, *start;  // n_rows each
+};
+
+__global__ void __launch_bounds__(256) win_count_kernel(const unsigned long long *__restrict__ pk_off, uint64_t n_sent,
+                                                        uint64_t K, uint64_t D, unsigned long long *__restrict__ w) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_sent; i += stride) {
+    const uint64_t n = pk_off[i + 1] - pk_off[i];
+    w[i] = n <= K ? 1ull : 1ull + (n - K + D - 1) / D;
+  }
+}
+
+template <bool SPANS>
+__global__ void __launch_bounds__(WIN_T) win_gather_kernel(WinArgs a) {
+  __shared__ unsigned long long s_src[WIN_T];  // packed index of the row's first content id
+  __shared__ unsigned long long s_lo[WIN_T], s_hi[WIN_T];  // offsets[i], offsets[i + 1] of the row's sentence
+  __shared__ uint32_t s_len[WIN_T];
+  const uint32_t tid = threadIdx.x;
+  const uint64_t r0 = (uint64_t)blockIdx.x * a.rows_per_tile;
+  const uint32_t nr = (uint32_t)min(a.rows_per_tile, a.n_rows - r0);
+  const uint32_t be = (a.bos ? 1u : 0u) + (a.eos ? 1u : 0u);
+  if (tid < nr) {
+    const uint64_t r = r0 + tid;
+    uint64_t lo = 0, hi = a.n_sent;  // the last sentence whose first row is at or before r (every sentence has one)
+    while (hi - lo > 1) { const uint64_t mid = (lo + hi) >> 1; if (a.row_base[mid] <= r) lo = mid; else hi = mid; }
+    const uint64_t k = r - a.row_base[lo], st = k * a.step;
+    const uint64_t p0 = a.pk_off[lo], n = a.pk_off[lo + 1] - p0;
+    const uint32_t len = (uint32_t)(min(a.content, n - st) + be);
+    a.lengths[r] = len;
+    a.sentence[r] = lo;
+    a.start[r] = st;
+    s_src[tid] = p0 + st;
+    s_len[tid] = len;
+    s_lo[tid] = a.offs[lo];
+    s_hi[tid] = a.offs[lo + 1];
+  }
+  __syncthreads();
+  // the tile's rows are the cells [r0 L, (r0 + nr) L); thread t takes cells t, t + WIN_T, ... and steps its (row,
+  // column) without a division per cell
+  const uint64_t L = a.width, n_cells = (uint64_t)nr * L, step_r = WIN_T / L, step_c = WIN_T % L;
+  uint64_t row = tid / L, col = tid % L;
+  int32_t *out = a.ids + r0 * L;
+  Span64 *sp = SPANS ? a.spans + r0 * L : nullptr;
+  for (uint64_t x = tid; x < n_cells; x += WIN_T) {
+    const uint32_t len = s_len[row];
+    int32_t id = a.pad_id;
+    unsigned long long slo = s_hi[row], shi = slo;  // pads and <EOS>: [offsets[i + 1], offsets[i + 1])
+    if (col < len) {
+      const uint64_t p = a.reverse ? len - 1 - col : col;  // place in the unreversed row
+      if (a.bos && p == 0) {
+        id = a.bos_id;
+        slo = shi = s_lo[row];
+      } else if (a.eos && p == len - 1) {
+        id = a.eos_id;
+      } else {
+        const uint64_t q = s_src[row] + p - (a.bos ? 1 : 0);
+        id = a.pk_ids[q];
+        if constexpr (SPANS) { const Span64 s = a.pk_spans[q]; slo = s.lo; shi = s.hi; }
+      }
+    }
+    out[x] = id;
+    if constexpr (SPANS) sp[x] = Span64{slo, shi};
+    row += step_r;
+    col += step_c;
+    if (col >= L) { col -= L; row++; }
+  }
+}
+
 // ---- subwords ---------------------------------------------------------------------------------------------------
 // One piece per output id: the model's piece of an ordinary id (recipe UTF-8, leading U+2581 kept) or of <BOS> / <EOS>,
 // and for <UNK> the characters of its run: the valid units of its span, copied from the source bytes.
@@ -1226,12 +1319,69 @@ struct PadReq {
   int32_t pad_id;
 };
 
+// The windowed form of an encode call: enc_device runs with bos = eos = reverse = 0 and cuts its packed ids (and
+// spans) into rows of `width`; bos / eos / reverse here are the rows'.  rows = W, set by enc_windows.
+struct WinReq {
+  uint64_t width, stride;
+  int32_t pad_id;
+  int bos, eos, reverse;
+  uint64_t rows;
+};
+
+// The windows of the packed output enc_device just wrote (e->out_off / out_ids / out_spans, n_sent > 0) into
+// e->win_*: row counts, their scan and one 8-byte read-back for W, then the gather.  Only W x width cells (20 bytes
+// per cell with spans) and 24 bytes per row are reserved; a request that does not fit fails with an error.
+int enc_windows(yttm_enc *enc, yttm_enc::Slot *e, const uint64_t *d_offs, uint64_t n_sent, bool spans, WinReq *win) {
+  yttm_ctx *c = enc->ctx;
+  const uint64_t be = (win->bos ? 1 : 0) + (win->eos ? 1 : 0), L = win->width, K = L - be, D = K - win->stride;
+  YT_CUDA(c, e->win_cnt.reserve((n_sent + 8) * 8));
+  YT_CUDA(c, e->win_base.reserve((n_sent + 8) * 8));
+  auto *cnt = e->win_cnt.as<unsigned long long>(), *base = e->win_base.as<unsigned long long>();
+  auto *d_rows = e->counter.as<unsigned long long>() + 4;  // counter words 0-3 belong to enc_device
+  const unsigned long long *pk_off = e->out_off.as<unsigned long long>();
+  ytc::timer_begin(c, "enc_windows");
+  const uint64_t blocks = std::max<uint64_t>(std::min<uint64_t>((n_sent + 255) / 256, (uint64_t)c->n_sm * 8), 1);
+  win_count_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(pk_off, n_sent, K, D, cnt);
+  c->launches++;
+  if (yttm_device_scan_u64(c, cnt, n_sent, base, d_rows)) return 1;
+  unsigned long long W = 0;
+  YT_CUDA(c, cudaMemcpyAsync(&W, d_rows, 8, cudaMemcpyDeviceToHost, c->stream));
+  YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  const uint64_t cells = W * L;  // W < 2^33 (at most one row per id and per sentence), L < 2^31
+  if (cells > (1ull << 40) || e->win_ids.reserve(cells * 4 + 16) != cudaSuccess ||
+      (spans && e->win_spans.reserve(cells * 16 + 16) != cudaSuccess) || e->win_len.reserve(W * 8 + 16) != cudaSuccess ||
+      e->win_sent.reserve(W * 8 + 16) != cudaSuccess || e->win_start.reserve(W * 8 + 16) != cudaSuccess) {
+    cudaGetLastError();  // the failed allocation is reported here, not by the next call
+    YT_FAIL(c, "encode windows: " + std::to_string(W) + " x " + std::to_string(L) +
+                   " rows do not fit in device memory (split the batch or lower the width)");
+  }
+  WinArgs a;
+  a.pk_off = pk_off; a.pk_ids = e->out_ids.as<int32_t>(); a.pk_spans = spans ? e->out_spans.as<Span64>() : nullptr;
+  a.offs = d_offs; a.row_base = base;
+  a.n_sent = n_sent; a.n_rows = W; a.width = L; a.content = K; a.step = D;
+  a.rows_per_tile = std::min<uint64_t>(std::max<uint64_t>(WIN_CELLS / L, 1), WIN_T);
+  a.bos = win->bos; a.eos = win->eos; a.reverse = win->reverse;
+  a.bos_id = enc->bos; a.eos_id = enc->eos; a.pad_id = win->pad_id;
+  a.ids = e->win_ids.as<int32_t>(); a.spans = spans ? e->win_spans.as<Span64>() : nullptr;
+  a.lengths = e->win_len.as<unsigned long long>(); a.sentence = e->win_sent.as<unsigned long long>();
+  a.start = e->win_start.as<unsigned long long>();
+  const uint64_t tiles = (W + a.rows_per_tile - 1) / a.rows_per_tile;  // < 2^30 (cells <= 2^40)
+  if (spans) win_gather_kernel<true><<<(unsigned)tiles, WIN_T, 0, c->stream>>>(a);
+  else win_gather_kernel<false><<<(unsigned)tiles, WIN_T, 0, c->stream>>>(a);
+  c->launches++;
+  ytc::timer_end(c, "enc_windows");
+  win->rows = W;
+  return 0;
+}
+
 // Encodes one batch on the device.  mode >= ENC_SPANS also writes e->out_spans; ENC_SUBWORDS also the pieces
 // (e->sub_off: out_n + 1 byte offsets, e->sub_out: *out_bytes bytes).  With pad (ENC_IDS / ENC_SPANS) the ids and
-// spans are the n_sent x pad->width rows of emit_padded_kernel and e->out_off holds the row lengths.
+// spans are the n_sent x pad->width rows of emit_padded_kernel and e->out_off holds the row lengths.  With win
+// (ENC_IDS / ENC_SPANS, bos = eos = reverse = 0) the packed output is also cut into the windows of enc_windows.
 int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const uint64_t *d_offs, uint64_t n_bytes,
                uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed, uint64_t first_sentence,
-               uint64_t *out_n, int mode = ENC_IDS, uint64_t *out_bytes = nullptr, PadReq *pad = nullptr) {
+               uint64_t *out_n, int mode = ENC_IDS, uint64_t *out_bytes = nullptr, PadReq *pad = nullptr,
+               WinReq *win = nullptr) {
   yttm_ctx *c = enc->ctx;
   if (n_bytes >= 0xfffffff0ull || n_sent >= 0xfffffff0ull)
     YT_FAIL(c, "encode batch too large: at most 2^32 bytes / sentences per call (split the batch)");
@@ -1412,6 +1562,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
   unsigned long long total = 0;
   YT_CUDA(c, cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, c->stream));
   YT_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (win && enc_windows(enc, e, d_offs, n_sent, mode != ENC_IDS, win)) return 1;
   if (mode == ENC_SUBWORDS && total == 0) {
     YT_CUDA(c, e->sub_off.reserve(16));
     YT_CUDA(c, cudaMemsetAsync(e->sub_off.p, 0, 8, c->stream));
@@ -1767,6 +1918,35 @@ int yttm_enc_run_padded_device(yttm_enc *e, const char *d_bytes, const uint64_t 
   if (d_lengths) *d_lengths = sl.out_off.as<uint64_t>();
   if (d_spans) *d_spans = with_spans ? sl.out_spans.as<uint64_t>() : nullptr;
   if (out_width) *out_width = (uint32_t)pr.width;
+  return 0;
+}
+
+int yttm_enc_run_windows_device(yttm_enc *e, const char *d_bytes, const uint64_t *d_offsets, uint64_t n_bytes,
+                                uint64_t n_sent, int bos, int eos, int reverse, double dropout, uint64_t seed,
+                                uint64_t first_sentence_index, uint64_t width, uint64_t stride, int32_t pad_id,
+                                int with_spans, const int32_t **d_ids, const uint64_t **d_lengths,
+                                const uint64_t **d_sentence, const uint64_t **d_start, const uint64_t **d_spans,
+                                uint64_t *n_rows) {
+  if (n_rows) *n_rows = 0;
+  if (yttm_enc_check(e, "yttm_enc_run_windows_device", bos, eos)) return 1;
+  const uint64_t be = (uint64_t)(bos ? 1 : 0) + (eos ? 1 : 0);
+  if (width < be + 1 || width > 0x7fffffffull)
+    YT_FAIL(e->ctx, "yttm_enc_run_windows_device: width must be at least bos + eos + 1, and below 2^31");
+  if (stride >= width - be)
+    YT_FAIL(e->ctx, "yttm_enc_run_windows_device: stride must be below width - bos - eos");
+  yttm_enc::Slot &sl = e->slot[0];
+  WinReq wr{width, stride, pad_id, bos, eos, reverse, 0};
+  uint64_t n = 0;
+  if (enc_device(e, &sl, (const uint8_t *)d_bytes, d_offsets, n_bytes, n_sent, 0, 0, 0, dropout, seed,
+                 first_sentence_index, &n, with_spans ? ENC_SPANS : ENC_IDS, nullptr, nullptr, &wr) ||
+      publish_device(e->ctx, n_sent, {&sl.win_ids, &sl.win_spans, &sl.win_len, &sl.win_sent, &sl.win_start}, {}))
+    return 1;
+  if (d_ids) *d_ids = sl.win_ids.as<int32_t>();
+  if (d_lengths) *d_lengths = sl.win_len.as<uint64_t>();
+  if (d_sentence) *d_sentence = sl.win_sent.as<uint64_t>();
+  if (d_start) *d_start = sl.win_start.as<uint64_t>();
+  if (d_spans) *d_spans = with_spans ? sl.win_spans.as<uint64_t>() : nullptr;
+  if (n_rows) *n_rows = wr.rows;
   return 0;
 }
 

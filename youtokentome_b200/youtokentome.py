@@ -3,6 +3,7 @@ youtokentome/cpp/yttm.pyx:52-181) over the CUDA library: same class, method name
 meaning, return types and exceptions (ValueError(status.message), TypeError for bad argument
 types).  Additions are additive only: `encode_packed` (zero-marshalling numpy path, optionally with the source byte
 span of every id), `encode_padded` (the same ids as padded, truncated [N, L] rows with their lengths),
+`encode_windows` (the same ids as overlapping [W, L] windows of every sentence, with each row's sentence and start),
 `encode_subwords_packed` (the subword pieces on the GPU), `encode_file` (a file of any size, line by line, to .npy files
 or the CLI's id or subword text), `decode_packed` (the inverse of `encode_packed`, on the GPU), `decode_file` (the inverse of
 `encode_file`: either of its outputs, of any size, back to text on the GPU), `count_words` / `train_from_counts` (a
@@ -38,6 +39,18 @@ def _check_dropout(dropout_prob):  # yttm.pyx:92-93
     if dropout_prob < 0 or dropout_prob > 1:
         raise ValueError("dropout_prob value must be in the range [0, 1]. Current value of dropout_prob = " +
                          str(dropout_prob))
+
+
+def _pad_arg(pad_id):
+    """encode_padded / encode_windows' pad_id as the library takes it (None: the model's, YTTM_PAD_FROM_MODEL)."""
+    if pad_id is None:
+        return -2**63
+    if isinstance(pad_id, bool) or not isinstance(pad_id, (int, np.integer)):
+        raise TypeError("pad_id must be an int or None, not %s" % type(pad_id).__name__)
+    pad = int(pad_id)
+    if not -2**31 <= pad < 2**31:
+        raise ValueError("pad_id must fit in int32. Current value of pad_id = %d" % pad)
+    return pad
 
 
 def _offsets_error(n_ids):  # the library's text for the same error
@@ -414,14 +427,7 @@ class BPE:
             if max_length < 1 or max_length < int(bos) + int(eos) or max_length >= 2**31:
                 raise ValueError("max_length must be at least 1 and at least bos + eos, and below 2^31. Current value "
                                  "of max_length = %d" % max_length)
-        if pad_id is None:
-            pad = -2**63   # YTTM_PAD_FROM_MODEL
-        else:
-            if isinstance(pad_id, bool) or not isinstance(pad_id, (int, np.integer)):
-                raise TypeError("pad_id must be an int or None, not %s" % type(pad_id).__name__)
-            pad = int(pad_id)
-            if not -2**31 <= pad < 2**31:
-                raise ValueError("pad_id must fit in int32. Current value of pad_id = %d" % pad)
+        pad = _pad_arg(pad_id)
         L = _lib.lib()
         flags = (int(bos), int(eos), int(reverse), float(dropout_prob))
         if out == "cuda" or (_is_torch(data) and data.is_cuda) or max_length is None:
@@ -444,6 +450,52 @@ class BPE:
         if rc != 0:
             raise self._err()
         return tuple(bufs)
+
+    def encode_windows(self, data, offsets, max_length, stride=0, pad_id=None, bos=False, eos=False, reverse=False,
+                       dropout_prob=0.0, out="numpy", with_spans=False):
+        """encode_packed as overlapping windows of model input, on the GPU: instead of truncating a sentence, its ids
+        are cut into windows of K = max_length - bos - eos content ids that overlap by `stride` ids (step
+        D = K - stride).  With c_i = the ids encode_packed gives sentence i without bos / eos / reverse, sentence i gives
+        one window if len(c_i) <= K, else 1 + ceil((len(c_i) - K) / D); window k holds c_i[k D : k D + K].  Every
+        window becomes a row [<BOS>]? + content + [<EOS>]?, reversed as a whole with reverse, its cells from len(row)
+        on holding the pad id (the model's <PAD> id unless pad_id is given); rows are in sentence order, then window
+        order (yttm_enc_run_windows_device in yttm_b200.h gives the definition).  Inputs as for encode_packed, staged
+        on the device; dropout draws once per word, as encode_packed does, and advances the dropout_seed counter the
+        same way.  Returns (ids int32 [W, L], lengths int64 [W], sentence int64 [W], start int64 [W]): row r comes from
+        sentence `sentence[r]` and its first content id is c_i[start[r]].  with_spans also returns spans [W, L, 2]
+        (encode_packed's span of every content id, [offsets[i], offsets[i]) for <BOS>, [offsets[i+1], offsets[i+1])
+        for <EOS> and pads), as numpy arrays (spans uint64), CPU torch tensors (out="torch") or CUDA tensors
+        (out="cuda")."""
+        _check_out(out)
+        _check_dropout(dropout_prob)
+        if isinstance(max_length, bool) or not isinstance(max_length, (int, np.integer)):
+            raise TypeError("max_length must be an int, not %s" % type(max_length).__name__)
+        max_length, be = int(max_length), int(bos) + int(eos)
+        if max_length < be + 1 or max_length >= 2**31:
+            raise ValueError("max_length must be at least bos + eos + 1, and below 2^31. Current value of max_length = "
+                             "%d" % max_length)
+        if isinstance(stride, bool) or not isinstance(stride, (int, np.integer)):
+            raise TypeError("stride must be an int, not %s" % type(stride).__name__)
+        stride = int(stride)
+        if not 0 <= stride < max_length - be:
+            raise ValueError("stride must be at least 0 and below max_length - bos - eos = %d. Current value of "
+                             "stride = %d" % (max_length - be, stride))
+        pad = _pad_arg(pad_id)
+        L = _lib.lib()
+        flags = (int(bos), int(eos), int(reverse), float(dropout_prob))
+        p, rows = [C.c_void_p() for _ in range(5)], C.c_uint64(0)
+        call = lambda ptr, d_offs, n_bytes, n: L.yttm_api_encode_windows_device(
+            self._h, ptr, d_offs, n_bytes, n, *flags, max_length, stride, pad, int(with_spans),
+            *[C.byref(x) for x in p], C.byref(rows))
+        if not L.yttm_api_device_context(self._h):   # no CUDA device: the library says so, before anything is staged
+            call(None, None, 0, 0)
+            raise self._err()
+        dev, keep, ptr, n_bytes, d_offs, n = _stage_bytes(data, offsets)
+        res = self._run_device(
+            dev, lambda: call(ptr, d_offs.data_ptr(), n_bytes, n),
+            lambda: [(p[0], "<i4", (rows.value, max_length))] + [(p[i], "<i8", (rows.value,)) for i in (1, 2, 3)] +
+                    ([(p[4], "<i8", (rows.value, max_length, 2))] if with_spans else []))
+        return _outputs(res, out, (4,))
 
     def encode_subwords_packed(self, data, offsets, bos=False, eos=False, reverse=False, dropout_prob=0.0, out="numpy"):
         """encode(output_type=SUBWORD) of a packed batch on the GPU (inputs as for encode_packed).  Returns
