@@ -11,7 +11,7 @@
 //     dedup_words_kernel        elects one representative occurrence per distinct word (16-byte vector loads)
 //     encode_rep_words_kernel   one thread per representative: UTF-8 decode -> char ids (unknown runs collapse to
 //                               one pseudo token, bpe.cpp:1513-1533) -> min-rank merge loop, leftmost first
-//                               (MergeEvent2::operator< bpe.cpp:1475-1478)
+//                               (MergeEvent2::operator< bpe.cpp:1475-1478), in shared memory for most words
 //     encode_long_words_kernel  one block per representative of more than LONG_W slots
 //   dropout > 0 (every occurrence draws for itself):
 //     encode_words_kernel       one thread per occurrence, the same merge loop with BPE-dropout (DropoutQueue
@@ -622,8 +622,10 @@ __device__ __forceinline__ uint32_t dd_eq16(Chunk16 c, uint32_t v4) {
 __device__ __forceinline__ uint64_t dd_rotl(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
 
 // (10 blocks of 128 threads per SM: latency-bound, so occupancy is what hides the chain of loads)
+// A length the finder did not know is written back (each work item owns its entry), so encode_rep_words_kernel never
+// scans for a word's end.
 __global__ void __launch_bounds__(128, 10) dedup_words_kernel(EncArgs a, uint64_t n_words, DedupArgs d,
-                                                              const uint16_t *__restrict__ word_len) {
+                                                              uint16_t *__restrict__ word_len) {
   const unsigned lane = threadIdx.x & 31;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t o0 = a.offs[0];
@@ -663,6 +665,7 @@ __global__ void __launch_bounds__(128, 10) dedup_words_kernel(EncArgs a, uint64_
           if (m) { end = q + __ffs((int)m) - 1; break; }
         }
         len = (uint32_t)(end - p0);
+        if (len < WORD_LEN_ESC) word_len[w] = (uint16_t)len;
       }
       // bytes 16 k .. of the word (n of them)
       auto own = [&](uint32_t k, uint32_t n) {
@@ -721,28 +724,70 @@ __global__ void __launch_bounds__(128, 10) dedup_words_kernel(EncArgs a, uint64_
   }
 }
 
-__global__ void __launch_bounds__(128) encode_rep_words_kernel(EncArgs a, DedupArgs d, LongList ll) {
+// Representatives, dropout = 0: one thread per word.  A word with at most SHARED_W tokens before merging (its "▁" and
+// one per valid unit; a word of at most SHARED_B bytes counts the bytes that are not continuation bytes, an upper bound
+// of its units) is merged in the thread's SHARED_W slots of shared memory; others in thread-private local arrays (up
+// to LOCAL_W slots) or in place in global memory.  Every distinct word of the bench batch takes the shared-memory
+// path.  Local arrays for all of them (320 B per thread) do not fit in L1 at the occupancy this kernel runs at, so
+// their traffic went to L2; a 16-lane group per word with the tokens in registers issues many more instructions per
+// word than a thread does (DESIGN.md §7.1).  The word's length comes from the finder or the dedup.  A word of at most
+// SHARED_B bytes is first copied with aligned 16-byte loads into the thread's rank slots, where encode_word walks it:
+// its bytes are all read before the first rank is written, and the walk costs no load from global memory per byte.
+constexpr uint32_t SHARED_W = 17;  // slots per thread (an odd stride: the lanes of a warp never share a bank)
+constexpr uint32_t SHARED_B = 64;  // bytes a word may have to be staged and counted for the shared-memory path
+static_assert(SHARED_B <= 4 * SHARED_W, "a staged word fits in the thread's rank slots");
+__global__ void __launch_bounds__(128) encode_rep_words_kernel(EncArgs a, DedupArgs d, LongList ll,
+                                                               const uint16_t *__restrict__ word_len) {
   constexpr uint32_t LOCAL_W = 40;
+  __shared__ int32_t s_t[128 * SHARED_W];
+  __shared__ uint32_t s_r[128 * SHARED_W];
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t o0 = a.offs[0];
+  const int64_t n_total = (int64_t)(a.offs[a.n_sent] - o0);
+  const int64_t mis = (int64_t)(reinterpret_cast<uintptr_t>(a.bytes) & 15u);
   const RuleTab rt = a.rt;
   auto rank = [&](uint32_t x, uint32_t y, uint32_t *z) { return rule_rank(rt, x, y, z); };
+  int32_t *const st = s_t + threadIdx.x * SHARED_W;
+  uint32_t *const sr = s_r + threadIdx.x * SHARED_W;
   const unsigned long long n_list = *d.n_list;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_list; i += stride) {
     const uint32_t w = d.list[i];
     const uint64_t p0 = a.word_pos[w], s = a.word_sent[w];
+    const uint32_t len = word_len[w];
     const uint64_t lo = a.offs[s] - o0, hi = a.offs[s + 1] - o0;
     const uint64_t slot0 = p0 + 3 * s + 1;
     int32_t *t = a.slots + slot0;  // k+1 private slots
-    uint64_t q = p0;
+    uint64_t q = p0 + len;
     uint32_t l;
-    while (q < hi && !space_at(a.bytes, q, hi, &l)) q++;
+    if (len == WORD_LEN_ESC)  // 64 KB or more
+      for (q = p0; q < hi && !space_at(a.bytes, q, hi, &l);) q++;
     uint32_t owned = (uint32_t)(q - p0) + 1, n;
     if (owned > LONG_W) {  // a whole block will take it (encode_long_words_kernel writes its record)
       const unsigned long long k = atomicAdd(ll.n, 1ull);
       if (k < ll.cap) { ll.pos[k] = (uint32_t)p0; ll.sent[k] = (uint32_t)s; ll.end[k] = (uint32_t)q; ll.item[k] = w; continue; }
     }
-    if (owned <= LOCAL_W) {
+    uint32_t units = owned - 1;  // at most one per byte
+    const bool staged = owned <= SHARED_B + 1;
+    if (staged) {
+      const uint32_t o = (uint32_t)((p0 + mis) & 15);
+      Chunk16 c0 = dd_chunk(a.bytes, (int64_t)p0 - o, n_total);
+      for (uint32_t k = 0; 16 * k < len; k++) {
+        const Chunk16 c1 = o + len > 16 * (k + 1) ? dd_chunk(a.bytes, (int64_t)p0 - o + 16 * (k + 1), n_total) : Chunk16{0, 0};
+        const Chunk16 x = dd_shift(c0, c1, o, min(16u, len - 16 * k));
+        sr[4 * k] = (uint32_t)x.lo; sr[4 * k + 1] = (uint32_t)(x.lo >> 32);
+        sr[4 * k + 2] = (uint32_t)x.hi; sr[4 * k + 3] = (uint32_t)(x.hi >> 32);
+        c0 = c1;
+      }
+      if (owned > SHARED_W) {
+        units = 0;
+        for (uint32_t k = 0; k < len; k++) units += is_cont(reinterpret_cast<const uint8_t *>(sr)[k]) ? 0u : 1u;
+      }
+    }
+    if (staged && units + 1 <= SHARED_W) {  // the word is bytes [0, len) of the staged copy
+      n = encode_word(reinterpret_cast<const uint8_t *>(sr), 0, 0, len, a.cp2id, a.space_id, rank, nullptr, 0, a.seed,
+                      a.first_sentence + s, st, sr, nullptr, &owned);
+      for (uint32_t k = 0; k < n; k++) t[k] = ((uint32_t)st[k] & UNK_FLAG) ? a.unk_id : st[k];
+    } else if (owned <= LOCAL_W) {
       int32_t lt[LOCAL_W];
       uint32_t lr[LOCAL_W];
       n = encode_word(a.bytes, p0, lo, hi, a.cp2id, a.space_id, rank, nullptr, 0, a.seed, a.first_sentence + s, lt, lr,
@@ -1482,7 +1527,7 @@ int enc_device(yttm_enc *enc, yttm_enc::Slot *e, const uint8_t *d_bytes, const u
       ytc::timer_end(c, "enc_dedup");
       c->launches++;
       ytc::timer_begin(c, "enc_rep");
-      encode_rep_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, d, ll);
+      encode_rep_words_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(a, d, ll, word_len);
       c->launches++;
       // no host round trip: the blocks read the list length themselves
       encode_long_words_kernel<<<(unsigned)c->n_sm, LONG_T, 0, c->stream>>>(a, ll);
